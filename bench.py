@@ -2,7 +2,7 @@
 """bench.py — SVG tokens/sec of the im2svg hot path (BASELINE.json metric), one JSON line on rank 0.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
-                    [--max-new-tokens 4096] [--batch-per-gpu 1] [--no-cpu-baseline]
+                    [--max-new-tokens 4096] [--batch-per-gpu 1] [--no-cpu-baseline] [--dump-outputs DIR]
 
 A "step" is one full `generate_im2svg` pass over one batch of synthetic 224x224 images with
 random-init StarVector-1B weights: ViT -> adapter -> decoder prefill -> `max_new_tokens` greedy
@@ -11,6 +11,8 @@ decode steps (EOS/stop disabled so the length is deterministic, SURVEY.md §8d).
   e2e   : same through the host-buffer entry point (pinned host image -> H2D -> ... -> D2H ids)
   roofline : decode step vs HBM (algorithmic bytes = W + kv*L per step, SURVEY.md §8d)
   cpu_baseline : the CPU oracle (HF generate on the host cores) on a bounded sample, rank 0, N=1
+`--dump-outputs DIR` writes what the last timed step returned (the generated ids, as float32) to DIR/ids.npy; the
+weights, images and prompt are seeded, so two builds run with the same arguments can be compared output for output.
 `--impl reference` times that CPU path as the reference arm (the reference is pure Python and has
 no GPU-independent build; its own decoder is the installed `transformers` class).
 """
@@ -41,7 +43,7 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler:
@@ -293,6 +295,7 @@ def measure(model: str, B: int, n_new: int, steps: int, warmup: int, world: int,
     launches = eng.launch_count() - launches0
     digests = [ids_digest(x) for x in passes]                 # after the timed region: what did the timed passes produce?
     first_ids = passes[0].detach().cpu()
+    last_ids = passes[-1].detach().cpu()
     del passes
 
     def prefill_only():
@@ -323,7 +326,7 @@ def measure(model: str, B: int, n_new: int, steps: int, warmup: int, world: int,
     return {
         "dims": d, "gb": gb, "t0": t0, "value": value, "e2e_value": e2e_value, "ms_per_step": ms_per_step, "prefill_ms_per_image": pf_ms / 5 / B,
         "step_ms": step_ms, "launches": int(launches), "engine": desc, "clocks": clocks.summary(), "achieved": achieved, "peak": peak,
-        "peak_src": peak_src, "bytes_per_step": int(bytes_per_step), "first_ids": first_ids,
+        "peak_src": peak_src, "bytes_per_step": int(bytes_per_step), "first_ids": first_ids, "last_ids": last_ids,
         "ids": {"sha256_16_per_pass": digests, "host_path": digests_host,
                 "identical_across_passes_and_paths": same if not sampling else None},
     }
@@ -378,6 +381,7 @@ def main():
     ap.add_argument("--model", default="1b", choices=["1b", "8b"],
                     help="1b = StarVector-1B (headline, configs[1]); 8b = StarVector-8B family dims (SigLIP + StarCoder2)")
     ap.add_argument("--sampling", action="store_true", help="temperature 0.8 / top_p 0.9 sampling instead of greedy (BASELINE configs[4])")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the ids the last timed step returned to DIR/ids.npy (float32)")
     args = ap.parse_args()
 
     if args.impl == "reference":
@@ -410,7 +414,7 @@ def main():
         "ms_per_step": m["ms_per_step"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
         "data": f"synthetic (random-init StarVector-{args.model.upper()} weights, seeded noise images)",
         "config": {"workload": workload.format(b=B, n=n_new), "global_batch": m["gb"], "parallelism": f"batch-shard x{world}",
-                   "l2": f"no flush needed: {d.decoder_weight_bytes() / 1e9:.2f} GB of weights stream per decode step (>> 126 MB L2)",
+                   "l2": f"no flush needed: {d.decoder_weight_bytes() / 1e9:.2f} GB of weights stream per decode step (>> 50 MB L2)",
                    "prompt_len": len(PROMPT_IDS), "prefix_len": m["t0"]},
         "prefill_ms_per_image": m["prefill_ms_per_image"],
         "decode_ms_per_token_step": m["step_ms"],
@@ -421,17 +425,16 @@ def main():
         "engine": m["engine"],
         "clocks": m["clocks"],
         "roofline": {"bound": "hbm", "achieved": m["achieved"], "peak": m["peak"], "unit": "GB/s", "frac": m["achieved"] / m["peak"],
-                     "traffic": None, "traffic_note": "not measured in this run (ncu captures: profiles/r02_*)",
+                     "traffic": None, "traffic_note": "not measured",
                      "peak_source": m["peak_src"], "kernel": "decode step (" + m["engine"].split(" ")[0] + ")",
                      "algorithmic_bytes_per_step": m["bytes_per_step"]},
         "ids": m["ids"],
     }
-    tpath = os.path.join(ROOT, "profiles", "r02_decode_step_traffic.json")
-    if os.path.exists(tpath) and B == 1 and args.model == "1b":
-        with open(tpath) as f:
-            tj = json.load(f)
-        line["roofline"]["traffic"] = int(tj["dram_bytes_read"] + tj["dram_bytes_write"])
-        line["roofline"]["traffic_note"] = f"static: ncu dram__bytes of one decode step from profiles/r02_decode_step_traffic.json ({tj.get('how', '')}), not re-measured in this run"
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "ids.npy"), m["last_ids"].numpy().astype(np.float32))
 
     if not args.no_extras and args.model == "1b" and not args.sampling and B == 1:
         # the other GPU workloads BASELINE.json names, as per-GPU slices (same timing rules, shorter passes)

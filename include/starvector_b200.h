@@ -1,5 +1,5 @@
 /*
- * starvector_b200 — C-ABI of the B200-native im2svg generation engine.
+ * starvector_b200 — C-ABI of the H100-native im2svg generation engine.
  *
  * The reference (joanrod/star-vector) has no FFI: its boundary for this path is the Python
  * method surface `StarVectorForCausalLM.generate_im2svg` / `.model.svg_transformer
@@ -13,7 +13,7 @@
  * a `cudaStream_t` passed as `void*` (NULL = legacy default stream); return 0 on success,
  * <0 on error with the message available from `sv_last_error`; no exceptions cross the
  * ABI; an engine is not re-entrant (the caller serialises; the Python shim holds a lock).
- * There is no CPU fallback: every call fails with SV_ERR_CUDA if no sm_100 device is usable.
+ * There is no CPU fallback: every call fails with SV_ERR_CUDA if no sm_90 (H100) device is usable.
  */
 #ifndef STARVECTOR_B200_H
 #define STARVECTOR_B200_H

@@ -16,7 +16,7 @@ What the oracle is: a CPU restatement of the reference's ``generate_im2svg`` pat
 
 Parity pinning: the reference has NO tests/golden vectors for this path (SURVEY.md §4,
 §8c).  The restatement is pinned instead against outputs of the reference's own modules
-run in the authoring container (`oracle/make_golden.py` imports
-``/root/reference/starvector/...`` and writes ``tests/golden/*.pt``); see
+(`oracle/make_golden.py` imports ``starvector/...`` from a checkout of the reference and
+writes ``tests/golden/*.pt``); see
 ``tests/test_oracle_golden.py``.
 """

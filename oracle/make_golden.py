@@ -1,7 +1,7 @@
 """Generate tests/golden/*.pt by running the REFERENCE's own modules in this container.
 
-Run from the repo root (authoring container only; needs /root/reference):
-    python -m oracle.make_golden
+Run from the repo root with a checkout of the reference:
+    STARVECTOR_REF=<path to joanrod/star-vector> python -m oracle.make_golden
 
 What is reference code here: ``VisionTransformer`` / ``LayerNorm``
 (starvector/model/image_encoder/clip_model.py) and ``Adapter``

@@ -23,7 +23,7 @@ def main():
         a = P.synthetic_image(*hwc, seed=seed)
         ref = P.reference_transform(a, 224, alpha)
         cases.append({"hwc": hwc, "seed": seed, "alpha": alpha, "image": torch.from_numpy(a),
-                      "resized_u8": torch.from_numpy(P.reference_resized_u8(a, 224, alpha)),      # right after Image.resize
+                      "resized_u8_sha256": P.tensor_sha256(torch.from_numpy(P.reference_resized_u8(a, 224, alpha))),   # after Image.resize
                       "sha256_f32": P.tensor_sha256(ref), "sha256_bf16": P.tensor_sha256(ref.to(torch.bfloat16))})
     siglip = []
     for hwc, seed in [((50, 70, 4), 7), ((400, 300, 3), 8)]:

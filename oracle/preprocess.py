@@ -13,7 +13,7 @@ Two checkers for the same function, `uint8 HWC image -> float [3,S,S]`:
    are not installed, so it cannot be imported).
 
 2. `restated_transform(arr, ...)`: a numpy restatement of what those library calls compute, in the integer arithmetic
-   of Pillow 12.2 (third-party dependency, absent from /root/reference; algorithm restated from its published source:
+   of Pillow 12.2 (third-party dependency, not part of the reference; algorithm restated from its published source:
    `src/libImaging/Paste.c` `paste_mask_L` / `ImagingUtils.h` `MULDIV255`, `src/libImaging/Resample.c`
    `precompute_coeffs` / `normalize_coeffs_8bpc` / `ImagingResampleHorizontal_8bpc` / `ImagingResampleVertical_8bpc`,
    `bicubic_filter`).  This is the specification the CUDA kernels follow; it is pinned bit-for-bit to (1) in

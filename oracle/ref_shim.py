@@ -1,6 +1,6 @@
-"""Import the reference's own in-tree modules (authoring container only).
+"""Import the reference's own in-tree modules from a checkout of joanrod/star-vector named by $STARVECTOR_REF.
 
-`/root/reference` does not exist on the GPU box; callers must check `available()` first.
+Only `oracle/make_golden.py` needs it; callers must check `available()` first.
 Only the fairscale import (used for grad-checkpointing, clip_model.py:10) needs a shim
 (SURVEY.md §8c).  Nothing here copies reference code: it imports it in place.
 """
@@ -10,17 +10,17 @@ import os
 import sys
 import types
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("STARVECTOR_REF", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REF_ROOT, "starvector"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "starvector"))
 
 
 def load():
     """Returns (VisionTransformer, LayerNorm, Adapter) classes of the reference."""
     if not available():
-        raise RuntimeError("/root/reference is not mounted")
+        raise RuntimeError("set STARVECTOR_REF to a checkout of joanrod/star-vector")
     for n in ("fairscale", "fairscale.nn", "fairscale.nn.checkpoint",
               "fairscale.nn.checkpoint.checkpoint_activations"):
         sys.modules.setdefault(n, types.ModuleType(n))

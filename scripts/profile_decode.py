@@ -1,4 +1,4 @@
-"""Short 1B run for ncu: encode + prefill + a few decode steps (see profiles/README.md for the commands)."""
+"""Short 1B run for a profiler: encode + prefill + a few decode steps."""
 import argparse
 import os
 import sys

@@ -1,4 +1,4 @@
-"""Build `libstarvector_b200.so` in-tree with nvcc for sm_100a (no torch extension, no JIT cache).
+"""Build `libstarvector_b200.so` in-tree with nvcc for sm_90a (no torch extension, no JIT cache).
 
     python -m starvector_b200.build            # incremental
     python -m starvector_b200.build --force
@@ -19,10 +19,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libstarvector_b200.so")
-SOURCES = ["sv_kernels_basic.cu", "sv_gemm_rowgroup.cu", "sv_gemm_tc05.cu", "sv_attention.cu", "sv_decode_fused.cu", "sv_decode_mega.cu", "sv_decode_flow.cu", "sv_beam.cu", "sv_preprocess.cu", "sv_engine.cu"]
+SOURCES = ["sv_kernels_basic.cu", "sv_gemm_rowgroup.cu", "sv_gemm_wgmma.cu", "sv_attention.cu", "sv_decode_fused.cu", "sv_decode_mega.cu", "sv_decode_flow.cu", "sv_beam.cu", "sv_preprocess.cu", "sv_engine.cu"]
 HEADERS = ["sv_common.cuh", "sv_kernels.h", "sv_ring.cuh", "sv_select.cuh", "sv_beam_core.h", "sv_preprocess_core.h", os.path.join("..", "..", "include", "starvector_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr", "-Xcompiler", "-ffp-contract=off",
 ]
 
@@ -75,7 +75,7 @@ def build(force: bool = False, verbose: bool = False, variant: str = "") -> str:
         list(ex.map(run, jobs))
     objs = [os.path.join(OBJ, s.replace(".cu", ".o")) for s in SOURCES]
     if force or jobs or _stale(LIB, objs):
-        run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs])
+        run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs])
     return LIB
 
 

@@ -1,4 +1,4 @@
-"""Model/configuration records for the B200 im2svg engine.
+"""Model/configuration records for the H100 im2svg engine.
 
 `StarVectorConfig` mirrors the field names and defaults of the reference's
 ``StarVectorConfig`` (reference: starvector/model/starvector_arch.py:96-131) so a

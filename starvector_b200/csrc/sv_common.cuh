@@ -1,11 +1,11 @@
-// Shared device helpers for the starvector_b200 kernels (sm_100a only).
+// Shared device helpers for the starvector_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "starvector_b200 kernels are written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "starvector_b200 kernels are written for sm_90a (H100) only"
 #endif
 
 typedef __nv_bfloat16 bf16;
@@ -66,7 +66,7 @@ SV_DEVINL float quad_max(float v) {
   return v;
 }
 
-// ---- legacy-path tensor core MMA (bandwidth-bound small-M work only; big GEMMs use tcgen05)
+// ---- legacy-path tensor core MMA (bandwidth-bound small-M work only; big GEMMs use wgmma)
 // D[16x8] += A[16x16] * B[16x8], bf16 in, fp32 accumulate.  Fragment layout (PTX ISA, g = lane>>2,
 // t = lane&3):  a0:(g, 2t..) a1:(g+8, 2t..) a2:(g, 2t+8..) a3:(g+8, 2t+8..);  b0:(k=2t.., n=g)
 // b1:(k=2t+8.., n=g);  c0,c1:(g, 2t..2t+1)  c2,c3:(g+8, 2t..2t+1).

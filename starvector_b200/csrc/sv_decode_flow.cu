@@ -103,9 +103,9 @@ SV_DEVINL unsigned long long tag32(uint32_t gp) { return (unsigned long long)(gp
 SV_DEVINL unsigned long long fword(float v, unsigned long long T) { return T | (unsigned long long)__float_as_uint(v); }
 
 // Layout of a flagged bf16 vector [B][n]: the 8 words of one MMA fragment (32 bytes = one L2 sector) are contiguous,
-// consecutive fragments are FRAG_STRIDE words (256 bytes) apart.  All 148 CTAs poll the same vector at the same moment: packed
-// densely (8 KB for n = 2048) those reads hit 32 L2 slices and one hop took 4.5K cycles; one fragment per 256-byte chunk (the
-// L2 slice hash works on address bits >= 8) spreads them over the whole L2: 3.1K cycles (scripts/hop_latency.cu).
+// consecutive fragments are FRAG_STRIDE words (256 bytes) apart.  All CTAs (one per SM) poll the same vector at the same moment:
+// packed densely (8 KB for n = 2048) those reads hit a few L2 slices; one fragment per 256-byte chunk (the L2 slice hash works
+// on address bits >= 8) spreads them over the whole L2.
 constexpr int FRAG_STRIDE = 64;
 SV_DEVINL int64_t ll_words(int n) { return (int64_t)(n >> 3) * FRAG_STRIDE; }                       // words per image row
 SV_DEVINL int64_t ll_off(int i) { return (int64_t)(i >> 3) * FRAG_STRIDE + (i & 7); }              // word i of a row
@@ -177,7 +177,7 @@ SV_DEVINL void produce_ln(LnRing& lr, const bf16* ln_w, const bf16* ln_b, int N,
 // X: flagged [B][K] carrying tag EX.  res (optional): flagged [B][N], tag ER.  EPI_LL: Y flagged [B][N], tag EY.
 // EPI_LMHEAD: plain bf16 logits + one flagged argmax partial per (tile, image).
 // ---- waiting for a flagged vector without flooding L2.  While a CTA waits for a phase's input, 256 threads re-issuing their
-// polls back to back put ~1 sector request per clock and CTA on L2 -- with most of the 148 CTAs waiting (e.g. for the one or
+// polls back to back put ~1 sector request per clock and CTA on L2 -- with most of the CTAs waiting (e.g. for the one or
 // two CTAs that run the attention) that alone saturates L2 and slows exactly the CTAs everybody is waiting for.  So one warp
 // watches 32 fragments spread over the vector, sleeping between looks; only when those carry the tag does every thread poll
 // its own share (which then mostly succeeds at once).
@@ -907,7 +907,7 @@ SV_DEVINL PhaseW phase_weights(const FlowArgs& a, const Layer* layers, int q) {
   return w;
 }
 
-// L2 prefetch that works (scripts/l2_prefetch_test.cu): one 4-byte ld.global.cg with the L2::128B prefetch size per 128-byte
+// L2 prefetch that leaves the region L2-resident: one 4-byte ld.global.cg with the L2::128B prefetch size per 128-byte
 // line.  `rows` pieces of `row_bytes` (a multiple of 128), `row_stride` bytes apart; one warp, 8 independent loads per lane in
 // flight.  The loaded words are folded into `t.acc` only at the NEXT call (by then they have long arrived): that keeps the
 // eight destination registers distinct and alive -- dead outputs would share one register and serialise on its scoreboard --
@@ -1008,8 +1008,7 @@ __global__ void __launch_bounds__(REALLOC ? FLOW_THREADS_REALLOC : FLOW_THREADS,
           stamp_raw(pdbg, pi, ST_PROD + 2 * w.kind);
           if (w.ln_w != nullptr) produce_ln(lnr, w.ln_w, w.ln_b, w.N, w.K, cta, ncta, lane);
           // the CTA's slabs of this matrix are one contiguous run of SLOT_BYTES blocks in the tiled copy (flow_repack_kernel):
-          // ONE bulk copy per slab (a 2 KB copy per weight row topped out at 19.5 B/clk/SM even from L2, one 30 KB copy
-          // reaches 36.8: scripts/ring_stream.cu)
+          // ONE bulk copy per slab (one large copy streams faster than one 2 KB copy per weight row)
           const char* src = reinterpret_cast<const char*>(w.W) + (int64_t)cta * p.tpc * p.nstg * SLOT_BYTES;
           const uint32_t bytes = (uint32_t)(p.R * p.pitch);
           const int nslab = p.ntile * p.nstg;

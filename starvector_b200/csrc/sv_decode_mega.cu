@@ -337,8 +337,8 @@ struct RingGemvArgs {
 
 // The c_attn GEMV's producer warp is idle once its two slabs are on their way: it pulls the K / V^T rows the NEXT kernel (the
 // decode attention) will read into L2 -- one 4-byte ld.global.cg with the L2::128B prefetch size per 128-byte line, the lines
-// dealt round-robin over all CTAs and lanes (scripts/l2_prefetch_test.cu: this, unlike cp.async.bulk.prefetch.L2, leaves the
-// region L2-resident).  The attention's dependent K -> softmax -> V loads then cost L2, not HBM, latency.
+// dealt round-robin over all CTAs and lanes (this, unlike cp.async.bulk.prefetch.L2, is meant to leave the region
+// L2-resident).  The attention's dependent K -> softmax -> V loads then cost L2, not HBM, latency.
 SV_DEVINL void l2_prefetch_kv(const bf16* kc, const bf16* vc, int nkeys, int nbk, int tcap, int cta, int ncta, int lane) {
   if (nkeys <= 0) return;
   const int klines = (nkeys * D * 2 + 127) >> 7;                 // per (image, kv head): K rows are contiguous
@@ -454,7 +454,7 @@ bool gemv_ring_supported(int K, bool has_ln) { (void)has_ln; return K >= 32 && K
 // the second slot is deliberately left free: it is where the NEXT kernel's CTA (launched early through PDL) becomes
 // resident and starts filling its ring while this kernel is still computing.
 int gemv_ring_ncta() {
-  int dev = 0, nsm = 148;
+  int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   return nsm;

@@ -374,11 +374,11 @@ bool build_buffers(sv_engine* e) {
 
 int do_linear(sv_engine* e, int impl, const bf16* x, const bf16* w, const bf16* bias, const bf16* res, bf16* y, int M,
               int N, int K, int act, cudaStream_t st) {
-  if (impl == SV_LINEAR_AUTO) impl = (M > 32 && tc05_supported(M, N, K)) ? SV_LINEAR_TCGEN05 : SV_LINEAR_ROWGROUP;
+  if (impl == SV_LINEAR_AUTO) impl = (M > 32 && wgmma_supported(M, N, K)) ? SV_LINEAR_TCGEN05 : SV_LINEAR_ROWGROUP;
   if (impl == SV_LINEAR_TCGEN05) {
-    if (!tc05_supported(M, N, K)) return fail(e, SV_ERR_INVALID, "tcgen05 linear needs N%%8==0, K%%64==0 (M=%d N=%d K=%d)", M, N, K);
-    cudaError_t r = launch_linear_tc05(x, w, bias, res, y, M, N, K, act, st);
-    if (r != cudaSuccess) return fail(e, SV_ERR_CUDA, "tcgen05 linear launch failed: %s", cudaGetErrorString(r));
+    if (!wgmma_supported(M, N, K)) return fail(e, SV_ERR_INVALID, "wgmma linear needs N%%8==0, K%%64==0 (M=%d N=%d K=%d)", M, N, K);
+    cudaError_t r = launch_linear_wgmma(x, w, bias, res, y, M, N, K, act, st);
+    if (r != cudaSuccess) return fail(e, SV_ERR_CUDA, "wgmma linear launch failed: %s", cudaGetErrorString(r));
     return SV_OK;
   }
   if (K % 32 != 0) return fail(e, SV_ERR_INVALID, "rowgroup linear needs K%%32==0 (K=%d)", K);
@@ -625,8 +625,8 @@ int sv_engine_create(const sv_model_desc* desc, int device, sv_engine** out) {
     return fail(nullptr, SV_ERR_CUDA, "no CUDA device %d (%s): this engine has no CPU fallback", device,
                 r == cudaSuccess ? "device count too small" : cudaGetErrorString(r));
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 10)
-    return fail(nullptr, SV_ERR_CUDA, "device %d is sm_%d%d; kernels are built for sm_100a (B200) only", device, prop.major, prop.minor);
+  if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, SV_ERR_CUDA, "device %d is sm_%d%d; kernels are built for sm_90a (H100) only", device, prop.major, prop.minor);
   if (cudaSetDevice(device) != cudaSuccess) return fail(nullptr, SV_ERR_CUDA, "cudaSetDevice(%d) failed", device);
 
   sv_engine* e = new sv_engine();
@@ -687,10 +687,8 @@ int sv_engine_create(const sv_model_desc* desc, int device, sv_engine** out) {
                         nullptr, nullptr, nullptr, nullptr};
     }
     // slab-tiled copies of the decode weights (one bulk copy per ring slot instead of one per weight row): what the dataflow
-    // kernel streams (SV_FLOW=1), and optionally the ring GEMVs of the graph path (SV_TILED=1).  In the streaming
-    // microbenchmark one 30 KB copy per slot beats 16 row copies (7.1 vs 6.1 TB/s, profiles/r02_ring_stream.txt), but inside
-    // the decode step the row-major weights measured 2 % faster (0.932 vs 0.954 ms/token, profiles/r02_summary.md), so the
-    // default keeps ONE copy of the decoder in HBM.
+    // kernel streams (SV_FLOW=1), and optionally the ring GEMVs of the graph path (SV_TILED=1).  The default keeps ONE copy
+    // of the decoder in HBM (row-major) and leaves the tiled copy opt-in.
     const char* tl = getenv("SV_TILED");
     const bool want_tiles = e->use_flow || (tl && !strcmp(tl, "1"));
     if (want_tiles && decode_flow_init() == cudaSuccess && e->fused_decode && decode_flow_ncta() == gemv_ring_ncta()) {

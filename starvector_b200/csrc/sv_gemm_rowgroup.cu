@@ -11,7 +11,7 @@
 //   * split-K partials are reduced across the 8 warps in shared memory in a fixed order
 //     (deterministic), then the reference's bf16 rounding points are applied (sv_common.cuh).
 // For M > 8 the CTA loops over 8-row groups (weights then come from L2): a correctness fallback
-// for shapes the tcgen05 GEMM does not take, never the fast path for large M.
+// for shapes the wgmma GEMM does not take, never the fast path for large M.
 #include "sv_kernels.h"
 
 namespace sv {

@@ -65,11 +65,11 @@ void launch_fill_i32(int32_t* p, int32_t v, int n, cudaStream_t st);
 void launch_linear_rowgroup(const bf16* x, const bf16* w, const bf16* bias, const bf16* res, bf16* y, int M, int N,
                             int K, int act, cudaStream_t st);
 
-// ---- sv_gemm_tc05.cu : same contract on tcgen05 + TMA + TMEM (M >= 1, N % 8 == 0, K % 64 == 0)
-bool tc05_supported(int M, int N, int K);
+// ---- sv_gemm_wgmma.cu : same contract on wgmma + TMA (M >= 1, N % 8 == 0, K % 64 == 0)
+bool wgmma_supported(int M, int N, int K);
 // returns cudaSuccess or the error of tensor-map creation / launch
-cudaError_t launch_linear_tc05(const bf16* x, const bf16* w, const bf16* bias, const bf16* res, bf16* y, int M, int N,
-                               int K, int act, cudaStream_t st);
+cudaError_t launch_linear_wgmma(const bf16* x, const bf16* w, const bf16* bias, const bf16* res, bf16* y, int M, int N,
+                                int K, int act, cudaStream_t st);
 
 // ---- sv_attention.cu
 void launch_attention_vit(const bf16* qkv, const bf16* vt, bf16* out, int batch, int seq, int heads, int seq_pad,

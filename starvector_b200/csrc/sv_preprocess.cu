@@ -294,7 +294,7 @@ int sv_preproc_create(const sv_preproc_desc* desc, int device, sv_preproc** out)
                 r == cudaSuccess ? "index out of range" : cudaGetErrorString(r));
   cudaDeviceProp prop;
   PRE_CK(nullptr, cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(nullptr, SV_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) return fail(nullptr, SV_ERR_CUDA, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
   PRE_CK(nullptr, cudaSetDevice(device));
   sv_preproc* p = new sv_preproc();
   p->device = device;

@@ -142,8 +142,7 @@ SV_DEVINL void produce_phase(Ring& r, const bf16* W, int N, int K, int cta, int 
 }
 
 // ---- the same on the slab-tiled copy of W (flow_repack_kernel in sv_decode_flow.cu): a slab is SLOT_BYTES-aligned and already
-// has the shared-memory row pitch, so ONE bulk copy fills a slot (per-row 2 KB copies top out at ~6.1 TB/s, a 30 KB copy
-// reaches 7.1: profiles/r02_ring_stream.txt).  Rows past N are zero in the copy.
+// has the shared-memory row pitch, so ONE bulk copy fills a slot instead of one 2 KB copy per row.  Rows past N are zero in the copy.
 SV_DEVINL void produce_phase_tiled(Ring& r, const uint8_t* T, int N, int K, int cta, int ncta, int lane) {
   if (lane != 0) return;
   const Plan p = make_plan(N, K, cta, ncta);

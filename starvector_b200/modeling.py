@@ -1,4 +1,4 @@
-"""Drop-in facade: the reference's `StarVectorForCausalLM` surface on top of the B200 engine.
+"""Drop-in facade: the reference's `StarVectorForCausalLM` surface on top of the H100 engine.
 
 Kept surface (SURVEY.md §8b; reference starvector/model/starvector_arch.py:133-193,
 starvector/model/models/starvector_base.py:203-295, starvector_v1.py):

@@ -25,7 +25,7 @@ ENGINE_NAME = "StarVectorB200Validator"
 
 
 class B200GenerateMixin:
-    """The model-facing half of `StarVectorHFSVGValidator` (starvector_hf_validator.py:43-88) on the B200 engine."""
+    """The model-facing half of `StarVectorHFSVGValidator` (starvector_hf_validator.py:43-88) on the H100 engine."""
 
     def init_engine(self, config) -> None:
         """`config`: the harness' omegaconf tree (model.name / model.from_checkpoint / model.torch_dtype / run.device)."""

@@ -16,10 +16,21 @@ from typing import Optional, Sequence
 import torch
 
 
+def _penalised(row: torch.Tensor, seen: set, repetition_penalty: float) -> torch.Tensor:
+    """HF RepetitionPenaltyLogitsProcessor on one fp32 logits row: the scores greedy selection compares."""
+    row = row.clone()
+    if repetition_penalty != 1.0 and seen:
+        idx = torch.tensor(sorted(seen))
+        v = row[idx]
+        row[idx] = torch.where(v < 0, v * repetition_penalty, v / repetition_penalty)
+    return row
+
+
 def check_greedy_ids(got: torch.Tensor, ref_new: torch.Tensor, ref_logits: torch.Tensor, tol: float, teacher_forced,
                      eos_token_id: Optional[int] = None, repetition_penalty: float = 1.0) -> dict:
-    """got / ref_new: [B, n] generated ids (engine / oracle).  ref_logits: [n_ref, B, V] fp32 logits the oracle selected
-    from.  teacher_forced(ids[B, n]) -> [B, n + 1, V] fp32 oracle logits under the engine's history (called at most once).
+    """got / ref_new: [B, n] generated ids (engine / oracle).  ref_logits: [n_ref, B, V] raw fp32 logits of the oracle
+    (before the repetition penalty, which is applied here to the ids generated so far).  teacher_forced(ids[B, n]) ->
+    [B, n + 1, V] fp32 oracle logits under the engine's history (called at most once).
     Returns counters for the caller's own asserts ("flips": tolerated disagreements, "resynced": steps checked by (3))."""
     got = got.cpu().long()
     ref_new = ref_new.cpu().long()
@@ -33,22 +44,18 @@ def check_greedy_ids(got: torch.Tensor, ref_new: torch.Tensor, ref_logits: torch
         first = next((s for s in range(n_cmp) if got[b, s] != ref_new[b, s]), None)
         if first is None:
             continue
-        top2 = ref_logits[first, b].float().topk(2).values
+        seen = set(int(t) for t in got[b, :first].tolist())
+        top2 = _penalised(ref_logits[first, b].float(), seen, repetition_penalty).topk(2).values
         margin = (top2[0] - top2[1]).item()
         assert margin < tol, f"row {b} step {first}: ids differ ({int(got[b, first])} vs {int(ref_new[b, first])}) at oracle margin {margin:.4f}"
         stats["flips"] += 1
         if tf is None:
             tf = teacher_forced(got).float()                       # [B, n + 1, V]
-        seen = set(int(t) for t in got[b, :first].tolist())
         for s in range(first, n):
             tok = int(got[b, s])
             if eos_token_id is not None and s > 0 and int(got[b, s - 1]) == eos_token_id:
                 break                                              # finished row: the rest is padding
-            row = tf[b, s].clone()
-            if repetition_penalty != 1.0 and seen:
-                idx = torch.tensor(sorted(seen))
-                v = row[idx]
-                row[idx] = torch.where(v < 0, v * repetition_penalty, v / repetition_penalty)
+            row = _penalised(tf[b, s], seen, repetition_penalty)
             gap = (row.max() - row[tok]).item()
             assert gap < tol, f"row {b} step {s} (after the flip at {first}): engine token {tok} is {gap:.4f} below the oracle's best for the engine's own history"
             stats["resynced"] += 1

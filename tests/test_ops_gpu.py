@@ -56,7 +56,7 @@ def test_layernorm():
                                    (257, 4096, 1024), (130, 128, 8192), (64, 64, 64)])
 def test_linear_shapes(impl, M, N, K):
     if impl == _lib.SV_LINEAR_TCGEN05 and (N % 8 or K % 64):
-        pytest.skip("shape not taken by the tcgen05 kernel")
+        pytest.skip("shape not taken by the wgmma kernel")
     if impl == _lib.SV_LINEAR_ROWGROUP and M > 300:
         pytest.skip("fallback path: covered at smaller M")
     x, w, b = _bf(M, K, seed=4), _bf(N, K, scale=1 / math.sqrt(K), seed=5), _bf(N, scale=0.1, seed=6)

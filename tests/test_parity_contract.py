@@ -66,3 +66,13 @@ def test_repetition_penalty_is_applied_to_the_resync_logits():
         return out
 
     assert check_greedy_ids(got, ref, rl, 0.05, teacher, repetition_penalty=2.0)["resynced"] == 2
+
+
+def test_repetition_penalty_is_applied_to_the_flip_margin():
+    ref, got = torch.tensor([[1, 2, 3]]), torch.tensor([[1, 5, 3]])
+    rl = _logits([1, 2, 3])
+    rl[1, 0, 1] = 1.5                                   # raw top-1 is token 1, 0.5 above the rest ...
+    rl[1, 0, 5] = 1.0                                   # ... but 1 was generated: 1.5 / 3 = 0.5, so 2 and 5 tie at 1.0
+    assert check_greedy_ids(got, ref, rl, 0.05, _teacher, repetition_penalty=3.0)["flips"] == 1
+    with pytest.raises(AssertionError, match="oracle margin"):
+        check_greedy_ids(got, ref, rl, 0.05, _teacher, repetition_penalty=1.2)   # 1.5 / 1.2 = 1.25: a clear margin
