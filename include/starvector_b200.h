@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define SV_ABI_VERSION 4
+#define SV_ABI_VERSION 5
 #if defined(__GNUC__)
 #define SV_API __attribute__((visibility("default")))
 #else
@@ -157,6 +157,17 @@ SV_API int sv_prefill_embeds(sv_engine* e, const void* inputs_embeds, int32_t ba
 /* One teacher-forced decode step: feed ids int32 [B], append to the KV cache, return fp32 logits
  * [B,V] (optional).  The parity-test hook; also the body the generate loop replays. */
 SV_API int sv_decode_step(sv_engine* e, const int32_t* ids, float* logits, void* stream);
+/* Teacher forcing at prefill speed: after sv_prefill / sv_prefill_embeds / sv_expand_batch / sv_decode_step /
+ * sv_score_tokens, feed ids int32 [batch, n_tokens] (device; batch == the current batch) at cache positions
+ * cur_len .. cur_len+n_tokens-1.  logprobs fp32 [batch, n_tokens] (device): logprobs[b][t] =
+ * log softmax(logits before ids[b][t])[ids[b][t]], where t = 0 uses the logits left resident by the previous call.  The
+ * logits are bf16 (as HF's lm_head output) and the log-softmax is fp32 over them; they are never written to memory.
+ * Leaves the engine as n_tokens sv_decode_step calls would (KV rows appended, cur_len advanced, the last position's bf16
+ * logits resident), and the scored tokens become part of the prefix, so sv_generate, a decode step or another
+ * sv_score_tokens may follow.  Out-of-range ids are clamped to [0, vocab) for both the embedding and the target.
+ * SV_ERR_STATE before a prefill; SV_ERR_INVALID when batch != the current batch, n_tokens < 1 or
+ * cur_len + n_tokens > max_len. */
+SV_API int sv_score_tokens(sv_engine* e, const int32_t* ids, int32_t batch, int32_t n_tokens, float* logprobs, void* stream);
 /* Beam search support (SURVEY.md §8f-1): permute the image rows of the KV cache, row r <- row src_rows[r]
  * (int32 [B] on the device) for the tokens cached so far = HF `_reorder_cache` (vendored modeling_gpt_bigcode.py:1282-1291). */
 SV_API int sv_reorder_cache(sv_engine* e, const int32_t* src_rows, void* stream);
@@ -235,6 +246,14 @@ SV_API int sv_op_linear(int32_t impl, const void* x, const void* w, const void* 
 SV_API int sv_op_attention_vit(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, void* stream);
 /* Causal multi-query attention over packed qkv [B*T, heads*D + 2*D] (D=128) -> out [B*T, heads*D]. */
 SV_API int sv_op_attention_mqa(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, void* stream);
+/* The scoring chunk attention: packed qkv [B*seq, (n_head + 2*n_kv)*D] (D=128) fills a cache with all seq positions;
+ * the queries of positions [q0, seq) attend causally (keys > pos - window when window > 0) -> out [B*(seq-q0), n_head*D]. */
+SV_API int sv_op_attention_chunk(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t q0, int32_t n_head,
+                                 int32_t n_kv, int32_t window, void* stream);
+/* The fused lm_head log-likelihood: logprob fp32 [M] = log_softmax(float(bf16(x[M,K] . w[N,K]^T)))[m, targets[m]],
+ * targets int32 [M] in [0, N) (device); any N, K % 64 == 0. */
+SV_API int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets, float* logprob, int32_t M, int32_t N,
+                            int32_t K, void* stream);
 
 /* ---- image preprocessing (SURVEY.md §8f-2) ------------------------------------------------ */
 /* Replaces `ImageTrainProcessor.__call__` (reference starvector/data/util.py:40-66: RGBA pasted on white, pad to

@@ -16,7 +16,7 @@ SV_OK, SV_ERR_INVALID, SV_ERR_CUDA, SV_ERR_UNSUPPORTED, SV_ERR_STATE = 0, -1, -2
 SV_DTYPE_BF16, SV_DTYPE_F32, SV_DTYPE_F16 = 0, 1, 2
 SV_ACT_NONE, SV_ACT_QUICKGELU, SV_ACT_GELU_TANH, SV_ACT_SILU = 0, 1, 2, 3
 SV_LINEAR_AUTO, SV_LINEAR_ROWGROUP, SV_LINEAR_TCGEN05 = 0, 1, 2
-ABI_VERSION = 4
+ABI_VERSION = 5
 SV_ALPHA_WHITE, SV_ALPHA_DROP = 0, 1
 
 
@@ -71,6 +71,7 @@ SIGNATURES = {
     "sv_prefill": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "sv_prefill_embeds": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "sv_decode_step": (C.c_int, [_P, _P, _P, _P]),
+    "sv_score_tokens": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "sv_reorder_cache": (C.c_int, [_P, _P, _P]),
     "sv_expand_batch": (C.c_int, [_P, _P, C.c_int32, _P]),
     "sv_beam_search": (C.c_int, [_P, C.POINTER(BeamParams), _I, _P, _P, _P]),
@@ -93,6 +94,8 @@ SIGNATURES = {
     "sv_op_linear": (C.c_int, [_I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "sv_op_attention_vit": (C.c_int, [_P, _P, _I, _I, _I, _P]),
     "sv_op_attention_mqa": (C.c_int, [_P, _P, _I, _I, _I, _P]),
+    "sv_op_attention_chunk": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "sv_op_lm_logprob": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
     "sv_preproc_create": (C.c_int, [C.POINTER(PreprocDesc), C.c_int, C.POINTER(_P)]),
     "sv_preproc_destroy": (None, [_P]),
     "sv_preproc_last_error": (C.c_char_p, [_P]),

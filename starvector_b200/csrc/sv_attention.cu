@@ -18,6 +18,7 @@
 #include <algorithm>
 
 #include "sv_kernels.h"
+#include "sv_ring.cuh"
 
 namespace sv {
 
@@ -46,7 +47,14 @@ SV_DEVINL void load_q_frag(uint32_t (&qa)[D / 16][4], const bf16* row_lo, bool o
 // output, row max (log2 domain) and per-lane partial row sums for rows g (index 0) and g+8 (1).
 // HOIST_V: issue the block's V^T loads together with its K loads (one dependent memory round instead of two;
 // costs 64 more live registers, used by the latency-critical single-token decode kernel).
-template <int D, bool CG = false, bool HOIST_V = false>
+// SMEM: kbase / vtbase point into shared memory (the chunk kernel's staged K / V^T tiles).
+template <bool CG, bool SMEM>
+SV_DEVINL uint4 ld16_any(const bf16* p) {
+  if constexpr (SMEM) return mega::lds16(mega::smem_u32(p));
+  else return ld16<CG>(p);
+}
+
+template <int D, bool CG = false, bool HOIST_V = false, bool SMEM = false>
 SV_DEVINL void attn_core(const uint32_t (&qa)[D / 16][4], const bf16* __restrict__ kbase, int64_t k_row_stride,
                          const bf16* __restrict__ vtbase, int64_t vt_dim_stride, int key_begin, int key_end,
                          float scale_log2, float (&acc)[D / 8][4], float (&mrow)[2], float (&lrow)[2], int lane,
@@ -57,7 +65,7 @@ SV_DEVINL void attn_core(const uint32_t (&qa)[D / 16][4], const bf16* __restrict
     uint4 vpre[HOIST_V ? D / 8 : 1];
     if constexpr (HOIST_V) {
 #pragma unroll
-      for (int nd = 0; nd < D / 8; ++nd) vpre[nd] = ld16<CG>(vtbase + (int64_t)(8 * nd + g) * vt_dim_stride + kb + 8 * t);
+      for (int nd = 0; nd < D / 8; ++nd) vpre[nd] = ld16_any<CG, SMEM>(vtbase + (int64_t)(8 * nd + g) * vt_dim_stride + kb + 8 * t);
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -67,7 +75,7 @@ SV_DEVINL void attn_core(const uint32_t (&qa)[D / 16][4], const bf16* __restrict
       const bf16* kp = kbase + (int64_t)key * k_row_stride + 8 * t;
 #pragma unroll
       for (int jj = 0; jj < D / 32; ++jj) {
-        const uint4 w = ld16<CG>(kp + 32 * jj);
+        const uint4 w = ld16_any<CG, SMEM>(kp + 32 * jj);
         mma_bf16_16816(s[j], qa[2 * jj][0], qa[2 * jj][1], qa[2 * jj][2], qa[2 * jj][3], w.x, w.y);
         mma_bf16_16816(s[j], qa[2 * jj + 1][0], qa[2 * jj + 1][1], qa[2 * jj + 1][2], qa[2 * jj + 1][3], w.z, w.w);
       }
@@ -113,7 +121,7 @@ SV_DEVINL void attn_core(const uint32_t (&qa)[D / 16][4], const bf16* __restrict
       acc[nd][0] *= corr0; acc[nd][1] *= corr0; acc[nd][2] *= corr1; acc[nd][3] *= corr1;
       uint4 w;
       if constexpr (HOIST_V) w = vpre[nd];
-      else w = ld16<CG>(vtbase + (int64_t)(8 * nd + g) * vt_dim_stride + kb + 8 * t);
+      else w = ld16_any<CG, SMEM>(vtbase + (int64_t)(8 * nd + g) * vt_dim_stride + kb + 8 * t);
       mma_bf16_16816(acc[nd], pa[0][0], pa[0][1], pa[0][2], pa[0][3], w.x, w.y);
       mma_bf16_16816(acc[nd], pa[1][0], pa[1][1], pa[1][2], pa[1][3], w.z, w.w);
     }
@@ -213,6 +221,110 @@ void launch_attention_heads(const bf16* qkv, int q_cols_total, const bf16* kcach
   attention_heads_kernel<128><<<(tiles + kAttnWarps - 1) / kAttnWarps, kAttnWarps * 32, 0, st>>>(
       qkv, ld, kcache, vtcache, out, batch, seq, n_head, n_kv, tcap, scale_log2, window);
   count_launch();
+}
+
+// ------------------------------------------------------------------------------------------
+// Decoder (scoring chunk): queries at cache positions q0 .. q0+C-1 of one (image, kv head) against keys
+// [max(0, pos + 1 - window), pos] of the cache.  A CTA = 8 warps = 8 consecutive positions (each warp the `group` query
+// heads of its position, as attention_heads_kernel); every 32-key tile of K rows and V^T columns the CTA needs is
+// brought into shared memory ONCE by bulk copies (warp 0, mbarrier completion, 4-deep ring) and read there by all 8 warps
+// (attention_heads_kernel re-reads the whole causal prefix from L2 for every position).
+// Shared K rows are padded to 320 bytes and V^T rows are 64 bytes: the 16-byte fragment loads of a quarter warp
+// (two rows, four 16-byte columns) hit distinct banks.
+constexpr int kChunkWarps = 8, kChunkStages = 4, kChunkKeys = 32;
+constexpr int kChunkKRow = 160;                                       // bf16 per shared K row (256 B + 64 B pad)
+constexpr int kChunkKBytes = kChunkKeys * kChunkKRow * 2, kChunkVBytes = 128 * kChunkKeys * 2;
+constexpr int kChunkStageBytes = kChunkKBytes + kChunkVBytes;
+constexpr int kChunkSmem = kChunkStages * kChunkStageBytes + 8 * kChunkStages + 128;
+
+template <int D>
+__global__ void __launch_bounds__(kChunkWarps * 32) attention_chunk_kernel(
+    const bf16* __restrict__ qkv, int ld, int q_rows_per_b, const bf16* __restrict__ kcache,
+    const bf16* __restrict__ vtcache, bf16* __restrict__ out, int C, int q0, int n_head, int n_kv, int tcap,
+    float scale_log2, int window) {
+  static_assert(D == 128, "the shared tile layout assumes head_dim 128");
+  extern __shared__ uint8_t csm_raw[];
+  uint8_t* csm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(csm_raw) + 127) & ~uintptr_t(127));
+  const uint32_t bars = mega::smem_u32(csm + kChunkStages * kChunkStageBytes);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int kvh = blockIdx.y, b = blockIdx.z, group = n_head / n_kv;
+  const int t_first = blockIdx.x * kChunkWarps, t_last = min(C, t_first + kChunkWarps) - 1;
+  const int tw = t_first + warp, pos = q0 + tw;
+  const bool active = tw < C;
+  const int key_lo = window > 0 ? max(0, pos + 1 - window) : 0;        // HF sliding window: keys in (q - window, q]
+  const int tile0 = (window > 0 ? max(0, q0 + t_first + 1 - window) : 0) / kChunkKeys;
+  const int ntile = (q0 + t_last) / kChunkKeys + 1 - tile0;
+  const int64_t bk = (int64_t)b * n_kv + kvh;
+  const bf16* kc = kcache + bk * tcap * D;
+  const bf16* vc = vtcache + bk * D * tcap;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kChunkStages; ++s) mega::mbar_init(bars + 8u * s, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  auto issue = [&](int i) {                                           // warp 0: tile i -> stage i % kChunkStages
+    const int s = i % kChunkStages, kb = (tile0 + i) * kChunkKeys;
+    const uint32_t sk = mega::smem_u32(csm + s * kChunkStageBytes), sv = sk + kChunkKBytes, bar = bars + 8u * s;
+    if (lane == 0) mega::mbar_expect_tx(bar, kChunkKeys * D * 2 + D * kChunkKeys * 2);
+    __syncwarp();
+    mega::bulk_g2s(sk + lane * kChunkKRow * 2, kc + (int64_t)(kb + lane) * D, D * 2, bar);
+#pragma unroll
+    for (int j = 0; j < D / 32; ++j) {
+      const int dim = lane + 32 * j;
+      mega::bulk_g2s(sv + dim * kChunkKeys * 2, vc + (int64_t)dim * tcap + kb, kChunkKeys * 2, bar);
+    }
+  };
+  if (warp == 0)
+    for (int i = 0; i < min(kChunkStages - 1, ntile); ++i) issue(i);
+
+  uint32_t qa[D / 16][4];
+  {
+    const bf16* qrow = qkv + ((int64_t)b * q_rows_per_b + (active ? tw : 0)) * ld + (int64_t)kvh * group * D;
+    load_q_frag<D>(qa, qrow + (int64_t)g * D, active && g < group, qrow + (int64_t)(g + 8) * D, active && g + 8 < group, t);
+  }
+  float acc[D / 8][4], mrow[2], lrow[2];
+  attn_init<D>(acc, mrow, lrow);
+  for (int i = 0; i < ntile; ++i) {
+    if (warp == 0 && i + kChunkStages - 1 < ntile) issue(i + kChunkStages - 1);   // its stage was released at the end of i - 1
+    const int s = i % kChunkStages, kb = (tile0 + i) * kChunkKeys;
+    mega::mbar_wait(bars + 8u * s, (uint32_t)(i / kChunkStages) & 1u);
+    if (active && kb <= pos && kb + kChunkKeys > key_lo) {
+      const bf16* sk = reinterpret_cast<const bf16*>(csm + s * kChunkStageBytes);
+      const bf16* sv = reinterpret_cast<const bf16*>(csm + s * kChunkStageBytes + kChunkKBytes);
+      // attn_core indexes keys absolutely: shift the tile bases by -kb so key kb is tile row 0
+      attn_core<D, false, false, true>(qa, sk - (int64_t)kb * kChunkKRow, kChunkKRow, sv - kb, kChunkKeys, kb,
+                                       min(pos + 1, kb + kChunkKeys), scale_log2, acc, mrow, lrow, lane, key_lo);
+    }
+    __syncthreads();
+  }
+  if (!active) return;
+  const float inv0 = 1.0f / quad_sum(lrow[0]), inv1 = 1.0f / quad_sum(lrow[1]);
+  bf16* o = out + ((int64_t)b * C + tw) * n_head * D + (int64_t)kvh * group * D;
+#pragma unroll
+  for (int nd = 0; nd < D / 8; ++nd) {
+    if (g < group)
+      *reinterpret_cast<uint32_t*>(o + (int64_t)g * D + 8 * nd + 2 * t) = pack_bf16x2(acc[nd][0] * inv0, acc[nd][1] * inv0);
+    if (g + 8 < group)
+      *reinterpret_cast<uint32_t*>(o + (int64_t)(g + 8) * D + 8 * nd + 2 * t) =
+          pack_bf16x2(acc[nd][2] * inv1, acc[nd][3] * inv1);
+  }
+}
+
+cudaError_t launch_attention_chunk(const bf16* qkv, int q_cols_total, int q_rows_per_b, const bf16* kcache,
+                                   const bf16* vtcache, bf16* out, int batch, int C, int q0, int n_head, int n_kv, int d,
+                                   int tcap, int window, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(attention_chunk_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChunkSmem);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  const float scale_log2 = 1.4426950408889634f / sqrtf((float)d);
+  attention_chunk_kernel<128><<<dim3((C + kChunkWarps - 1) / kChunkWarps, n_kv, batch), kChunkWarps * 32, kChunkSmem, st>>>(
+      qkv, q_cols_total, q_rows_per_b, kcache, vtcache, out, C, q0, n_head, n_kv, tcap, scale_log2, window);
+  count_launch();
+  return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------

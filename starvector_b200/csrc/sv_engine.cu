@@ -27,6 +27,7 @@ namespace {
 constexpr int kMaxPrompt = 64;
 constexpr int kStreamChunk = 1024;   // tokens per row handed to a streaming callback at once
 constexpr int kMaxSplit = 128;
+constexpr int kScoreRows = 4096;     // rows (batch x positions) of one sv_score_tokens chunk: keeps the layer GEMMs tensor-bound
 
 std::string g_create_error;
 
@@ -114,6 +115,12 @@ struct sv_engine {
   int32_t* im2svg_out = nullptr;    //   call, sized for max_batch rows, kept for the engine's lifetime
   int32_t* host_flag = nullptr;     // pinned
   int32_t* host_stream = nullptr;   // pinned staging of streamed tokens [max_batch][kStreamChunk], allocated on first use
+  // sv_score_tokens chunk buffers (kScoreRows rows each), allocated by its first call: an engine that never scores keeps
+  // the footprint it had without them
+  bf16 *s_x = nullptr, *s_ln = nullptr, *s_qkv = nullptr, *s_attn = nullptr, *s_h = nullptr;
+  int32_t* s_tgt = nullptr;
+  float2* s_part = nullptr;
+  float* s_tl = nullptr;
 
   // run state (host mirror)
   int cur_batch = 0, prefix_len = 0, host_cur_len = 0;
@@ -431,7 +438,7 @@ int run_encode(sv_engine* e, const bf16* pixels, int B, cudaStream_t st) {
 int run_prefill(sv_engine* e, const bf16* prefix, int q, const int32_t* prompt_ids, int B, int P, cudaStream_t st) {
   const sv_model_desc& d = e->d;
   const int H = d.hidden, T0 = q + P, M = B * T0, D = d.head_dim;
-  launch_embed_prefix(prefix, prompt_ids, e->wte, e->wpe, e->p_x, B, q, P, H, d.vocab, st);
+  launch_embed_prefix(prefix, prompt_ids, e->wte, e->wpe, e->p_x, B, q, P, H, d.vocab, 0, P, st);
   for (int i = 0; i < d.n_layer; ++i) {
     const DecLayer& L = e->dec[i];
     bf16* kc = e->kcache + e->cache_layer_stride * i;
@@ -439,7 +446,7 @@ int run_prefill(sv_engine* e, const bf16* prefix, int q, const int32_t* prompt_i
     launch_layernorm(e->p_x, L.ln1_w, L.ln1_b, e->p_ln, M, H, d.ln_eps, H, st);
     LIN(e->p_ln, L.attn_w, L.attn_b, nullptr, e->p_qkv, M, e->qkv_cols, H, SV_ACT_NONE, st);
     if (e->v2)   // RoPE on q and k (positions 0..T0-1), modeling_starcoder2.py:167-168
-      launch_rope(e->p_qkv, M, T0, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, nullptr, d.n_positions, st);
+      launch_rope(e->p_qkv, M, T0, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, nullptr, d.n_positions, 0, st);
     launch_kv_scatter(e->p_qkv, kc, vc, B, T0, d.n_head * D, d.n_kv_head, D, e->tcap, 0, st);
     launch_attention_heads(e->p_qkv, e->qkv_cols, kc, vc, e->p_attn, B, T0, d.n_head, d.n_kv_head, D, e->tcap, e->window, st);
     LIN(e->p_attn, L.proj_w, L.proj_b, e->p_x, e->p_x, M, H, H, SV_ACT_NONE, st);
@@ -451,6 +458,54 @@ int run_prefill(sv_engine* e, const bf16* prefix, int q, const int32_t* prompt_i
   launch_gather_rows(e->p_x, e->d_last, B, T0, T0 - 1, H, st);
   launch_layernorm(e->d_last, e->lnf_w, e->lnf_b, e->d_ln, B, H, d.ln_eps, H, st);
   launch_linear_rowgroup(e->d_ln, e->lm_head, nullptr, nullptr, e->logits, B, d.vocab, H, SV_ACT_NONE, st);
+  return SV_OK;
+}
+
+// ---- stage: teacher-forced scoring chunk ------------------------------------------------------
+// Rows [b][t] = ids[b][c0 + t] (row stride n) at cache positions pos0 + t, t < C, through the decoder at prefill shape:
+// KV rows appended, the log-likelihood of ids[b][c0 + t + 1] written to logprobs[b][c0 + t + 1] without materialising
+// the logits.  `last`: also leave the bf16 logits of the final position resident (as run_prefill does).
+// Every GEMM runs on the wgmma kernel whatever M is, and the resident logits come from the same lm_head tiling as the
+// fused log-likelihood, so the log-probs of a sequence do not depend on how it is split over calls or chunks.
+int run_score_chunk(sv_engine* e, const int32_t* ids, int n, int c0, int C, int B, int pos0, float* logprobs, bool last,
+                    cudaStream_t st) {
+  const sv_model_desc& d = e->d;
+  const int H = d.hidden, M = B * C, D = d.head_dim;
+#define SLIN(...)                                           \
+  do {                                                      \
+    int _r = do_linear(e, SV_LINEAR_TCGEN05, __VA_ARGS__);  \
+    if (_r != SV_OK) return _r;                             \
+  } while (0)
+  launch_embed_prefix(nullptr, ids + c0, e->wte, e->wpe, e->s_x, B, 0, C, H, d.vocab, pos0, n, st);
+  for (int i = 0; i < d.n_layer; ++i) {
+    const DecLayer& L = e->dec[i];
+    bf16* kc = e->kcache + e->cache_layer_stride * i;
+    bf16* vc = e->vtcache + e->cache_layer_stride * i;
+    launch_layernorm(e->s_x, L.ln1_w, L.ln1_b, e->s_ln, M, H, d.ln_eps, H, st);
+    SLIN(e->s_ln, L.attn_w, L.attn_b, nullptr, e->s_qkv, M, e->qkv_cols, H, SV_ACT_NONE, st);
+    if (e->v2)
+      launch_rope(e->s_qkv, M, C, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, nullptr, d.n_positions, pos0, st);
+    launch_kv_scatter(e->s_qkv, kc, vc, B, C, d.n_head * D, d.n_kv_head, D, e->tcap, pos0, st);
+    cudaError_t ce = launch_attention_chunk(e->s_qkv, e->qkv_cols, C, kc, vc, e->s_attn, B, C, pos0, d.n_head, d.n_kv_head, D,
+                                            e->tcap, e->window, st);
+    if (ce != cudaSuccess) return fail(e, SV_ERR_CUDA, "chunk attention launch failed: %s", cudaGetErrorString(ce));
+    SLIN(e->s_attn, L.proj_w, L.proj_b, e->s_x, e->s_x, M, H, H, SV_ACT_NONE, st);
+    launch_layernorm(e->s_x, L.ln2_w, L.ln2_b, e->s_ln, M, H, d.ln_eps, H, st);
+    SLIN(e->s_ln, L.fc_w, L.fc_b, nullptr, e->s_h, M, d.n_inner, H, SV_ACT_GELU_TANH, st);
+    SLIN(e->s_h, L.fc2_w, L.fc2_b, e->s_x, e->s_x, M, H, d.n_inner, SV_ACT_NONE, st);
+  }
+  launch_layernorm(e->s_x, e->lnf_w, e->lnf_b, e->s_ln, M, H, d.ln_eps, H, st);
+  launch_score_targets(ids, n, c0, B, C, d.vocab, e->s_tgt, st);
+  cudaError_t ce = launch_lm_logprob_partials(e->s_ln, e->lm_head, e->s_tgt, e->s_part, e->s_tl, M, d.vocab, H, st);
+  if (ce != cudaSuccess) return fail(e, SV_ERR_CUDA, "lm_head log-likelihood launch failed: %s", cudaGetErrorString(ce));
+  launch_logprob_merge(e->s_part, lm_logprob_ntiles(d.vocab), e->s_tl, M, C, c0 + 1, n, logprobs, st);
+  if (last) {
+    launch_gather_rows(e->s_x, e->d_last, B, C, C - 1, H, st);
+    launch_layernorm(e->d_last, e->lnf_w, e->lnf_b, e->d_ln, B, H, d.ln_eps, H, st);
+    ce = launch_lm_logits(e->d_ln, e->lm_head, e->logits, B, d.vocab, H, st);
+    if (ce != cudaSuccess) return fail(e, SV_ERR_CUDA, "lm_head launch failed: %s", cudaGetErrorString(ce));
+  }
+#undef SLIN
   return SV_OK;
 }
 
@@ -466,7 +521,7 @@ int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaS
     launch_layernorm(e->d_x, L.ln1_w, L.ln1_b, e->d_ln, B, H, d.ln_eps, H, st);
     launch_linear_rowgroup(e->d_ln, L.attn_w, L.attn_b, nullptr, e->d_qkv, B, e->qkv_cols, H, SV_ACT_NONE, st);
     if (e->v2)
-      launch_rope(e->d_qkv, B, 1, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, e->state, d.n_positions, st);
+      launch_rope(e->d_qkv, B, 1, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, e->state, d.n_positions, 0, st);
     launch_kv_append(e->d_qkv, kc, vc, e->state, B, d.n_head * D, d.n_kv_head, D, e->tcap, st);
     launch_attention_decode(e->d_qkv, e->qkv_cols, kc, vc, e->d_attn, e->attn_partial, e->state, B, d.n_head,
                             d.n_kv_head, D, e->tcap, nsplit, e->window, st);
@@ -893,6 +948,41 @@ int sv_decode_step(sv_engine* e, const int32_t* ids, float* logits, void* stream
   SV_CK(e, cudaGetLastError());
   e->host_cur_len += 1;
   return SV_OK;
+}
+
+int sv_score_tokens(sv_engine* e, const int32_t* ids, int32_t batch, int32_t n_tokens, float* logprobs, void* stream) {
+  if (!e || !ids || !logprobs) return fail(e, SV_ERR_INVALID, "null argument");
+  if (!e->prefilled) return fail(e, SV_ERR_STATE, "sv_score_tokens needs sv_prefill first");
+  if (batch != e->cur_batch) return fail(e, SV_ERR_INVALID, "batch %d != the current batch %d", batch, e->cur_batch);
+  if (n_tokens < 1) return fail(e, SV_ERR_INVALID, "n_tokens must be >= 1");
+  if ((int64_t)e->host_cur_len + n_tokens > e->d.max_len)
+    return fail(e, SV_ERR_INVALID, "cache length %d + n_tokens %d exceeds max_len %d", e->host_cur_len, n_tokens, e->d.max_len);
+  SV_CK(e, cudaSetDevice(e->device));
+  LaunchScope scope(e);
+  cudaStream_t st = (cudaStream_t)stream;
+  const sv_model_desc& d = e->d;
+  if (!e->s_x) {
+    const int64_t R = kScoreRows;
+    bool ok = true;
+#define SAL(ptr, n) ok = ok && (dev_alloc(e, &e->ptr, (n)) == cudaSuccess)
+    SAL(s_ln, R * d.hidden); SAL(s_qkv, R * e->qkv_cols); SAL(s_attn, R * d.hidden); SAL(s_h, R * d.n_inner);
+    SAL(s_tgt, R); SAL(s_part, R * lm_logprob_ntiles(d.vocab)); SAL(s_tl, R); SAL(s_x, R * d.hidden);
+#undef SAL
+    if (!ok) { e->s_x = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the scoring buffers failed: %s", cudaGetErrorString(cudaGetLastError())); }
+  }
+  const int B = batch, n = n_tokens, pos0 = e->host_cur_len, C = std::max(1, kScoreRows / B);
+  // position 0: from the logits the previous call left resident, with the same partials + merge
+  launch_score_targets(ids, n, -1, B, 1, d.vocab, e->s_tgt, st);
+  launch_logits_logprob_partials(e->logits, d.vocab, B, e->s_tgt, e->s_part, e->s_tl, st);
+  launch_logprob_merge(e->s_part, lm_logprob_ntiles(d.vocab), e->s_tl, B, 1, 0, n, logprobs, st);
+  for (int c0 = 0; c0 < n; c0 += C) {
+    const int Cc = std::min(C, n - c0);
+    int r = run_score_chunk(e, ids, n, c0, Cc, B, pos0 + c0, logprobs, c0 + Cc == n, st);
+    if (r != SV_OK) return r;
+  }
+  SV_CK(e, cudaGetLastError());
+  // the scored tokens extend the prefix: a decode step, another scoring call or a generation continues from here
+  return finish_prefill_impl(e, B, pos0 + n, nullptr, st);
 }
 
 // The generate loop.  `cb` (optional) receives the new tokens of every row each time the host polls the device
@@ -1368,6 +1458,46 @@ int sv_op_attention_mqa(const void* qkv, void* out, int32_t batch, int32_t seq, 
   r = cudaStreamSynchronize(st);
   cudaFree(kc);
   return r == cudaSuccess ? SV_OK : op_fail("attention_mqa", r);
+}
+
+int sv_op_attention_chunk(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t q0, int32_t n_head, int32_t n_kv,
+                          int32_t window, void* stream) {
+  if (!qkv || !out || batch < 1 || seq < 1 || q0 < 0 || q0 >= seq || n_kv < 1 || n_head % n_kv || n_head / n_kv > 16 ||
+      window < 0)
+    return fail(nullptr, SV_ERR_INVALID, "bad attention arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = 128, tcap = (seq + 31) / 32 * 32, cols = (n_head + 2 * n_kv) * D;
+  const size_t n = (size_t)batch * n_kv * tcap * D;
+  bf16* kc = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&kc), 2 * n * 2);
+  if (r != cudaSuccess) return op_fail("attention_chunk alloc", r);
+  bf16* vc = kc + n;
+  cudaMemsetAsync(kc, 0, 2 * n * 2, st);
+  launch_kv_scatter((const bf16*)qkv, kc, vc, batch, seq, n_head * D, n_kv, D, tcap, 0, st);
+  r = launch_attention_chunk((const bf16*)qkv + (size_t)q0 * cols, cols, seq, kc, vc, (bf16*)out, batch, seq - q0, q0, n_head,
+                             n_kv, D, tcap, window, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(kc);
+  return r == cudaSuccess ? SV_OK : op_fail("attention_chunk", r);
+}
+
+int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets, float* logprob, int32_t M, int32_t N, int32_t K,
+                     void* stream) {
+  if (!x || !w || !targets || !logprob || M < 1 || N < 1 || K < 64 || K % 64) return fail(nullptr, SV_ERR_INVALID, "bad lm_logprob arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nt = lm_logprob_ntiles(N);
+  void* buf = nullptr;
+  cudaError_t r = cudaMalloc(&buf, (size_t)M * nt * sizeof(float2) + (size_t)M * sizeof(float));
+  if (r != cudaSuccess) return op_fail("lm_logprob alloc", r);
+  float2* part = reinterpret_cast<float2*>(buf);
+  float* tl = reinterpret_cast<float*>(part + (size_t)M * nt);
+  r = launch_lm_logprob_partials((const bf16*)x, (const bf16*)w, targets, part, tl, M, N, K, st);
+  if (r == cudaSuccess) {
+    launch_logprob_merge(part, nt, tl, M, M, 0, M, logprob, st);
+    r = cudaStreamSynchronize(st);
+  }
+  cudaFree(buf);
+  return r == cudaSuccess ? SV_OK : op_fail("lm_logprob", r);
 }
 
 }  // extern "C"

@@ -12,6 +12,9 @@
 //               bias / activation / residual with the reference's bf16 rounding points to 8 consecutive
 //               columns of a row, 16-byte global stores.
 // Rows beyond M and weight rows beyond N are zero-filled by TMA (OOB fill) and masked at the store.
+// EPI = kEpiLogprob (the fused lm_head log-likelihood of sv_score.cu) replaces the store: straight from the accumulator
+// registers, every logit is rounded to bf16 and each (row, N-tile) writes its (max, sum of exp) pair and, in the tile that
+// holds it, the target's logit; the [M, N] logits never reach global memory and N needs no alignment.
 // Every mbarrier wait is bounded: a protocol bug traps (CUDA error) instead of hanging the GPU.
 #include <cuda.h>
 
@@ -116,12 +119,18 @@ SV_DEVINL void wgmma_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
 }
 #undef SV_ACC8
 
-template <int BN>
+// kEpiLogits: the plain epilogue for any N (columns masked one by one), so that resident logits carry exactly the bf16
+// values the kEpiLogprob epilogue sees
+constexpr int kEpiLinear = 0, kEpiLogprob = 1, kEpiLogits = 2;
+
+template <int BN, int EPI = kEpiLinear>
 __global__ void __launch_bounds__(kThreads, 2) linear_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_x,
                                                                    const __grid_constant__ CUtensorMap tmap_w,
                                                                    const bf16* __restrict__ bias,
                                                                    const bf16* __restrict__ res, bf16* __restrict__ Y,
-                                                                   int M, int N, int K, int act) {
+                                                                   int M, int N, int K, int act,
+                                                                   const int32_t* __restrict__ targets,
+                                                                   float2* __restrict__ part, float* __restrict__ tgt_logit) {
   using C = Cfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -179,6 +188,42 @@ __global__ void __launch_bounds__(kThreads, 2) linear_wgmma_kernel(const __grid_
   wgmma_wait<0>();
   fence_acc(acc);
 
+  if constexpr (EPI == kEpiLogprob) {
+    // d[i] is row r0 + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (lane % 4) + i % 2: the 4 lanes of a quad hold a row's BN columns
+    const int r0 = m_blk * BM + half * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c0 = n_blk * BN + 2 * (lane & 3);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) {
+      const int col = c0 + 8 * (i >> 2) + (i & 1);
+      acc[i] = col < N ? bf16_round(acc[i]) : -INFINITY;          // HF: lm_head output is bf16
+      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], acc[i]);
+    }
+    mx[0] = quad_max(mx[0]);
+    mx[1] = quad_max(mx[1]);
+    float se[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) se[(i >> 1) & 1] += expf(acc[i] - mx[(i >> 1) & 1]);
+    se[0] = quad_sum(se[0]);
+    se[1] = quad_sum(se[1]);
+    const int tg0 = r0 < M ? targets[r0] : -1, tg1 = r0 + 8 < M ? targets[r0 + 8] : -1;
+    float tv0 = 0.f, tv1 = 0.f;
+    bool hit0 = false, hit1 = false;
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) {
+      const int col = c0 + 8 * (i >> 2) + (i & 1);
+      if ((i >> 1) & 1) { if (col == tg1) { tv1 = acc[i]; hit1 = true; } }
+      else if (col == tg0) { tv0 = acc[i]; hit0 = true; }
+    }
+    if (hit0) tgt_logit[r0] = tv0;
+    if (hit1) tgt_logit[r0 + 8] = tv1;
+    if ((lane & 3) == 0) {
+      if (r0 < M) part[(int64_t)r0 * gridDim.x + n_blk] = make_float2(mx[0], se[0]);
+      if (r0 + 8 < M) part[(int64_t)(r0 + 8) * gridDim.x + n_blk] = make_float2(mx[1], se[1]);
+    }
+    return;
+  }
+
   // both warpgroups are done reading the ring before either overwrites it with the fp32 tile
   asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
   float* tile = reinterpret_cast<float*>(smem_raw + (base - raw));
@@ -196,7 +241,11 @@ __global__ void __launch_bounds__(kThreads, 2) linear_wgmma_kernel(const __grid_
   for (int c = threadIdx.x; c < BM * BN / 8; c += kConsumers) {
     const int r = c / (BN / 8), c8 = (c % (BN / 8)) * 8;
     const int row = m_blk * BM + r, col = n_blk * BN + c8;
-    if (row >= M || col + 8 > N) continue;
+    if constexpr (EPI == kEpiLogits) {
+      if (row >= M || col >= N) continue;
+    } else {
+      if (row >= M || col + 8 > N) continue;
+    }
     const float4 lo = *reinterpret_cast<const float4*>(tile + r * C::kOutStride + c8);
     const float4 hi = *reinterpret_cast<const float4*>(tile + r * C::kOutStride + c8 + 4);
     const float a[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
@@ -207,7 +256,11 @@ __global__ void __launch_bounds__(kThreads, 2) linear_wgmma_kernel(const __grid_
     else { for (int j = 0; j < 8; ++j) rv[j] = 0.f; }
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = epilogue_elem(a[j], bv[j], act, has_res, rv[j]);
-    *reinterpret_cast<uint4*>(Y + (int64_t)row * N + col) = pack8(o);
+    if constexpr (EPI == kEpiLogits) {
+      for (int j = 0; j < 8 && col + j < N; ++j) Y[(int64_t)row * N + col + j] = __float2bfloat16_rn(o[j]);
+    } else {
+      *reinterpret_cast<uint4*>(Y + (int64_t)row * N + col) = pack8(o);
+    }
   }
 }
 
@@ -264,20 +317,22 @@ static bool cached_map(CUtensorMap* out, const void* ptr, int64_t rows, int64_t 
   return true;
 }
 
-template <int BN>
+template <int BN, int EPI = kEpiLinear>
 static cudaError_t launch(const bf16* x, const bf16* w, const bf16* bias, const bf16* res, bf16* y, int M, int N,
-                          int K, int act, cudaStream_t st) {
+                          int K, int act, cudaStream_t st, const int32_t* targets = nullptr, float2* part = nullptr,
+                          float* tgt_logit = nullptr) {
   CUtensorMap mx, mw;
   if (!cached_map(&mx, x, M, K, BM) || !cached_map(&mw, w, N, K, BN)) return cudaErrorInvalidValue;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(linear_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(linear_wgmma_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg<BN>::kSmemBytes);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
-  linear_wgmma_kernel<BN><<<grid, kThreads, Cfg<BN>::kSmemBytes, st>>>(mx, mw, bias, res, y, M, N, K, act);
+  linear_wgmma_kernel<BN, EPI><<<grid, kThreads, Cfg<BN>::kSmemBytes, st>>>(mx, mw, bias, res, y, M, N, K, act, targets,
+                                                                             part, tgt_logit);
   count_launch();
   return cudaGetLastError();
 }
@@ -298,6 +353,19 @@ cudaError_t launch_linear_wgmma(const bf16* x, const bf16* w, const bf16* bias, 
   const bool wide = (N % 128 == 0) && ((int64_t)mt * ((N + 63) / 64) > (int64_t)nsm * 2);
   return wide ? wg::launch<128>(x, w, bias, res, y, M, N, K, act, st)
               : wg::launch<64>(x, w, bias, res, y, M, N, K, act, st);
+}
+
+int lm_logprob_ntiles(int N) { return (N + 127) / 128; }
+
+cudaError_t launch_lm_logits(const bf16* x, const bf16* w, bf16* y, int M, int N, int K, cudaStream_t st) {
+  if (M < 1 || N < 1 || K < 64 || K % 64) return cudaErrorInvalidValue;
+  return wg::launch<128, wg::kEpiLogits>(x, w, nullptr, nullptr, y, M, N, K, /*act=*/0, st);
+}
+
+cudaError_t launch_lm_logprob_partials(const bf16* x, const bf16* w, const int32_t* targets, float2* part, float* tgt_logit,
+                                       int M, int N, int K, cudaStream_t st) {
+  if (M < 1 || N < 1 || K < 64 || K % 64) return cudaErrorInvalidValue;
+  return wg::launch<128, wg::kEpiLogprob>(x, w, nullptr, nullptr, nullptr, M, N, K, /*act=*/0, st, targets, part, tgt_logit);
 }
 
 }  // namespace sv

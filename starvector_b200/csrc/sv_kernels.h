@@ -41,12 +41,14 @@ void launch_slab_layernorm(const bf16* z, const bf16* w, const bf16* b, bf16* y,
                            int64_t slab, float eps, cudaStream_t st);
 void launch_batchnorm_tokens(const bf16* z, const bf16* w, const bf16* b, const bf16* rmean, const bf16* rvar, bf16* y,
                              int batch, int q, int h, float eps, cudaStream_t st);
+// rows [b][t] of x: visual[b][t] for t < q, else wte[prompt_ids[b * id_stride + t - q]]; + wpe[pos0 + t] when wpe != nullptr
 void launch_embed_prefix(const bf16* visual, const int32_t* prompt_ids, const bf16* wte, const bf16* wpe, bf16* x,
-                         int batch, int q, int p, int h, int vocab, cudaStream_t st);
+                         int batch, int q, int p, int h, int vocab, int pos0, int id_stride, cudaStream_t st);
 void launch_embed_tokens(const int32_t* ids, const bf16* wte, const bf16* wpe, const GenState* state, bf16* x,
                          int batch, int h, int vocab, int n_positions, cudaStream_t st);
+// K/V of qkv rows [b][0, seq) -> cache positions t0 .. t0+seq-1
 void launch_kv_scatter(const bf16* qkv, bf16* kcache, bf16* vtcache, int batch, int seq, int q_cols, int n_kv, int d,
-                       int tcap, int max_batch_unused, cudaStream_t st);
+                       int tcap, int t0, cudaStream_t st);
 void launch_kv_append(const bf16* qkv, bf16* kcache, bf16* vtcache, const GenState* state, int batch, int q_cols,
                       int n_kv, int d, int tcap, cudaStream_t st);
 void launch_kv_gather(const bf16* ksrc, const bf16* vsrc, bf16* kdst, bf16* vdst, const int32_t* idx, int rows, int n_kv,
@@ -70,6 +72,25 @@ bool wgmma_supported(int M, int N, int K);
 // returns cudaSuccess or the error of tensor-map creation / launch
 cudaError_t launch_linear_wgmma(const bf16* x, const bf16* w, const bf16* bias, const bf16* res, bf16* y, int M, int N,
                                 int K, int act, cudaStream_t st);
+// fused lm_head log-likelihood, first half: logits = bf16(x[M,K] . w[N,K]^T) stay on chip; per (row, 128-column tile)
+// part[row * lm_logprob_ntiles(N) + tile] = (max, sum exp(logit - max)) and tgt_logit[row] = logit[targets[row]]
+// (any N; K % 64 == 0; targets must lie in [0, N))
+int lm_logprob_ntiles(int N);
+// y[M,N] = bf16(x . w^T) for any N, with the same tiling and rounding as launch_lm_logprob_partials
+cudaError_t launch_lm_logits(const bf16* x, const bf16* w, bf16* y, int M, int N, int K, cudaStream_t st);
+cudaError_t launch_lm_logprob_partials(const bf16* x, const bf16* w, const int32_t* targets, float2* part, float* tgt_logit,
+                                       int M, int N, int K, cudaStream_t st);
+
+// ---- sv_score.cu : the rest of teacher-forced scoring
+// tgt[b * C + t] = clamp(ids[b * n + c0 + t + 1], 0, vocab) (0 past the end of the row)
+void launch_score_targets(const int32_t* ids, int n, int c0, int batch, int C, int vocab, int32_t* tgt, cudaStream_t st);
+// the partials of launch_lm_logprob_partials for resident bf16 logits rows [batch][vocab]
+void launch_logits_logprob_partials(const bf16* logits, int vocab, int batch, const int32_t* targets, float2* part,
+                                    float* tgt_logit, cudaStream_t st);
+// logprob of row r = tgt_logit[r] - (m + log s) over its tiles' partials, written to out[(r / C) * n + off + r % C]
+// when off + r % C < n
+void launch_logprob_merge(const float2* part, int ntiles, const float* tgt_logit, int rows, int C, int off, int n,
+                          float* out, cudaStream_t st);
 
 // ---- sv_attention.cu
 void launch_attention_vit(const bf16* qkv, const bf16* vt, bf16* out, int batch, int seq, int heads, int seq_pad,
@@ -77,13 +98,18 @@ void launch_attention_vit(const bf16* qkv, const bf16* vt, bf16* out, int batch,
 // causal attention of `seq` new tokens per row against the cache (prefill: cache already holds them)
 void launch_attention_heads(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache, bf16* out,
                             int batch, int seq, int n_head, int n_kv, int d, int tcap, int window, cudaStream_t st);
+// scoring chunk: queries of qkv rows [b * q_rows_per_b + t], t < C, at cache positions q0 + t (the cache already holds
+// positions <= q0 + C - 1); out rows [b * C + t]
+cudaError_t launch_attention_chunk(const bf16* qkv, int q_cols_total, int q_rows_per_b, const bf16* kcache,
+                                   const bf16* vtcache, bf16* out, int batch, int C, int q0, int n_head, int n_kv, int d,
+                                   int tcap, int window, cudaStream_t st);
 void launch_attention_decode(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache, bf16* out,
                              float* partial, const GenState* state, int batch, int n_head, int n_kv, int d, int tcap,
                              int nsplit, int window, cudaStream_t st);
 // RoPE in place on the q and k parts of packed qkv rows [rows][qkv_cols] (StarCoder2, rotate_half convention);
 // cos/sin tables are bf16 [max_pos][D/2]; position of row r = pos0 + (r % seq) or state->cur_len when state != nullptr.
 void launch_rope(bf16* qkv, int rows, int seq, int qkv_cols, int n_rot_heads, int d, const bf16* cos_t, const bf16* sin_t,
-                 const GenState* state, int max_pos, cudaStream_t st);
+                 const GenState* state, int max_pos, int pos0, cudaStream_t st);
 void launch_rope_append(bf16* qkv, int batch, int qkv_cols, int n_head, int n_kv, int d, const bf16* cos_t,
                         const bf16* sin_t, bf16* kcache, bf16* vtcache, const GenState* state, int tcap, int max_pos,
                         bool pdl, cudaStream_t st);

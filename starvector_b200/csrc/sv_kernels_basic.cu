@@ -234,21 +234,22 @@ void launch_batchnorm_tokens(const bf16* z, const bf16* w, const bf16* b, const 
 
 // ------------------------------------------------------------------------------------------
 // inputs_embeds = cat([visual, wte(prompt)]) (starvector_base.py:218-219) + wpe[position]
-// (GPTBigCodeModel.forward: hidden = inputs_embeds + position_embeds), bf16 add.
+// (GPTBigCodeModel.forward: hidden = inputs_embeds + position_embeds), bf16 add.  Row t sits at position pos0 + t
+// (pos0 > 0: a scoring chunk appended to a filled cache); prompt row b starts at prompt + b * id_stride.
 __global__ void embed_prefix_kernel(const bf16* __restrict__ visual, const int32_t* __restrict__ prompt,
                                     const bf16* __restrict__ wte, const bf16* __restrict__ wpe, bf16* __restrict__ x,
-                                    int q, int p, int h, int vocab) {
+                                    int q, int p, int h, int vocab, int pos0, int id_stride) {
   const int t0 = q + p;
   const int b = blockIdx.x / t0, t = blockIdx.x % t0;
   const bf16* src;
   if (t < q) {
     src = visual + ((int64_t)b * q + t) * h;
   } else {
-    int id = prompt[b * p + (t - q)];
+    int id = prompt[(int64_t)b * id_stride + (t - q)];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
     src = wte + (int64_t)id * h;
   }
-  const bf16* pos = wpe ? wpe + (int64_t)t * h : nullptr;   // RoPE models (StarCoder2) have no learned positions
+  const bf16* pos = wpe ? wpe + (int64_t)(pos0 + t) * h : nullptr;   // RoPE models (StarCoder2) have no learned positions
   for (int c = threadIdx.x * 8; c < h; c += blockDim.x * 8) {
     float a[8], d[8];
     unpack8(ldg_cached(src + c), a);
@@ -261,8 +262,8 @@ __global__ void embed_prefix_kernel(const bf16* __restrict__ visual, const int32
   }
 }
 void launch_embed_prefix(const bf16* visual, const int32_t* prompt_ids, const bf16* wte, const bf16* wpe, bf16* x,
-                         int batch, int q, int p, int h, int vocab, cudaStream_t st) {
-  embed_prefix_kernel<<<batch * (q + p), 128, 0, st>>>(visual, prompt_ids, wte, wpe, x, q, p, h, vocab);
+                         int batch, int q, int p, int h, int vocab, int pos0, int id_stride, cudaStream_t st) {
+  embed_prefix_kernel<<<batch * (q + p), 128, 0, st>>>(visual, prompt_ids, wte, wpe, x, q, p, h, vocab, pos0, id_stride);
   count_launch();
 }
 
@@ -298,9 +299,9 @@ void launch_embed_tokens(const int32_t* ids, const bf16* wte, const bf16* wpe, c
 // (so the P.V tensor-core operand is a contiguous 16-byte load per lane; see sv_attention.cu).
 // The reference re-allocates and copies the whole cache every step (torch.cat, SURVEY.md K15).
 __global__ void kv_write_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kcache, bf16* __restrict__ vtcache,
-                                const GenState* __restrict__ state, int seq, int q_cols, int n_kv, int d, int tcap) {
+                                const GenState* __restrict__ state, int t0, int seq, int q_cols, int n_kv, int d, int tcap) {
   const int b = blockIdx.y, ts = blockIdx.x;
-  const int t = state ? state->cur_len + ts : ts;
+  const int t = (state ? state->cur_len : t0) + ts;
   if (t >= tcap) return;
   const int cols = q_cols + 2 * n_kv * d;
   const bf16* row = qkv + ((int64_t)b * seq + ts) * cols;
@@ -311,13 +312,13 @@ __global__ void kv_write_kernel(const bf16* __restrict__ qkv, bf16* __restrict__
   }
 }
 void launch_kv_scatter(const bf16* qkv, bf16* kcache, bf16* vtcache, int batch, int seq, int q_cols, int n_kv, int d,
-                       int tcap, int, cudaStream_t st) {
-  kv_write_kernel<<<dim3(seq, batch), 128, 0, st>>>(qkv, kcache, vtcache, nullptr, seq, q_cols, n_kv, d, tcap);
+                       int tcap, int t0, cudaStream_t st) {
+  kv_write_kernel<<<dim3(seq, batch), 128, 0, st>>>(qkv, kcache, vtcache, nullptr, t0, seq, q_cols, n_kv, d, tcap);
   count_launch();
 }
 void launch_kv_append(const bf16* qkv, bf16* kcache, bf16* vtcache, const GenState* state, int batch, int q_cols,
                       int n_kv, int d, int tcap, cudaStream_t st) {
-  kv_write_kernel<<<dim3(1, batch), 128, 0, st>>>(qkv, kcache, vtcache, state, 1, q_cols, n_kv, d, tcap);
+  kv_write_kernel<<<dim3(1, batch), 128, 0, st>>>(qkv, kcache, vtcache, state, 0, 1, q_cols, n_kv, d, tcap);
   count_launch();
 }
 
@@ -585,9 +586,9 @@ void launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int d, float theta
 }
 __global__ void rope_kernel(bf16* __restrict__ qkv, int seq, int qkv_cols, int n_rot_heads, int d,
                             const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
-                            const GenState* __restrict__ state, int max_pos) {
+                            const GenState* __restrict__ state, int max_pos, int pos0) {
   const int row = blockIdx.x, half = d >> 1;
-  int pos = state ? state->cur_len : (row % seq);
+  int pos = state ? state->cur_len : pos0 + (row % seq);
   pos = pos >= max_pos ? max_pos - 1 : pos;
   bf16* base = qkv + (int64_t)row * qkv_cols;
   for (int i = threadIdx.x; i < n_rot_heads * half; i += blockDim.x) {
@@ -649,8 +650,8 @@ void launch_rope_append(bf16* qkv, int batch, int qkv_cols, int n_head, int n_kv
 }
 
 void launch_rope(bf16* qkv, int rows, int seq, int qkv_cols, int n_rot_heads, int d, const bf16* cos_t, const bf16* sin_t,
-                 const GenState* state, int max_pos, cudaStream_t st) {
-  rope_kernel<<<rows, 256, 0, st>>>(qkv, seq, qkv_cols, n_rot_heads, d, cos_t, sin_t, state, max_pos);
+                 const GenState* state, int max_pos, int pos0, cudaStream_t st) {
+  rope_kernel<<<rows, 256, 0, st>>>(qkv, seq, qkv_cols, n_rot_heads, d, cos_t, sin_t, state, max_pos, pos0);
   count_launch();
 }
 

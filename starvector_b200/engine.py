@@ -198,6 +198,20 @@ class Engine:
                                               _stream_ptr(self.device)))
         return logits
 
+    def score(self, ids: torch.Tensor) -> torch.Tensor:
+        """Teacher-forced log-likelihoods at prefill speed (`sv_score_tokens`): ids `[B, T]` are appended to the cache of the
+        current batch and fp32 `[B, T]` is returned, `out[b, t] = log p(ids[b, t] | cache, ids[b, :t])` (t = 0 from the
+        resident logits of the previous prefill / decode step / score call).  The tokens extend the prefix, so `decode_step`,
+        `score` or `generate` may follow."""
+        t = self._dev(ids, torch.int32)
+        if t.dim() != 2 or t.shape[0] != self._batch:
+            raise ValueError(f"ids must be [B, T] with B = the current batch ({self._batch}), got {tuple(t.shape)}")
+        out = torch.empty(t.shape[0], t.shape[1], dtype=torch.float32, device=self.device)
+        with self._lock:
+            self._ck(self._lib.sv_score_tokens(self._h, C.c_void_p(t.data_ptr()), t.shape[0], t.shape[1],
+                                               C.c_void_p(out.data_ptr()), _stream_ptr(self.device)))
+        return out
+
     def reorder_cache(self, src_rows: torch.Tensor) -> None:
         """KV-cache row permutation for beam search: row r <- row src_rows[r]."""
         idx = self._dev(src_rows, torch.int32).reshape(-1)
@@ -349,4 +363,22 @@ def op_attention_mqa(qkv: torch.Tensor, batch: int, seq: int, heads: int) -> tor
     lib = _lib.load()
     out = torch.empty(batch * seq, heads * 128, dtype=torch.bfloat16, device=qkv.device)
     _lib.check(lib, lib.sv_op_attention_mqa(_p(qkv), _p(out), batch, seq, heads, _stream_ptr(qkv.device)))
+    return out
+
+
+def op_attention_chunk(qkv: torch.Tensor, batch: int, seq: int, q0: int, n_head: int, n_kv: int, window: int = 0) -> torch.Tensor:
+    """Queries of positions [q0, seq) against a cache of all `seq` positions of packed qkv `[batch * seq, (n_head + 2 n_kv) * 128]`."""
+    lib = _lib.load()
+    out = torch.empty(batch * (seq - q0), n_head * 128, dtype=torch.bfloat16, device=qkv.device)
+    _lib.check(lib, lib.sv_op_attention_chunk(_p(qkv), _p(out), batch, seq, q0, n_head, n_kv, window, _stream_ptr(qkv.device)))
+    return out
+
+
+def op_lm_logprob(x: torch.Tensor, w: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
+    """`log_softmax(float(bf16(x @ w.T)))[m, targets[m]]`, fp32 `[M]`, without materialising the logits."""
+    lib = _lib.load()
+    M, K = x.shape
+    tg = targets.to(device=x.device, dtype=torch.int32).contiguous()
+    out = torch.empty(M, dtype=torch.float32, device=x.device)
+    _lib.check(lib, lib.sv_op_lm_logprob(_p(x), _p(w), _p(tg), _p(out), M, w.shape[0], K, _stream_ptr(x.device)))
     return out

@@ -95,6 +95,8 @@ class _SvgTransformer:
         self.transformer = _Transformer(owner)
         self.prompt = "<svg"                                   # starcoder.py:38
         self.svg_start_token = "<svg-start>"
+        if owner.v2:
+            self.svg_end_token = "<svg-end>"                   # starcoder2.py:46
 
 
 class _ImageEncoder:
@@ -149,6 +151,53 @@ class StarVectorStarCoder:
         enc = self.svg_transformer.tokenizer([prompt] * batch, add_special_tokens=False, return_tensors="pt",
                                              padding="longest", truncation=True)
         return enc["input_ids"]
+
+    def _get_svg_text(self, svg_list: List[str]) -> List[str]:                # starvector_v1.py:20-22, starvector_v2.py:49-51
+        tok = self.svg_transformer.tokenizer
+        if self.v2:
+            return [t + self.svg_transformer.svg_end_token + tok.eos_token for t in svg_list]
+        return [t + tok.eos_token for t in svg_list]
+
+    def _tokenize(self, text: List[str], max_length: int) -> Dict[str, torch.Tensor]:   # starvector_base.py:108-118
+        return self.svg_transformer.tokenizer(text, truncation=True, add_special_tokens=True, padding="longest",
+                                              max_length=max_length, return_tensors="pt")
+
+    def _create_targets(self, input_ids: torch.Tensor) -> torch.Tensor:     # starvector_base.py:120-123
+        return input_ids.masked_fill(input_ids == self.svg_transformer.tokenizer.pad_token_id, -100)
+
+    def _score_group(self, image: torch.Tensor, svg_ids: torch.Tensor) -> torch.Tensor:
+        """log p(svg_ids[:, t] | visual prefix, svg_ids[:, :t]) fp32 `[b, T]` for at most max_batch images."""
+        emb, _ = self.engine.encode_images(image, return_embeds=True)
+        self.engine.prefill_embeds(emb)
+        return self.engine.score(svg_ids)
+
+    @torch.no_grad()
+    def forward(self, batch: Dict[str, Any]) -> torch.Tensor:
+        """`StarVectorBase.forward(batch)` for the im2svg task (starvector_base.py:150-194, `embed_im_to_svg`): the causal-LM
+        cross-entropy of `svg + eos` (v2: `svg + <svg-end> + eos`) after the visual prefix, HF's mean over every non-ignored
+        token of the batch (pads -> -100).  Runs as encode -> prefill of the prefix -> teacher-forced scoring; batches above
+        max_batch run in groups whose NLL sums and token counts are added (not their means averaged)."""
+        image, svgs = batch["image"], list(batch["svg"])
+        if image.shape[0] != len(svgs):
+            raise ValueError(f"{image.shape[0]} images but {len(svgs)} svg strings")
+        tokens = self._tokenize(self._get_svg_text(svgs), self.max_length)
+        ids, mask = tokens["input_ids"], tokens["attention_mask"]
+        if self.v2 and not bool(torch.all(mask == 1)):
+            # the v2 tokenizer pads on the left: HF would put masked pads between the prefix and the svg and shift the RoPE
+            # positions of the shorter rows
+            raise NotImplementedError("v2 batches of unequal svg token lengths (left padding) are not built")
+        targets = self._create_targets(ids)
+        mb = self.engine.dims.max_batch
+        nll, count = None, 0
+        for lo in range(0, len(svgs), mb):
+            lp = self._score_group(image[lo:lo + mb], ids[lo:lo + mb])
+            keep = (targets[lo:lo + mb] != -100).to(lp.device)
+            part = -(lp.double() * keep).sum()
+            nll = part if nll is None else nll + part
+            count += int(keep.sum())
+        return (nll / count).float()
+
+    __call__ = forward
 
     def _stop_ids(self) -> List[int]:
         return list(self.svg_transformer.tokenizer("</svg>", add_special_tokens=False)["input_ids"])   # base:226
@@ -361,6 +410,46 @@ class StarVectorForCausalLM:
         write_checkpoint(path, self.config, state_dict)
 
     # -- scoring (starvector_arch.py:161-184) ------------------------------------------------
+    def _check_scoring_args(self, vision_embeds: torch.Tensor, input_ids: torch.Tensor, num_generations: int,
+                            attention_mask: Optional[torch.Tensor]):
+        """Argument checks shared by `forward` and `score`: `(ids on the engine's device, b, G, completion mask or None)`."""
+        eng = self.model.engine
+        b, G = vision_embeds.shape[0], int(num_generations)
+        ids = input_ids.to(eng.device)
+        if ids.shape[0] != b * G:
+            raise ValueError(f"input_ids has {ids.shape[0]} rows, expected vision rows {b} x num_generations {G}")
+        if b * G > eng.dims.max_batch:
+            raise ValueError(f"{b} x {G} rows exceed the engine's max_batch {eng.dims.max_batch}")
+        T = ids.shape[1]
+        tail = None
+        if attention_mask is not None:
+            m = attention_mask.to(torch.bool)
+            tail = m[:, m.shape[1] - T:] if m.shape[1] >= T else m
+            if not bool(torch.all(m[:, : m.shape[1] - T])) or bool(torch.any(tail[:, 1:] & ~tail[:, :-1])):
+                raise NotImplementedError("only right-padded completions (mask = ones then zeros) are supported")
+        return ids, b, G, tail
+
+    def _prefill_shared_prefix(self, vision_embeds: torch.Tensor, b: int, G: int) -> None:
+        eng = self.model.engine
+        eng.prefill_embeds(vision_embeds.to(eng.device, torch.bfloat16))
+        if G > 1:
+            eng.expand_batch([r % b for r in range(b * G)])
+
+    @torch.no_grad()
+    def score(self, vision_embeds: torch.Tensor, input_ids: torch.Tensor, num_generations: int = 1,
+              attention_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Per-token log-likelihoods of the completions `forward` scores, without its `[rows, T, V]` logits:
+        fp32 `[b*G, T]`, `out[r, t] = log p(input_ids[r, t] | vision_embeds[r % b], input_ids[r, :t])`, the log-softmax
+        taken in fp32 over bf16 logits as `log_softmax(logits.float())` does.  Same prefix handling (prefilled once per image,
+        rows replicated in `.repeat` order) and argument checks as `forward`; the completion runs through the chunked
+        scoring path (`sv_score_tokens`).  Positions beyond a right-padded `attention_mask` are 0."""
+        ids, b, G, tail = self._check_scoring_args(vision_embeds, input_ids, num_generations, attention_mask)
+        self._prefill_shared_prefix(vision_embeds, b, G)
+        lp = self.model.engine.score(ids)
+        if tail is not None and tail.shape[1] == lp.shape[1]:
+            lp = lp.masked_fill(~tail.to(lp.device), 0.0)
+        return lp
+
     @torch.no_grad()
     def forward(self, vision_embeds: torch.Tensor, input_ids: torch.Tensor, num_generations: int = 1,
                 attention_mask: Optional[torch.Tensor] = None, num_logits_to_keep: int = 0):
@@ -371,24 +460,12 @@ class StarVectorForCausalLM:
         completion is teacher-forced through `sv_decode_step`.  Returns an object with `.logits` fp32 `[b*G, n_keep, V]`
         and `.loss = None`.  `attention_mask` may only mask a right-padded tail (what GRPO completions carry)."""
         eng = self.model.engine
-        b, G = vision_embeds.shape[0], int(num_generations)
-        ids = input_ids.to(eng.device)
-        if ids.shape[0] != b * G:
-            raise ValueError(f"input_ids has {ids.shape[0]} rows, expected vision rows {b} x num_generations {G}")
-        if b * G > eng.dims.max_batch:
-            raise ValueError(f"{b} x {G} rows exceed the engine's max_batch {eng.dims.max_batch}")
+        ids, b, G, _ = self._check_scoring_args(vision_embeds, input_ids, num_generations, attention_mask)
         T = ids.shape[1]
-        if attention_mask is not None:
-            m = attention_mask.to(torch.bool)
-            tail = m[:, m.shape[1] - T:] if m.shape[1] >= T else m
-            if not bool(torch.all(m[:, : m.shape[1] - T])) or bool(torch.any(tail[:, 1:] & ~tail[:, :-1])):
-                raise NotImplementedError("only right-padded completions (mask = ones then zeros) are supported")
         n_keep = T if int(num_logits_to_keep) <= 0 else int(num_logits_to_keep)
         if n_keep > T:
             raise NotImplementedError("num_logits_to_keep beyond the completion (prefix positions) is not built")
-        eng.prefill_embeds(vision_embeds.to(eng.device, torch.bfloat16))
-        if G > 1:
-            eng.expand_batch([r % b for r in range(b * G)])
+        self._prefill_shared_prefix(vision_embeds, b, G)
         out = torch.empty(b * G, n_keep, eng.dims.vocab, dtype=torch.float32, device=eng.device)
         for t in range(T):
             keep = t >= T - n_keep

@@ -31,6 +31,9 @@ class SyntheticTokenizer:
             "</svg>": [1245 % base or 3, 7 % base or 4, 29 % base or 5],
         }
         self._special = {self.eos_token_id, self.pad_token_id}
+        self._named = {self.eos_token: self.eos_token_id, self.pad_token: self.pad_token_id}
+        if n_added >= 5:                                  # v2 (llm/starcoder2.py:45-50): <svg-end> is the 4th token after [PAD]
+            self._named["<svg-end>"] = self.pad_token_id + 4
 
     def __len__(self) -> int:
         return self.vocab_size
@@ -39,9 +42,12 @@ class SyntheticTokenizer:
         if text in self._known:
             return list(self._known[text])
         ids: List[int] = []
-        for m in re.finditer(r"<t(\d+)>|<svg|</svg>|\S+", text):
+        named = "".join(re.escape(k) + "|" for k in self._named)
+        for m in re.finditer(r"<t(\d+)>|" + named + r"<svg|</svg>|\S+", text):
             tok = m.group(0)
-            if m.group(1) is not None:
+            if tok in self._named:
+                ids.append(self._named[tok])
+            elif m.group(1) is not None:
                 ids.append(int(m.group(1)) % self.vocab_size)
             elif tok in self._known:
                 ids.extend(self._known[tok])
@@ -52,6 +58,8 @@ class SyntheticTokenizer:
     def __call__(self, text: Union[str, Sequence[str]], add_special_tokens: bool = True, return_tensors=None, **kw):
         single = isinstance(text, str)
         rows = [self.encode(t) for t in ([text] if single else text)]
+        if kw.get("truncation") and kw.get("max_length") is not None:
+            rows = [r[: int(kw["max_length"])] for r in rows]
         if single and return_tensors is None:
             return {"input_ids": rows[0], "attention_mask": [1] * len(rows[0])}
         width = max(len(r) for r in rows)
