@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define SV_ABI_VERSION 5
+#define SV_ABI_VERSION 6
 #if defined(__GNUC__)
 #define SV_API __attribute__((visibility("default")))
 #else
@@ -76,7 +76,7 @@ typedef struct sv_model_desc {
   int32_t n_positions;  /* 8192 learned absolute positions */
   int32_t vocab;        /* 49156 = 49152 + [PAD] + 3 added tokens (llm/starcoder.py:43-53) */
   float ln_eps;         /* 1e-5 */
-  int32_t max_batch;    /* images per call on this GPU */
+  int32_t max_batch;    /* cache rows (images x beams / completions) per call on this GPU, [1,16] */
   int32_t max_len;      /* KV-cache capacity in tokens (prefix + generated) */
   /* v2 only (ignored for variant 0) */
   float rope_theta;       /* StarCoder2 rope_theta (hub config of bigcode/starcoder2-7b; default 10000 in transformers) */
@@ -106,7 +106,7 @@ typedef struct sv_gen_params {
  * (starvector_base.py:231-241: num_beams=2, do_sample, top_p, temperature, repetition_penalty, length_penalty;
  * :289-295: early_stopping=True, pad_token_id; starvector_v2.py:53-57: nothing -> HF defaults). */
 typedef struct sv_beam_params {
-  int32_t num_beams;          /* >= 2; batch * num_beams <= 8 cache rows */
+  int32_t num_beams;          /* >= 2 and <= 8; batch * num_beams <= 16 cache rows (and <= the engine's max_batch) */
   int32_t max_new_tokens;
   int32_t do_sample;          /* 1 = beam-sample (candidates drawn without replacement, device Philox stream) */
   int32_t early_stopping;     /* 0 = False (HF default), 1 = True (v1), 2 = "never" */
@@ -192,11 +192,14 @@ SV_API int sv_beam_search(sv_engine* e, const sv_beam_params* p, int32_t batch, 
  * over row candidates [batch * num_beams][2 * num_beams] with the double-buffered sequence arrays
  * [2][batch * num_beams][seq_stride] -> next tokens, parent rows (= HF beam_idx), returns 1 while the search continues.
  * tests/test_beam_core.py runs whole searches with them against HF generate(num_beams > 1). */
-SV_API int sv_beam_params_check(const sv_beam_params* p, int32_t batch);
+SV_API int sv_beam_params_check(const sv_beam_params* p, int32_t batch);   /* for an engine of 8 rows (the default) */
+SV_API int sv_beam_params_check_rows(const sv_beam_params* p, int32_t batch, int32_t max_rows);   /* max_rows <= 16 */
 SV_API int sv_beam_state_bytes(void);
 SV_API int sv_beam_state_init_host(const sv_beam_params* p, int32_t batch, int32_t first_cache_pos, void* state);
 SV_API int sv_beam_state_read_host(const void* state, int32_t* parity, int32_t* cur_len, int32_t* fin_len8,
-                                   float* beam_scores8);
+                                   float* beam_scores8);           /* rows 0-7 */
+SV_API int sv_beam_state_read16_host(const void* state, int32_t* parity, int32_t* cur_len, int32_t* fin_len16,
+                                     float* beam_scores16, float* running_scores16);
 SV_API int sv_beam_row_candidates_host(const sv_beam_params* p, const float* logits, int32_t vocab, const int32_t* seq,
                                        int32_t seq_len, float running_score, int32_t step, int32_t row, float* cand_key,
                                        float* cand_val, int32_t* cand_tok);

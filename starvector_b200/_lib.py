@@ -16,7 +16,7 @@ SV_OK, SV_ERR_INVALID, SV_ERR_CUDA, SV_ERR_UNSUPPORTED, SV_ERR_STATE = 0, -1, -2
 SV_DTYPE_BF16, SV_DTYPE_F32, SV_DTYPE_F16 = 0, 1, 2
 SV_ACT_NONE, SV_ACT_QUICKGELU, SV_ACT_GELU_TANH, SV_ACT_SILU = 0, 1, 2, 3
 SV_LINEAR_AUTO, SV_LINEAR_ROWGROUP, SV_LINEAR_TCGEN05 = 0, 1, 2
-ABI_VERSION = 5
+ABI_VERSION = 6
 SV_ALPHA_WHITE, SV_ALPHA_DROP = 0, 1
 
 
@@ -76,9 +76,12 @@ SIGNATURES = {
     "sv_expand_batch": (C.c_int, [_P, _P, C.c_int32, _P]),
     "sv_beam_search": (C.c_int, [_P, C.POINTER(BeamParams), _I, _P, _P, _P]),
     "sv_beam_params_check": (C.c_int, [C.POINTER(BeamParams), _I]),
+    "sv_beam_params_check_rows": (C.c_int, [C.POINTER(BeamParams), _I, _I]),
     "sv_beam_state_bytes": (C.c_int, []),
     "sv_beam_state_init_host": (C.c_int, [C.POINTER(BeamParams), _I, _I, _P]),
     "sv_beam_state_read_host": (C.c_int, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I), C.POINTER(C.c_float)]),
+    "sv_beam_state_read16_host": (C.c_int, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I), C.POINTER(C.c_float),
+                                            C.POINTER(C.c_float)]),
     "sv_beam_row_candidates_host": (C.c_int, [C.POINTER(BeamParams), C.POINTER(C.c_float), _I, C.POINTER(_I), _I, _F, _I, _I,
                                               C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(_I)]),
     "sv_beam_step_host": (C.c_int, [C.POINTER(BeamParams), _I, _I, _I, _P, C.POINTER(C.c_float), C.POINTER(C.c_float),

@@ -39,7 +39,7 @@ class ModelDims:
     vocab: int = 49156
     ln_eps: float = 1e-5
     # engine capacity
-    max_batch: int = 8
+    max_batch: int = 8            # cache rows (images x beams / completions) per GPU, 1..16
     max_len: int = 8192           # KV-cache capacity in tokens (<= n_positions for v1)
     # v2 (SigLIP + StarCoder2) only
     rope_theta: float = 0.0       # 0 = learned absolute positions (v1)

@@ -339,9 +339,9 @@ static svbeam::Params params_from_abi(const sv_beam_params* bp, int32_t batch, i
   return p;
 }
 
-int sv_beam_params_check(const sv_beam_params* bp, int32_t batch) {
-  if (!bp || batch < 1) return SV_ERR_INVALID;
-  if (bp->num_beams < 2 || batch * bp->num_beams > svbeam::kMaxRows) return SV_ERR_INVALID;
+int sv_beam_params_check_rows(const sv_beam_params* bp, int32_t batch, int32_t max_rows) {
+  if (!bp || batch < 1 || max_rows < 1 || max_rows > svbeam::kMaxRows) return SV_ERR_INVALID;
+  if (bp->num_beams < 2 || batch * bp->num_beams > max_rows || 2 * bp->num_beams > svbeam::kMaxK) return SV_ERR_INVALID;
   if (bp->max_new_tokens < 1 || bp->n_stop_ids < 0 || bp->n_stop_ids > svbeam::kMaxStop) return SV_ERR_INVALID;
   if (bp->early_stopping < 0 || bp->early_stopping > 2) return SV_ERR_INVALID;
   if (bp->do_sample && !(bp->temperature > 0.f)) return SV_ERR_INVALID;
@@ -349,10 +349,12 @@ int sv_beam_params_check(const sv_beam_params* bp, int32_t batch) {
   return SV_OK;
 }
 
+int sv_beam_params_check(const sv_beam_params* bp, int32_t batch) { return sv_beam_params_check_rows(bp, batch, 8); }
+
 int sv_beam_state_bytes(void) { return (int)sizeof(svbeam::State); }
 
 int sv_beam_state_init_host(const sv_beam_params* bp, int32_t batch, int32_t first_cache_pos, void* state) {
-  if (sv_beam_params_check(bp, batch) != SV_OK || !state) return SV_ERR_INVALID;
+  if (sv_beam_params_check_rows(bp, batch, svbeam::kMaxRows) != SV_OK || !state) return SV_ERR_INVALID;
   svbeam::Params p = params_from_abi(bp, batch, 8, bp->max_new_tokens);
   svbeam::init_state(p, *reinterpret_cast<svbeam::State*>(state), first_cache_pos);
   return SV_OK;
@@ -409,11 +411,14 @@ int sv_beam_row_candidates_host(const sv_beam_params* bp, const float* logits, i
 
 // One bookkeeping step on the host: row candidates [batch * num_beams][K] -> merged -> beam_step.  `state` is the opaque
 // State blob; run_seq / fin_seq are the double-buffered sequence arrays [2][batch * num_beams][seq_stride].  plan_out (optional)
-// receives the Plan as int32 [sizeof(Plan) / 4].  Returns 1 while the search continues, 0 when it is over, < 0 on error.
+// receives the plan of rows 0-7 as int32 [7 * 8 + 3]: run_parent, run_tok, fin_old, fin_parent, fin_tok, copy_src, copy_lo
+// (8 entries each), copy_hi, cont, old_len; it must be NULL above 8 rows.  Returns 1 while the search continues, 0 when it
+// is over, < 0 on error.
 int sv_beam_step_host(const sv_beam_params* bp, int32_t batch, int32_t vocab, int32_t seq_stride, void* state,
                       const float* cand_key, const float* cand_val, const int32_t* cand_tok, int32_t* run_seq,
                       int32_t* fin_seq, int32_t cache_hi, int32_t* next_tokens, int32_t* src_rows, int32_t* plan_out) {
-  if (sv_beam_params_check(bp, batch) != SV_OK || !state || !cand_key || !cand_val || !cand_tok || !run_seq || !fin_seq)
+  if (sv_beam_params_check_rows(bp, batch, svbeam::kMaxRows) != SV_OK || !state || !cand_key || !cand_val || !cand_tok ||
+      !run_seq || !fin_seq || (plan_out && batch * bp->num_beams > 8))
     return SV_ERR_INVALID;
   svbeam::Params p = params_from_abi(bp, batch, vocab, seq_stride);
   svbeam::State& s = *reinterpret_cast<svbeam::State*>(state);
@@ -444,7 +449,11 @@ int sv_beam_step_host(const sv_beam_params* bp, int32_t batch, int32_t vocab, in
     if (next_tokens) next_tokens[r] = plan.run_tok[r];
     if (src_rows) src_rows[r] = plan.run_parent[r];
   }
-  if (plan_out) memcpy(plan_out, &plan, sizeof(plan));
+  if (plan_out) {
+    const int32_t* rows[7] = {plan.run_parent, plan.run_tok, plan.fin_old, plan.fin_parent, plan.fin_tok, plan.copy_src, plan.copy_lo};
+    for (int a = 0; a < 7; ++a) memcpy(plan_out + 8 * a, rows[a], 8 * sizeof(int32_t));
+    plan_out[56] = plan.copy_hi; plan_out[57] = plan.cont; plan_out[58] = plan.old_len;
+  }
   return plan.cont;
 }
 
@@ -454,9 +463,24 @@ int sv_beam_state_read_host(const void* state, int32_t* parity, int32_t* cur_len
   const svbeam::State& s = *reinterpret_cast<const svbeam::State*>(state);
   if (parity) *parity = s.parity;
   if (cur_len) *cur_len = s.cur_len;
-  for (int r = 0; r < svbeam::kMaxRows; ++r) {
+  for (int r = 0; r < 8; ++r) {
     if (fin_len8) fin_len8[r] = s.fin_len[r];
     if (beam_scores8) beam_scores8[r] = s.beam_scores[r];
+  }
+  return SV_OK;
+}
+
+// The same for all 16 rows, with the running scores.
+int sv_beam_state_read16_host(const void* state, int32_t* parity, int32_t* cur_len, int32_t* fin_len16, float* beam_scores16,
+                              float* running_scores16) {
+  if (!state) return SV_ERR_INVALID;
+  const svbeam::State& s = *reinterpret_cast<const svbeam::State*>(state);
+  if (parity) *parity = s.parity;
+  if (cur_len) *cur_len = s.cur_len;
+  for (int r = 0; r < svbeam::kMaxRows; ++r) {
+    if (fin_len16) fin_len16[r] = s.fin_len[r];
+    if (beam_scores16) beam_scores16[r] = s.beam_scores[r];
+    if (running_scores16) running_scores16[r] = s.running_scores[r];
   }
   return SV_OK;
 }

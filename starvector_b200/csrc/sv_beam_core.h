@@ -4,7 +4,7 @@
 // starvector_v2.py:53-57 -> HF defaults), restated from the installed transformers 5.5 (generation/utils.py
 // `_get_top_k_continuations`, `_get_running_beams_for_next_iteration`, `_update_finished_beams`,
 // `_check_early_stop_heuristic`, `_beam_search_has_unfinished_sequences`) exactly as starvector_b200/beam_search.py
-// does with torch ops -- that file is this one's oracle.  Plain scalar code over <= 8 cache rows and <= 16 candidates.
+// does with torch ops -- that file is this one's oracle.  Plain scalar code over <= 16 cache rows and <= 16 candidates.
 //
 // Everything is in GENERATED-token coordinates (prompt_len = 0: the reference calls generate(inputs_embeds=...)).
 // fp32 arithmetic and its order follow the torch expressions (a python scalar operand is an fp32 scalar there).
@@ -20,7 +20,7 @@
 
 namespace svbeam {
 
-constexpr int kMaxRows = 8;      // image rows of the engine = batch * num_beams
+constexpr int kMaxRows = 16;     // image rows of the engine = batch * num_beams
 constexpr int kMaxK = 16;        // beams_to_keep = max(2, 1 + n_eos) * num_beams = 2 * num_beams
 constexpr int kMaxStop = 8;
 constexpr float kNegBig = -1.0e9f;
@@ -84,8 +84,10 @@ SVB_HD float philox_u01(unsigned long long seed, uint32_t c0, uint32_t c1) {
 }
 // Gumbel(0,1) for (step, row, token): sorting `score + gumbel` in descending order draws WITHOUT replacement from
 // softmax(score) in exactly the order sequential sampling would (Plackett-Luce) = torch.multinomial(softmax, K).
+// Counter: (token + (row / 8) * 2^24, step * 8 + row % 8).  Rows 0-7 draw what they drew when the engine held 8 rows, rows
+// 8-15 are told apart through the first word (vocabularies are < 2^24, the engine takes <= 2^20).
 SVB_HD float gumbel_noise(unsigned long long seed, int step, int row, int token) {
-  const float u = philox_u01(seed, (uint32_t)token, (uint32_t)(step * kMaxRows + row));
+  const float u = philox_u01(seed, (uint32_t)token + ((uint32_t)(row >> 3) << 24), (uint32_t)(step * 8 + (row & 7)));
   return -logf(-logf(u));
 }
 // log-softmax value -> RepetitionPenaltyLogitsProcessor (on log-probs, generated ids only) -> TemperatureLogitsWarper

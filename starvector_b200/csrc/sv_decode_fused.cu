@@ -30,7 +30,7 @@ static void launch_ex(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem
 // full bf16 logits row is scanned (penalty changes the order).  Semantics: SURVEY.md App. B.3-6.
 __global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restrict__ logits, int vocab, int batch,
                                                             const float* __restrict__ amax_val,
-                                                            const int* __restrict__ amax_idx, int ntiles,
+                                                            const int* __restrict__ amax_idx, int ntiles, int amax_stride,
                                                             GenState* state, const GenParamsDev* __restrict__ p,
                                                             uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
                                                             int advance_len, const bf16* __restrict__ wte,
@@ -40,7 +40,7 @@ __global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restri
   pdl_wait();
   if (state->done) return;
   __shared__ AmaxPair sm[32];
-  __shared__ int s_tok[8];
+  __shared__ int s_tok[16];
   const int tid = threadIdx.x;
   const float rp = p->rep_penalty;
   const bool use_partials = (rp == 1.0f) && amax_val != nullptr;
@@ -48,8 +48,8 @@ __global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restri
     AmaxPair best{-INFINITY, 0x7fffffff};
     if (use_partials) {
       for (int i = tid; i < ntiles; i += 1024) {
-        const float v = __ldcg(amax_val + (int64_t)i * 8 + b);
-        const int id = __ldcg(amax_idx + (int64_t)i * 8 + b);
+        const float v = __ldcg(amax_val + (int64_t)i * amax_stride + b);
+        const int id = __ldcg(amax_idx + (int64_t)i * amax_stride + b);
         best = amax_better(best, AmaxPair{v, id});
       }
     } else {
@@ -97,11 +97,11 @@ __global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restri
 }
 
 void launch_select_fused(const bf16* logits, int vocab, int batch, const float* amax_val, const int* amax_idx,
-                         int ntiles, GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
+                         int ntiles, int amax_stride, GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
                          int32_t* out_ids, int advance_len, const bf16* wte, const bf16* wpe, bf16* x, int h,
                          int n_positions, bool pdl, cudaStream_t st) {
   launch_ex(select_fused_kernel, dim3(1), dim3(1024), 0, st, pdl, logits, vocab, batch, amax_val, amax_idx, ntiles,
-            state, params, seen, next_ids, out_ids, advance_len, wte, wpe, x, h, n_positions);
+            amax_stride, state, params, seen, next_ids, out_ids, advance_len, wte, wpe, x, h, n_positions);
 }
 
 }  // namespace sv

@@ -1,11 +1,11 @@
 // Per-phase decode GEMV on a shared-memory weight ring (the kernels of the CUDA-graph decode step):
-//   Y[B,N] = epilogue( LayerNorm?(X)[B,K] . W[N,K]^T ),  B <= 8 image rows, one CTA per SM.
+//   Y[B,N] = epilogue( LayerNorm?(X)[B,K] . W[N,K]^T ),  B <= 16 image rows (one or two groups of 8), one CTA per SM.
 //
 //   warp 8 (producer, one elected lane per row): copies [R rows x 1024 k] weight slabs into a 5-slot shared-memory ring with
 //       cp.async.bulk (completion on the slot's "full" mbarrier).  It starts BEFORE the programmatic-dependency wait --
 //       weights are immutable -- so ~165 KB per SM of HBM reads are in flight while the previous kernel drains.
 //   warps 0-7 (consumers): LayerNorm prologue on register-resident activation fragments, 128-bit MMA fragments from the slot
-//       (row pitch = 2 KB + 64 B, bank-conflict free), mma.sync m16n8k16 (weights = A, the <= 8 image rows = B), slot
+//       (row pitch = 2 KB + 64 B, bank-conflict free), mma.sync m16n8k16 (weights = A, each group of <= 8 image rows = B), slot
 //       release ("empty" mbarrier, one arrive per warp), deterministic cross-warp split-K reduction and the reference's
 //       bf16 epilogue (bias, gelu, residual, KV-cache append, argmax partials).
 //
@@ -29,8 +29,8 @@ struct Ctx {
   const Args* a;
   uint8_t* smem;
   int cta, ncta, warp, lane, g, t;
-  float* red;     // [2][NWC][16][8]
-  float* stat;    // [NWC][8]
+  float* red;     // [2][NWC][16][8 * NG]
+  float* stat;    // [NWC][8 * NG]
   // optional (per-phase ring kernels): parameters staged into shared memory BEFORE the programmatic-dependency wait, so that
   // their HBM misses overlap the previous kernel's tail instead of sitting on this kernel's critical path
   uint32_t ln_s = 0;            // shared address of [ln_w row | ln_b row] (K bf16 each), 0 = read them from global
@@ -320,6 +320,288 @@ SV_DEVINL void gemv_phase(const Ctx& cx, Ring& r, const bf16* __restrict__ X, co
 }
 
 
+// ---- the same phase over NG groups of 8 image rows (NG = 2: 9-16 rows).  Lane (g, t) feeds the activation fragments of
+// rows g and g + 8 to the MMAs, and every weight fragment read from a ring slot feeds NG MMAs, so all rows share one weight
+// stream.  Group 0's fragments live in registers as in gemv_phase; group gi > 0 keeps its fragments in shared memory at
+// x1_s (fragment i of consumer thread c at x1_s + ((gi - 1) * 2 * CPW + i) * NCT * 16 + c * 16: adjacent lanes, adjacent
+// 16 bytes), which keeps the kernel inside the 168 registers a 288-thread CTA can have without spilling.
+// Kept apart from gemv_phase so that the 8-row kernels compile to exactly the instructions they had; the K > 2048
+// LayerNorm path (v2, which decodes through the per-op kernels above 8 rows) is not part of it.
+SV_DEVINL void sts16(uint32_t addr, const uint4& v) {
+  asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+template <bool HAS_LN, int EPI, int NG>
+SV_DEVINL void gemv_phase_wide(const Ctx& cx, Ring& r, const bf16* __restrict__ X, const bf16* __restrict__ bias,
+                          const bf16* res, bf16* Y, int N, int K, int act, const bf16* __restrict__ ln_w,
+                          const bf16* __restrict__ ln_b, const Layer* L, uint32_t x1_s) {
+  static_assert(NG == 1 || NG == 2, "8 or 16 image rows");
+  constexpr int MR = 8 * NG;                         // image rows of the split-K buffer, the statistics and the partials
+  const Args& a = *cx.a;
+  const Plan p = make_plan(N, K, cx.cta, cx.ncta);
+  const int warp = cx.warp, g = cx.g, t = cx.t;
+  const int cps = p.KS >> 5;                         // 32-wide chunks per slot row
+  const int cpws = (cps + NWC - 1) / NWC;            // chunks per warp per slot (<= CPW)
+  bool row_ok[NG];
+  const bf16* xp[NG];
+#pragma unroll
+  for (int gi = 0; gi < NG; ++gi) {
+    row_ok[gi] = g + 8 * gi < a.B;
+    xp[gi] = X + (int64_t)(row_ok[gi] ? g + 8 * gi : 0) * K + 8 * t;
+  }
+  const bool big_k = p.nstg > 2;
+
+  // activations for the whole phase stay on chip when K <= 2048 (8 fragments per lane and row group)
+  uint4 xr[2 * CPW];
+#pragma unroll
+  for (int i = 0; i < 2 * CPW; ++i) xr[i] = make_uint4(0u, 0u, 0u, 0u);
+  const uint32_t xs = x1_s + (uint32_t)threadIdx.x * 16;
+  auto xget = [&](int gi, int i) -> uint4 { return gi == 0 ? xr[i] : lds16(xs + ((gi - 1) * 2 * CPW + i) * NCT * 16); };
+  auto xset = [&](int gi, int i, const uint4& v) {
+    if (gi == 0) xr[i] = v;
+    else sts16(xs + ((gi - 1) * 2 * CPW + i) * NCT * 16, v);
+  };
+  if (!big_k && p.ntile > 0) {
+#pragma unroll
+    for (int gi = 0; gi < NG; ++gi) {
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) {
+#pragma unroll
+        for (int j = 0; j < CPW; ++j) {
+          const int cl = warp + NWC * j;
+          const bool okc = ks < p.nstg && j < cpws && cl < cps;
+          if (gi == 0) {
+            if (okc && row_ok[gi]) xr[ks * CPW + j] = ldcg16(xp[gi] + (ks * cps + cl) * 32);
+          } else {                                     // every slot is written: the LayerNorm sums read all of them
+            xset(gi, ks * CPW + j, (okc && row_ok[gi]) ? ldcg16(xp[gi] + (ks * cps + cl) * 32) : make_uint4(0u, 0u, 0u, 0u));
+          }
+        }
+      }
+    }
+    if constexpr (HAS_LN) {
+#pragma unroll
+      for (int gi = 0; gi < NG; ++gi) {
+        float s = 0.f;
+#pragma unroll
+        for (int i = 0; i < 2 * CPW; ++i) {
+          float f[8];
+          unpack8(xget(gi, i), f);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) s += f[j];
+        }
+        s = quad_sum(s);
+        if (t == 0) cx.stat[warp * MR + 8 * gi + g] = s;
+      }
+      consumer_sync();
+      float mean[NG];
+#pragma unroll
+      for (int gi = 0; gi < NG; ++gi) {
+        mean[gi] = 0.f;
+#pragma unroll
+        for (int w = 0; w < NWC; ++w) mean[gi] += cx.stat[w * MR + 8 * gi + g];
+        mean[gi] /= (float)K;
+      }
+      float q[NG];
+#pragma unroll
+      for (int gi = 0; gi < NG; ++gi) {
+        q[gi] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < 2; ++ks) {
+#pragma unroll
+          for (int j = 0; j < CPW; ++j) {
+            const bool okc = ks < p.nstg && j < cpws && (warp + NWC * j) < cps;
+            if (okc) {
+              float f[8];
+              unpack8(xget(gi, ks * CPW + j), f);
+#pragma unroll
+              for (int e = 0; e < 8; ++e) { const float dlt = f[e] - mean[gi]; q[gi] += dlt * dlt; }
+            }
+          }
+        }
+        q[gi] = quad_sum(q[gi]);
+      }
+      consumer_sync();
+#pragma unroll
+      for (int gi = 0; gi < NG; ++gi)
+        if (t == 0) cx.stat[warp * MR + 8 * gi + g] = q[gi];
+      consumer_sync();
+      float rstd[NG];
+#pragma unroll
+      for (int gi = 0; gi < NG; ++gi) {
+        float var = 0.f;
+#pragma unroll
+        for (int w = 0; w < NWC; ++w) var += cx.stat[w * MR + 8 * gi + g];
+        rstd[gi] = 1.0f / sqrtf(var / (float)K + a.ln_eps);
+      }
+      // (the weight ring keeps HBM busy on its own, so the LN affine is fetched late to save registers)
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) {
+#pragma unroll
+        for (int j = 0; j < CPW; ++j) {
+          const int cl = warp + NWC * j;
+          const bool okc = ks < p.nstg && j < cpws && cl < cps;
+          float wf[8], bfv[8];
+          const int ch = okc ? ks * cps + cl : 0;
+          if (cx.ln_s) {
+            unpack8(lds16(cx.ln_s + (ch * 32 + 8 * t) * 2), wf);
+            unpack8(lds16(cx.ln_s + (K + ch * 32 + 8 * t) * 2), bfv);
+          } else {
+            unpack8(ldg_cached(ln_w + ch * 32 + 8 * t), wf);
+            unpack8(ldg_cached(ln_b + ch * 32 + 8 * t), bfv);
+          }
+#pragma unroll
+          for (int gi = 0; gi < NG; ++gi) {
+            float f[8];
+            unpack8(xget(gi, ks * CPW + j), f);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) f[e] = (row_ok[gi] && okc) ? (f[e] - mean[gi]) * rstd[gi] * wf[e] + bfv[e] : 0.f;
+            xset(gi, ks * CPW + j, pack8(f));   // ln output is a bf16 tensor in the reference; 0 on padded chunks
+          }
+        }
+      }
+    }
+  }
+
+  float c[NG][4];
+#pragma unroll
+  for (int gi = 0; gi < NG; ++gi) { c[gi][0] = 0.f; c[gi][1] = 0.f; c[gi][2] = 0.f; c[gi][3] = 0.f; }
+  int pos_now = 0;
+  if constexpr (EPI == EPI_QKV) pos_now = __ldcg(&a.state->cur_len);         // read here, not behind the last MMA
+  for (int tl = 0; tl < p.ntile; ++tl) {
+    const int tile = p.tile0 + tl;
+    // the epilogue thread's residual value: requested now, used after the MMAs (an L2 round trip off the tail)
+    float res_pre = 0.f;
+    {
+      const int n_ = threadIdx.x & 15, mm_ = threadIdx.x >> 4, col_ = tile * p.R + n_;
+      if (res != nullptr && threadIdx.x < 16 * MR && n_ < p.R && col_ < N && mm_ < a.B) res_pre = __bfloat162float(__ldcg(res + (int64_t)mm_ * N + col_));
+    }
+    if (!big_k) {
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) {
+        if (ks < p.nstg) {
+          mbar_wait(r.full0 + 8u * r.slot, r.phase);
+          const uint32_t sb = r.base + r.slot * SLOT_BYTES + g * p.pitch + t * 16;
+#pragma unroll
+          for (int j = 0; j < CPW; ++j) {
+            const int cl = warp + NWC * j;
+            if (j < cpws && cl < cps) {
+              const uint4 lo = lds16(sb + cl * 64), hi = lds16(sb + 8 * p.pitch + cl * 64);
+#pragma unroll
+              for (int gi = 0; gi < NG; ++gi) {
+                const uint4 xv = xget(gi, ks * CPW + j);
+                mma_bf16_16816(c[gi], lo.x, hi.x, lo.y, hi.y, xv.x, xv.y);
+                mma_bf16_16816(c[gi], lo.z, hi.z, lo.w, hi.w, xv.z, xv.w);
+              }
+            }
+          }
+          __syncwarp();
+          if (cx.lane == 0) mbar_arrive(r.empty0 + 8u * r.slot);
+          r.advance();
+        }
+      }
+    } else {
+      // K > 2048 without LayerNorm (fc2): activation fragments are fetched per slab from L2, one slab ahead of their use
+      uint4 xc[NG][CPW], xn[NG][CPW];
+      auto fetch = [&](int ks) {
+#pragma unroll
+        for (int j = 0; j < CPW; ++j) {
+          const int cl = warp + NWC * j;
+          const bool okc = ks < p.nstg && j < cpws && cl < cps;
+          const int ch = okc ? ks * cps + cl : 0;
+#pragma unroll
+          for (int gi = 0; gi < NG; ++gi)
+            xn[gi][j] = (row_ok[gi] && okc) ? ldcg16(xp[gi] + ch * 32) : make_uint4(0u, 0u, 0u, 0u);
+        }
+      };
+      auto promote = [&]() {                   // xn (raw) -> xc (what the MMAs consume)
+#pragma unroll
+        for (int j = 0; j < CPW; ++j)
+#pragma unroll
+          for (int gi = 0; gi < NG; ++gi) xc[gi][j] = xn[gi][j];
+      };
+      fetch(0);
+      promote();
+      for (int ks = 0; ks < p.nstg; ++ks) {
+        fetch(ks + 1);
+        mbar_wait(r.full0 + 8u * r.slot, r.phase);
+        const uint32_t sb = r.base + r.slot * SLOT_BYTES + g * p.pitch + t * 16;
+#pragma unroll
+        for (int j = 0; j < CPW; ++j) {
+          const int cl = warp + NWC * j;
+          if (j < cpws && cl < cps) {
+            const uint4 lo = lds16(sb + cl * 64), hi = lds16(sb + 8 * p.pitch + cl * 64);
+#pragma unroll
+            for (int gi = 0; gi < NG; ++gi) {
+              mma_bf16_16816(c[gi], lo.x, hi.x, lo.y, hi.y, xc[gi][j].x, xc[gi][j].y);
+              mma_bf16_16816(c[gi], lo.z, hi.z, lo.w, hi.w, xc[gi][j].z, xc[gi][j].w);
+            }
+          }
+        }
+        __syncwarp();
+        if (cx.lane == 0) mbar_arrive(r.empty0 + 8u * r.slot);
+        r.advance();
+        promote();
+      }
+    }
+    // ---- tile finished: deterministic cross-warp split-K reduction + epilogue
+    // red[tl & 1][warp][16 weight rows][MR image rows]; c[gi] holds image columns 8 * gi + 2t, 8 * gi + 2t + 1
+    float* rd = cx.red + (tl & 1) * (NWC * 16 * MR);
+#pragma unroll
+    for (int gi = 0; gi < NG; ++gi) {
+      rd[(warp * 16 + g) * MR + 8 * gi + 2 * t] = c[gi][0]; rd[(warp * 16 + g) * MR + 8 * gi + 2 * t + 1] = c[gi][1];
+      rd[(warp * 16 + g + 8) * MR + 8 * gi + 2 * t] = c[gi][2]; rd[(warp * 16 + g + 8) * MR + 8 * gi + 2 * t + 1] = c[gi][3];
+      c[gi][0] = c[gi][1] = c[gi][2] = c[gi][3] = 0.f;
+    }
+    consumer_sync();
+    if (threadIdx.x < 16 * MR) {
+      const int n = threadIdx.x & 15, mm = threadIdx.x >> 4;
+      float acc = 0.f;
+#pragma unroll
+      for (int w = 0; w < NWC; ++w) acc += rd[(w * 16 + n) * MR + mm];
+      const int col = tile * p.R + n;
+      const bool ok = n < p.R && col < N && mm < a.B;
+      float v = 0.f, v_bf = 0.f;          // v_bf: the value as the bf16 logits tensor holds it
+      if (ok) {
+        const float bv = bias ? (cx.bias_s ? cx.bias_s[tl * 16 + n] : __bfloat162float(bias[col])) : 0.f;
+        const float rv = res_pre;
+        v = epilogue_elem(acc, bv, act, res != nullptr, rv);
+        const bf16 vb = __float2bfloat16_rn(v);
+        v_bf = __bfloat162float(vb);
+        Y[(int64_t)mm * N + col] = vb;
+        if constexpr (EPI == EPI_QKV) {
+          const int q_cols = a.n_head * D, j = col - q_cols;
+          const int pos = pos_now;
+          if (j >= 0 && pos < a.tcap) {
+            if (j < a.n_kv * D) {
+              const int kvh = j / D, dim = j % D;
+              L->kc[(((int64_t)mm * a.n_kv + kvh) * a.tcap + pos) * D + dim] = vb;
+            } else {
+              const int jj = j - a.n_kv * D, kvh = jj / D, dim = jj % D;
+              L->vc[(((int64_t)mm * a.n_kv + kvh) * D + dim) * a.tcap + pos] = vb;
+            }
+          }
+        }
+      }
+      if constexpr (EPI == EPI_LMHEAD) {
+        // greedy = argmax over the bf16 logits cast to float, lowest index wins ties (HF _sample): reduce the ROUNDED value
+        float bv = ok ? v_bf : -INFINITY;
+        int bi = ok ? col : 0x7fffffff;
+#pragma unroll
+        for (int o = 1; o < 16; o <<= 1) {
+          const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+          const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+        }
+        if (n == 0 && mm < a.B) {          // partials [tile][MR]: the row stride is the launch's 8 * NG
+          a.amax_val[(int64_t)tile * MR + mm] = bv;
+          a.amax_idx[(int64_t)tile * MR + mm] = bi;
+        }
+      }
+    }
+    // red[] is double-buffered by tile parity: one barrier per tile
+  }
+}
+
+
 // ------------------------------------------------------------------------------------------
 // One-phase kernels of the per-phase CUDA-graph decode path: a producer warp
 // streams this GEMV's slabs through shared memory (starting before the PDL dependency wait, weights
@@ -356,18 +638,21 @@ SV_DEVINL void l2_prefetch_kv(const bf16* kc, const bf16* vc, int nkeys, int nbk
   if (acc == 0x9e3779b9u && nkeys < 0) asm volatile("trap;");     // (never: keeps the loads' results alive)
 }
 constexpr int RING_BIAS_TILES = 8;     // biases staged for up to this many tiles per CTA (mlp.c_fc has 4)
-SV_DEVINL constexpr int ring_smem_bytes(int nslots) {
-  return nslots * SLOT_BYTES + RED_BYTES + NWC * 8 * 4 + 2 * 8 * 8 + 16 + 2 * 2 * KS_MAX * 2 + RING_BIAS_TILES * 16 * 4 + 256;
+constexpr int X1_BYTES = 2 * CPW * NCT * 16;  // activation fragments of one more row group (gemv_phase_wide), 32 KB
+SV_DEVINL constexpr int ring_smem_bytes(int nslots, int ng) {
+  return nslots * SLOT_BYTES + ng * RED_BYTES + NWC * 8 * ng * 4 + 2 * 8 * 8 + 16 + 2 * 2 * KS_MAX * 2 + RING_BIAS_TILES * 16 * 4 +
+         (ng - 1) * X1_BYTES + 256;
 }
+// 222.4 KB with 5 slots: the 16-row kernel keeps the ring depth of the 8-row one within the 227 KB a CTA may opt in to
+static_assert(ring_smem_bytes(STAGES, 2) <= 227 * 1024, "the 16-row ring kernel must fit the opt-in shared memory");
 
-// (A 2-CTA/SM register budget (96 regs) so that consecutive kernels co-reside under PDL was measured 25% slower.)
-template <bool HAS_LN, int EPI, bool LN_BIGK = false>
-__global__ void __launch_bounds__(NTHREADS, RING_MINBLOCKS) gemv_ring_kernel(const RingGemvArgs ra) {
+template <bool HAS_LN, int EPI, bool LN_BIGK, int NG>
+SV_DEVINL void gemv_ring_body(const RingGemvArgs& ra) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~(uintptr_t)127);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int cta = blockIdx.x, ncta = gridDim.x;
-  const int off_red = ra.nslots * SLOT_BYTES, off_stat = off_red + RED_BYTES, off_bar = off_stat + NWC * 8 * 4;
+  const int off_red = ra.nslots * SLOT_BYTES, off_stat = off_red + NG * RED_BYTES, off_bar = off_stat + NWC * 8 * NG * 4;
   Ring ring;
   ring.base = smem_u32(smem);
   ring.full0 = smem_u32(smem + off_bar);
@@ -413,23 +698,44 @@ __global__ void __launch_bounds__(NTHREADS, RING_MINBLOCKS) gemv_ring_kernel(con
     }
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  gemv_phase<HAS_LN, EPI, LN_BIGK>(cx, ring, ra.X, ra.bias, ra.res, ra.Y, ra.N, ra.K, ra.act, ra.ln_w, ra.ln_b, &ra.L);
+  if constexpr (NG == 1)
+    gemv_phase<HAS_LN, EPI, LN_BIGK>(cx, ring, ra.X, ra.bias, ra.res, ra.Y, ra.N, ra.K, ra.act, ra.ln_w, ra.ln_b, &ra.L);
+  else
+    gemv_phase_wide<HAS_LN, EPI, NG>(cx, ring, ra.X, ra.bias, ra.res, ra.Y, ra.N, ra.K, ra.act, ra.ln_w, ra.ln_b, &ra.L,
+                                     smem_u32(smem + ((off_bar + 2 * 8 * 8 + 15) & ~15) + 2 * 2 * KS_MAX * 2 + RING_BIAS_TILES * 16 * 4));
+}
+
+// (A 2-CTA/SM register budget (96 regs) so that consecutive kernels co-reside under PDL was measured 25% slower.)
+template <bool HAS_LN, int EPI, bool LN_BIGK = false>
+__global__ void __launch_bounds__(NTHREADS, RING_MINBLOCKS) gemv_ring_kernel(const RingGemvArgs ra) {
+  gemv_ring_body<HAS_LN, EPI, LN_BIGK, 1>(ra);
+}
+
+// 9-16 image rows.  168 registers is the most a 288-thread CTA can have (Hopper charges registers to warps in groups of
+// four: 9 warps count as 12), and the second row group's fragments in registers would need ~184, so they are kept in
+// shared memory instead (gemv_phase_wide): no local memory.
+template <bool HAS_LN, int EPI>
+__global__ void __launch_bounds__(NTHREADS, 1) gemv_ring16_kernel(const RingGemvArgs ra) {
+  gemv_ring_body<HAS_LN, EPI, false, 2>(ra);
 }
 
 }  // namespace mega
 
 // ---- host side
 // ---- per-phase ring GEMV launchers (used by the CUDA-graph decode path)
-template <bool HAS_LN, int EPI, bool LN_BIGK = false>
+template <bool HAS_LN, int EPI, bool LN_BIGK = false, int NG = 1>
 static void launch_ring_t(const mega::RingGemvArgs& ra, int ncta, bool pdl, cudaStream_t st) {
+  void (*kern)(const mega::RingGemvArgs);
+  if constexpr (NG == 1) kern = mega::gemv_ring_kernel<HAS_LN, EPI, LN_BIGK>;
+  else kern = mega::gemv_ring16_kernel<HAS_LN, EPI>;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(ncta); cfg.blockDim = dim3(mega::NTHREADS); cfg.stream = st;
-  cfg.dynamicSmemBytes = mega::ring_smem_bytes(ra.nslots);
+  cfg.dynamicSmemBytes = mega::ring_smem_bytes(ra.nslots, NG);
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, mega::gemv_ring_kernel<HAS_LN, EPI, LN_BIGK>, ra);
+  cudaLaunchKernelEx(&cfg, kern, ra);
   count_launch();
 }
 
@@ -437,6 +743,9 @@ cudaError_t gemv_ring_init() {   // set the shared-memory opt-in outside of any 
   cudaError_t e;
 #define SV_RING_ATTR(LN, EPI)                                                                                          \
   e = cudaFuncSetAttribute(mega::gemv_ring_kernel<LN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, mega::SMEM_BYTES); \
+  if (e != cudaSuccess) return e;                                                                                      \
+  e = cudaFuncSetAttribute(mega::gemv_ring16_kernel<LN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,                \
+                           mega::ring_smem_bytes(mega::STAGES, 2));                                                   \
   if (e != cudaSuccess) return e;
   SV_RING_ATTR(true, mega::EPI_QKV) SV_RING_ATTR(true, mega::EPI_PLAIN) SV_RING_ATTR(true, mega::EPI_LMHEAD)
   SV_RING_ATTR(false, mega::EPI_PLAIN)
@@ -449,6 +758,9 @@ cudaError_t gemv_ring_init() {   // set the shared-memory opt-in outside of any 
 }
 
 bool gemv_ring_supported(int K, bool has_ln) { (void)has_ln; return K >= 32 && K % 32 == 0; }
+
+// The 16-row kernels' epilogue gives one (weight row, image row) pair of a 16 x 16 tile to each consumer thread.
+int gemv_ring_max_rows() { return mega::NCT >= 256 ? 16 : 8; }
 
 // CTAs of one ring GEMV: one per SM in every build.  With RING_MINBLOCKS = 2 the CTA is small enough for two per SM, and
 // the second slot is deliberately left free: it is where the NEXT kernel's CTA (launched early through PDL) becomes
@@ -482,12 +794,24 @@ void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st) {
     for (int c : {1024, 768, 512, 256, 128, 64}) if (c <= g.K && g.K % c == 0) { ks = c; break; }
     const int need = tpc * (g.K / ks);
     ra.nslots = need < cap ? need : cap;
+    if (ring_row_groups(g.B) == 2 && ra.nslots > mega::STAGES) ra.nslots = mega::STAGES;   // + 32 KB of fragments must fit
     if (ra.nslots < 1) ra.nslots = 1;
   }
   const bool ln = g.ln_w != nullptr;
-  if (ln && g.K > 2 * mega::KS_MAX) {       // LayerNorm over K > 2048 (v2): separate instantiations
+  if (ln && g.K > 2 * mega::KS_MAX) {       // LayerNorm over K > 2048 (v2): separate instantiations, 8 rows only
+    if (ring_row_groups(g.B) != 1) {          // sv_engine_create keeps such engines off this path above 8 rows
+      fprintf(stderr, "starvector_b200: LayerNorm GEMV with K = %d over %d rows has no ring kernel\n", g.K, g.B);
+      abort();
+    }
     if (g.epi == mega::EPI_LMHEAD) launch_ring_t<true, mega::EPI_LMHEAD, true>(ra, nsm, g.pdl, st);
     else launch_ring_t<true, mega::EPI_PLAIN, true>(ra, nsm, g.pdl, st);
+    return;
+  }
+  if (ring_row_groups(g.B) == 2) {           // 9-16 rows: two row groups share each weight fragment
+    if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV, false, 2>(ra, nsm, g.pdl, st);
+    else if (ln && g.epi == mega::EPI_LMHEAD) launch_ring_t<true, mega::EPI_LMHEAD, false, 2>(ra, nsm, g.pdl, st);
+    else if (ln) launch_ring_t<true, mega::EPI_PLAIN, false, 2>(ra, nsm, g.pdl, st);
+    else launch_ring_t<false, mega::EPI_PLAIN, false, 2>(ra, nsm, g.pdl, st);
     return;
   }
   if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV>(ra, nsm, g.pdl, st);

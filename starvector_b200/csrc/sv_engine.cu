@@ -82,7 +82,7 @@ struct sv_engine {
   long long* mega_dbg = nullptr;
   bool mega_debug = false;
   // dataflow persistent decode kernel (sv_decode_flow.cu): flagged exchange buffers in one allocation
-  bool use_flow = false, flow_realloc = false;
+  bool use_flow = false, flow_realloc = false, flow_requested = false;
   bool use_tiles = false;           // slab-tiled weight copies exist (the dataflow kernel streams them)
   bool ring_tiles = false;          // SV_TILED=1: the ring GEMVs of the graph path stream them too
   uint8_t* flow_mem = nullptr;
@@ -341,8 +341,8 @@ bool build_buffers(sv_engine* e) {
   AL(d_x, B * H); AL(d_ln, B * H); AL(d_qkv, B * e->qkv_cols); AL(d_attn, B * H); AL(d_h, B * I); AL(d_last, B * H);
   AL(logits, B * d.vocab); AL(logits_f32, B * d.vocab);
   AL(attn_partial, B * d.n_kv_head * kMaxSplit * (32 + 16 * D));
-  const int64_t amax_rows = gemv_ring_ntiles(d.vocab);
-  AL(amax_val, amax_rows * 8); AL(amax_idx, amax_rows * 8);
+  const int64_t amax_rows = gemv_ring_ntiles(d.vocab) * 8 * ring_row_groups((int)B);    // [tile][8 * row groups]
+  AL(amax_val, amax_rows); AL(amax_idx, amax_rows);
   AL(mega_layers, d.n_layer); AL(mega_dbg, 8192);
   {
     // flagged exchange buffers of the dataflow decode kernel, cleared together when a sequence starts
@@ -670,7 +670,7 @@ int sv_engine_create(const sv_model_desc* desc, int device, sv_engine** out) {
   if (d.n_kv_head < 1 || d.n_head % d.n_kv_head || d.n_head / d.n_kv_head > 16) return fail(nullptr, SV_ERR_INVALID, "need 1 <= n_head/n_kv_head <= 16");
   if (d.image_size % d.patch_size) return fail(nullptr, SV_ERR_INVALID, "image_size %% patch_size != 0");
   if (d.vit_width % 64 || d.vit_mlp % 64 || d.hidden % 64 || d.n_inner % 64) return fail(nullptr, SV_ERR_INVALID, "widths must be multiples of 64");
-  if (d.max_batch < 1 || d.max_batch > 8) return fail(nullptr, SV_ERR_INVALID, "max_batch must be in [1,8] (decode kernels hold 8 rows per MMA)");
+  if (d.max_batch < 1 || d.max_batch > 16) return fail(nullptr, SV_ERR_INVALID, "max_batch must be in [1,16] (decode kernels hold two groups of 8 rows per MMA)");
   if (d.adapter_norm != 0 && d.adapter_norm != 1) return fail(nullptr, SV_ERR_INVALID, "adapter_norm must be 0 or 1");
   if (d.vocab < 8 || d.vocab > (1 << 20)) return fail(nullptr, SV_ERR_INVALID, "vocab out of range");
 
@@ -713,7 +713,9 @@ int sv_engine_create(const sv_model_desc* desc, int device, sv_engine** out) {
   e->mega_debug = getenv("SV_MEGA_DEBUG") != nullptr;
   { const char* fl = getenv("SV_FLOW");          // "1": dataflow persistent kernel for greedy decode / teacher forcing (opt-in: the
     // per-phase CUDA graph is still faster, DESIGN.md §4); "3": the same without setmaxnreg register reallocation
-    e->use_flow = fl && (!strcmp(fl, "1") || !strcmp(fl, "2") || !strcmp(fl, "3")); 
+    e->use_flow = fl && (!strcmp(fl, "1") || !strcmp(fl, "2") || !strcmp(fl, "3"));
+    e->flow_requested = e->use_flow;
+    if (d.max_batch > 8) e->use_flow = false;     // the dataflow kernel holds 8 rows (decode_flow_supported); no tiled copies
     e->flow_realloc = !(fl && !strcmp(fl, "3"));
     const char* la = getenv("SV_FLOW_L2AHEAD");
     if (la) e->flow_l2_ahead = std::max(0, std::min(64, atoi(la))); }
@@ -721,6 +723,9 @@ int sv_engine_create(const sv_model_desc* desc, int device, sv_engine** out) {
   // v2 at full size: the per-op kernels measure faster (4.4 vs 5.8 ms/token at 8B; 768-wide slabs + per-slab LayerNorm
   // on the consumer path), so the fused ring step is opt-in for v2 (SV_DECODE=fused) until that is fixed.
   if (e->v2 && !(dec && !strcmp(dec, "fused"))) e->fused_decode = false;
+  // above 8 rows the fused step needs the 16-row ring kernels: v1 with hidden <= 2048 (they have no K > 2048 LayerNorm
+  // path) and 8 consumer warps
+  if (d.max_batch > 8 && (e->v2 || d.hidden > 2048 || d.max_batch > gemv_ring_max_rows())) e->fused_decode = false;
   if (!build_weights(e) || !build_buffers(e)) {
     std::string msg = std::string("device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
     sv_engine_destroy(e);
@@ -1023,7 +1028,8 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
   const int ntiles = gemv_ring_ntiles(e->d.vocab);
   auto select_step = [&](int advance_len, bool have_partials, bool pdl) {
     if (fused_select) {
-      launch_select_fused(e->logits, e->d.vocab, B, have_partials ? e->amax_val : nullptr, e->amax_idx, ntiles, e->state,
+      launch_select_fused(e->logits, e->d.vocab, B, have_partials ? e->amax_val : nullptr, e->amax_idx, ntiles,
+                          8 * ring_row_groups(B), e->state,
                           e->params, e->seen, e->next_ids, e->out_ids, advance_len, e->wte, e->wpe, e->d_x, e->d.hidden,
                           e->d.n_positions, pdl, st);
     } else {
@@ -1205,9 +1211,9 @@ int sv_generate_im2svg_host(sv_engine* e, const void* pixels_host, int32_t batch
 // candidates -> bookkeeping (+ next-token embeddings) -> KV suffix copies; the host replays it and polls `done`.
 int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_t* out_ids, int32_t* out_len, void* stream) {
   if (!e || !bp || !out_ids) return fail(e, SV_ERR_INVALID, "null argument");
-  if (sv_beam_params_check(bp, batch) != SV_OK)
-    return fail(e, SV_ERR_INVALID, "bad beam parameters (need num_beams >= 2, batch * num_beams <= 8, max_new_tokens >= 1, "
-                                   "n_stop_ids in [0,8], early_stopping in {0,1,2}, temperature > 0, repetition_penalty > 0)");
+  if (sv_beam_params_check_rows(bp, batch, e->d.max_batch) != SV_OK)
+    return fail(e, SV_ERR_INVALID, "bad beam parameters (need num_beams >= 2, batch * num_beams <= max_batch (%d), max_new_tokens >= 1, "
+                                   "n_stop_ids in [0,8], early_stopping in {0,1,2}, temperature > 0, repetition_penalty > 0)", e->d.max_batch);
   if (!e->prefilled) return fail(e, SV_ERR_STATE, "sv_beam_search needs sv_prefill first");
   if (e->host_cur_len != e->prefix_len) return fail(e, SV_ERR_STATE, "sv_beam_search must directly follow sv_prefill");
   const sv_model_desc& d = e->d;
@@ -1390,9 +1396,10 @@ int sv_debug_read_timeline(sv_engine* e, long long* out_host, int32_t n) {
 const char* sv_engine_describe(sv_engine* e) {
   if (!e) return "";
   char buf[512];
-  snprintf(buf, sizeof(buf), "decode=%s weights=%s attn=cluster-dsmem pdl=%d linear_impl=%d flow[%s]",
+  snprintf(buf, sizeof(buf), "decode=%s weights=%s attn=cluster-dsmem pdl=%d linear_impl=%d max_batch=%d flow[%s]%s",
            !e->fused_decode ? "legacy-kernels" : e->use_flow ? (e->flow_realloc ? "dataflow-kernel-setmaxnreg" : "dataflow-kernel") : "ring-gemv-graph",
-           e->ring_tiles ? "slab-tiled" : "row-major", (int)e->use_pdl, e->linear_impl, decode_flow_status());
+           e->ring_tiles ? "slab-tiled" : "row-major", (int)e->use_pdl, e->linear_impl, e->d.max_batch, decode_flow_status(),
+           e->flow_requested && !e->use_flow && e->d.max_batch > 8 ? " SV_FLOW ignored: the dataflow kernel holds 8 rows, max_batch > 8 runs the graph path" : "");
   e->describe = buf;
   return e->describe.c_str();
 }

@@ -124,7 +124,7 @@ cudaError_t launch_attention_decode_cluster(const bf16* qkv, int q_cols_total, c
 
 // ---- sv_decode_fused.cu : token selection fused with the next step's embedding, PDL-ready
 void launch_select_fused(const bf16* logits, int vocab, int batch, const float* amax_val, const int* amax_idx,
-                         int ntiles, GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
+                         int ntiles, int amax_stride, GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
                          int32_t* out_ids, int advance_len, const bf16* wte, const bf16* wpe, bf16* x, int h,
                          int n_positions, bool pdl, cudaStream_t st);
 
@@ -152,6 +152,10 @@ cudaError_t gemv_ring_init();
 bool gemv_ring_supported(int K, bool has_ln);
 int gemv_ring_ntiles(int N);
 int gemv_ring_ncta();
+int gemv_ring_max_rows();
+// Row groups of 8 a decode launch over B image rows uses (1 up to 8 rows, 2 for 9-16); the lm_head's argmax partials have
+// a row stride of 8 * groups.
+inline int ring_row_groups(int B) { return B > 8 ? 2 : 1; }
 void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st);
 // ---- sv_decode_flow.cu : dataflow persistent decode kernel (flagged activation words through L2, no grid barriers)
 struct FlowLaunch {

@@ -33,9 +33,12 @@ class B200GenerateMixin:
 
         self.torch_dtype = {"bfloat16": torch.bfloat16, "float16": torch.float16, "float32": torch.float32}[config.model.torch_dtype]
         path = getattr(self, "resume_from_checkpoint", None) if config.model.from_checkpoint else config.model.name   # :55-58
-        max_batch = int(getattr(config.dataset, "batch_size", 8))
+        batch_size = int(getattr(config.dataset, "batch_size", 8))
+        num_beams = max(1, int(getattr(config.generation_params, "num_beams", 2)))   # generate_im2svg's default (:234)
         max_len = int(getattr(config.generation_params, "max_length", 8192))
-        self.model = StarVectorForCausalLM.from_pretrained(path, torch_dtype=self.torch_dtype, max_batch=min(max_batch, 8), max_len=max_len)
+        # beams are cache rows: size the engine for a whole batch of beams when it fits the 16 rows a GPU holds
+        self.model = StarVectorForCausalLM.from_pretrained(path, torch_dtype=self.torch_dtype, max_batch=min(batch_size * num_beams, 16),
+                                                           max_len=max_len)
         self.bind_model(self.model)
 
     def bind_model(self, model) -> None:
