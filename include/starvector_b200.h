@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define SV_ABI_VERSION 6
+#define SV_ABI_VERSION 7
 #if defined(__GNUC__)
 #define SV_API __attribute__((visibility("default")))
 #else
@@ -224,6 +224,40 @@ SV_API int sv_generate_stream(sv_engine* e, const sv_gen_params* p, int32_t* out
 SV_API int sv_generate_im2svg_host(sv_engine* e, const void* pixels_host, int32_t batch,
                             const int32_t* prompt_ids_host, int32_t prompt_len, const sv_gen_params* p,
                             int32_t* out_ids_host, int32_t* out_len_host, void* stream);
+
+/* ---- continuous batching (vLLM-style serving; the reference's fast validator backend,
+ * starvector/validation/starvector_vllm_svg_validator.py) -------------------------------------- */
+/* A decode session keeps `slots` (<= max_batch) cache rows; every row decodes at its own position, has its own token cap
+ * and Philox seed and finishes on its own (EOS, the '</svg>' stop sequence over its own tokens, or its cap).  A finished
+ * row is refilled by sv_session_admit while the other rows keep their caches; the decode graph (captured once per session
+ * shape) then continues.  Every request gets the tokens a one-image sv_generate with the same parameters gives
+ * (greedy and sampling, bit for bit), up to and including its stop.  While a session is open, sv_encode_images,
+ * sv_prefill*, sv_decode_step, sv_score_tokens, sv_generate*, sv_beam_search, sv_reorder_cache, sv_expand_batch and
+ * sv_engine_load_weight return SV_ERR_STATE.  The session runs the CUDA-graph decode path (never the SV_FLOW dataflow kernel); beam search has
+ * no session form.
+ *
+ * sv_session_begin: p = the session's generation parameters: max_new_tokens is the session cap (it fixes the decode
+ * attention's split count together with the prompt length, as prefix + max_new_tokens does in sv_generate), eos, stop ids
+ * (always per row; stop_row0_only is ignored), sampling parameters, seed (the default of admitted rows), poll_interval. */
+SV_API int sv_session_begin(sv_engine* e, const sv_gen_params* p, int32_t slots);
+/* Encode and prefill images into free slots.  pixels bf16 [n_img,3,S,S] and prompt_ids int32 [n_img,prompt_len] (device);
+ * slots_host int32 [k]: the slots to fill; src_host int32 [k] (NULL = identity): the image index of each slot, so an
+ * image listed for n slots is prefilled once and its cache rows copied (n completions); max_new_host int32 [k] (NULL =
+ * the session cap, else in [1, cap]); seeds_host uint64 [k] (NULL = the session seed).  Token 0 of every admitted slot is
+ * selected here.  The prompt length is fixed by the first admission of the session; prefix + cap <= max_len.  Each image
+ * is encoded and prefilled at batch 1, with the kernels a one-image generate uses.  Synchronises `stream`. */
+SV_API int sv_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t* prompt_ids, int32_t prompt_len,
+                            const int32_t* slots_host, const int32_t* max_new_host, const uint64_t* seeds_host,
+                            const int32_t* src_host, void* stream);
+/* Replay the decode graph for up to max_steps steps, polling every poll_interval steps; returns (the number of steps run,
+ * >= 0) as soon as a poll finds a finished slot or no slot decoding.  finished_host int32 [slots] (optional): 1 for the
+ * slots whose finish this call reports (each finish is reported once; the slot is free again), len_host int32 [slots]
+ * (optional): tokens each slot holds.  Synchronises `stream`. */
+SV_API int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int32_t* len_host, void* stream);
+/* Copy the tokens of `slot` (as of the last sv_session_run) to ids (int32, host or device); returns their count. */
+SV_API int sv_session_read(sv_engine* e, int32_t slot, int32_t* ids, void* stream);
+/* Close the session: the rectangle-batch entry points work again (after a new prefill). */
+SV_API int sv_session_end(sv_engine* e);
 
 /* ---- introspection for bench/profiles ------------------------------------------------- */
 /* Kernel launches issued by this engine since creation (graph replays count their nodes). */

@@ -16,7 +16,7 @@ SV_OK, SV_ERR_INVALID, SV_ERR_CUDA, SV_ERR_UNSUPPORTED, SV_ERR_STATE = 0, -1, -2
 SV_DTYPE_BF16, SV_DTYPE_F32, SV_DTYPE_F16 = 0, 1, 2
 SV_ACT_NONE, SV_ACT_QUICKGELU, SV_ACT_GELU_TANH, SV_ACT_SILU = 0, 1, 2, 3
 SV_LINEAR_AUTO, SV_LINEAR_ROWGROUP, SV_LINEAR_TCGEN05 = 0, 1, 2
-ABI_VERSION = 6
+ABI_VERSION = 7
 SV_ALPHA_WHITE, SV_ALPHA_DROP = 0, 1
 
 
@@ -89,6 +89,11 @@ SIGNATURES = {
     "sv_generate": (C.c_int, [_P, C.POINTER(GenParams), _P, _P, _P]),
     "sv_generate_stream": (C.c_int, [_P, C.POINTER(GenParams), _P, _P, TOKEN_CALLBACK, _P, _P]),
     "sv_generate_im2svg_host": (C.c_int, [_P, _P, _I, _P, _I, C.POINTER(GenParams), _P, _P, _P]),
+    "sv_session_begin": (C.c_int, [_P, C.POINTER(GenParams), _I]),
+    "sv_session_admit": (C.c_int, [_P, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
+    "sv_session_run": (C.c_int, [_P, _I, _P, _P, _P]),
+    "sv_session_read": (C.c_int, [_P, _I, _P, _P]),
+    "sv_session_end": (C.c_int, [_P]),
     "sv_launch_count": (C.c_int64, [_P]),
     "sv_engine_describe": (C.c_char_p, [_P]),
     "sv_debug_read_timeline": (C.c_int, [_P, C.POINTER(C.c_longlong), _I]),

@@ -332,15 +332,17 @@ cudaError_t launch_attention_chunk(const bf16* qkv, int q_cols_total, int q_rows
 // each) so every SM pulls a slice of the cache; partial (m, l, acc) go to an fp32 scratch and a
 // second small kernel merges them in a fixed order (deterministic).
 //   partial layout: [b][kvh][split][ 16 (m) | 16 (l) | 16*D (acc) ]
-template <int D>
-__global__ void __launch_bounds__(32) attention_decode_split_kernel(
+// ROWS (the session variants): image b's keys are [0, rows->row_len[b]] instead of [0, cur_len]; the split count stays a
+// launch parameter, so a row's partition and merge order depend only on its own length.
+template <int D, bool ROWS>
+SV_DEVINL void attention_decode_split_body(
     const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
-    float* __restrict__ partial, const GenState* __restrict__ state, int n_head, int n_kv, int tcap, int nsplit,
-    float scale_log2, int window) {
+    float* __restrict__ partial, const GenState* __restrict__ state, const RowState* __restrict__ rows, int n_head,
+    int n_kv, int tcap, int nsplit, float scale_log2, int window) {
   const int lane = threadIdx.x, g = lane >> 2, t = lane & 3;
   const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
   const int group = n_head / n_kv;
-  const int nkeys = state->cur_len + 1;                       // the new token's K/V is already appended
+  const int nkeys = (ROWS ? rows->row_len[b] : state->cur_len) + 1;   // the new token's K/V is already appended
   const int key_lo = window > 0 ? max(0, nkeys - window) : 0;
   const int blk_lo = key_lo / 32;
   const int blocks = (nkeys + 31) / 32 - blk_lo;
@@ -370,16 +372,31 @@ __global__ void __launch_bounds__(32) attention_decode_split_kernel(
     *reinterpret_cast<float2*>(pout + 32 + (g + 8) * D + 8 * nd + 2 * t) = make_float2(acc[nd][2], acc[nd][3]);
   }
 }
-
 template <int D>
-__global__ void __launch_bounds__(D) attention_decode_merge_kernel(const float* __restrict__ partial,
-                                                                   bf16* __restrict__ out,
-                                                                   const GenState* __restrict__ state, int n_head,
-                                                                   int n_kv, int nsplit, int window) {
+__global__ void __launch_bounds__(32) attention_decode_split_kernel(
+    const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
+    float* __restrict__ partial, const GenState* __restrict__ state, int n_head, int n_kv, int tcap, int nsplit,
+    float scale_log2, int window) {
+  attention_decode_split_body<D, false>(qkv, ld, kcache, vtcache, partial, state, nullptr, n_head, n_kv, tcap, nsplit,
+                                        scale_log2, window);
+}
+template <int D>
+__global__ void __launch_bounds__(32) attention_decode_split_rows_kernel(
+    const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
+    float* __restrict__ partial, const RowState* __restrict__ rows, int n_head, int n_kv, int tcap, int nsplit,
+    float scale_log2, int window) {
+  attention_decode_split_body<D, true>(qkv, ld, kcache, vtcache, partial, nullptr, rows, n_head, n_kv, tcap, nsplit,
+                                       scale_log2, window);
+}
+
+template <int D, bool ROWS>
+SV_DEVINL void attention_decode_merge_body(const float* __restrict__ partial, bf16* __restrict__ out,
+                                           const GenState* __restrict__ state, const RowState* __restrict__ rows,
+                                           int n_head, int n_kv, int nsplit, int window) {
   const int r = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z, dim = threadIdx.x;
   const int group = n_head / n_kv;
   if (r >= group) return;
-  const int nkeys = state->cur_len + 1;
+  const int nkeys = (ROWS ? rows->row_len[b] : state->cur_len) + 1;
   const int blocks = (nkeys + 31) / 32 - (window > 0 ? max(0, nkeys - window) : 0) / 32;
   const int per = (blocks + nsplit - 1) / nsplit;
   const int nact = (blocks + per - 1) / per;                  // splits that had keys (same rule as above)
@@ -396,16 +413,37 @@ __global__ void __launch_bounds__(D) attention_decode_merge_kernel(const float* 
   }
   out[(int64_t)b * n_head * D + ((int64_t)kvh * group + r) * D + dim] = __float2bfloat16_rn(A / L);
 }
+template <int D>
+__global__ void __launch_bounds__(D) attention_decode_merge_kernel(const float* __restrict__ partial,
+                                                                   bf16* __restrict__ out,
+                                                                   const GenState* __restrict__ state, int n_head,
+                                                                   int n_kv, int nsplit, int window) {
+  attention_decode_merge_body<D, false>(partial, out, state, nullptr, n_head, n_kv, nsplit, window);
+}
+template <int D>
+__global__ void __launch_bounds__(D) attention_decode_merge_rows_kernel(const float* __restrict__ partial,
+                                                                        bf16* __restrict__ out,
+                                                                        const RowState* __restrict__ rows, int n_head,
+                                                                        int n_kv, int nsplit, int window) {
+  attention_decode_merge_body<D, true>(partial, out, nullptr, rows, n_head, n_kv, nsplit, window);
+}
 
 void launch_attention_decode(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache, bf16* out,
                              float* partial, const GenState* state, int batch, int n_head, int n_kv, int d, int tcap,
-                             int nsplit, int window, cudaStream_t st) {
+                             int nsplit, int window, cudaStream_t st, const RowState* rows) {
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)d);
-  attention_decode_split_kernel<128><<<dim3(nsplit, n_kv, batch), 32, 0, st>>>(qkv, q_cols_total, kcache, vtcache,
-                                                                              partial, state, n_head, n_kv, tcap,
-                                                                              nsplit, scale_log2, window);
-  attention_decode_merge_kernel<128><<<dim3(n_head / n_kv, n_kv, batch), 128, 0, st>>>(partial, out, state, n_head,
-                                                                                      n_kv, nsplit, window);
+  if (rows) {
+    attention_decode_split_rows_kernel<128><<<dim3(nsplit, n_kv, batch), 32, 0, st>>>(
+        qkv, q_cols_total, kcache, vtcache, partial, rows, n_head, n_kv, tcap, nsplit, scale_log2, window);
+    attention_decode_merge_rows_kernel<128><<<dim3(n_head / n_kv, n_kv, batch), 128, 0, st>>>(partial, out, rows, n_head,
+                                                                                              n_kv, nsplit, window);
+  } else {
+    attention_decode_split_kernel<128><<<dim3(nsplit, n_kv, batch), 32, 0, st>>>(qkv, q_cols_total, kcache, vtcache,
+                                                                                partial, state, n_head, n_kv, tcap,
+                                                                                nsplit, scale_log2, window);
+    attention_decode_merge_kernel<128><<<dim3(n_head / n_kv, n_kv, batch), 128, 0, st>>>(partial, out, state, n_head,
+                                                                                        n_kv, nsplit, window);
+  }
   count_launch(2);
 }
 
@@ -428,17 +466,19 @@ SV_DEVINL float ld_dsmem(uint32_t local_addr, uint32_t cta_rank) {
   return v;
 }
 
-template <int D>
-__global__ void __launch_bounds__(kDecWarps * 32, 1) attention_decode_cluster_kernel(
+// ROWS (the session variant): image b's keys are [0, rows->row_len[b]]; the cluster size stays the launch's, so CTAs
+// of a short row that get no key block still join both cluster barriers and contribute m = -inf.
+template <int D, bool ROWS>
+SV_DEVINL void attention_decode_cluster_body(
     const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
-    bf16* __restrict__ out, const GenState* __restrict__ state, int n_head, int n_kv, int tcap, float scale_log2,
-    int window) {
+    bf16* __restrict__ out, const GenState* __restrict__ state, const RowState* __restrict__ rows, int n_head, int n_kv,
+    int tcap, float scale_log2, int window) {
   extern __shared__ float dsm[];                               // [kDecWarps][PSZ] warp partials | [PSZ] CTA partial
   constexpr int PSZ = 32 + 16 * D;
   float* cta_part = dsm + kDecWarps * PSZ;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   // cur_len was written by the previous token's select kernel (long complete): read it before the PDL wait
-  const int nkeys = state->cur_len + 1;
+  const int nkeys = (ROWS ? rows->row_len[blockIdx.z] : state->cur_len) + 1;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const int cta = blockIdx.x, ncta = gridDim.x, kvh = blockIdx.y, b = blockIdx.z;
   const int group = n_head / n_kv;
@@ -513,6 +553,22 @@ __global__ void __launch_bounds__(kDecWarps * 32, 1) attention_decode_cluster_ke
   }
   cluster_sync_all();                                           // nobody exits while its smem may still be read
 }
+template <int D>
+__global__ void __launch_bounds__(kDecWarps * 32, 1) attention_decode_cluster_kernel(
+    const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
+    bf16* __restrict__ out, const GenState* __restrict__ state, int n_head, int n_kv, int tcap, float scale_log2,
+    int window) {
+  attention_decode_cluster_body<D, false>(qkv, ld, kcache, vtcache, out, state, nullptr, n_head, n_kv, tcap, scale_log2,
+                                          window);
+}
+template <int D>
+__global__ void __launch_bounds__(kDecWarps * 32, 1) attention_decode_cluster_rows_kernel(
+    const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
+    bf16* __restrict__ out, const RowState* __restrict__ rows, int n_head, int n_kv, int tcap, float scale_log2,
+    int window) {
+  attention_decode_cluster_body<D, true>(qkv, ld, kcache, vtcache, out, nullptr, rows, n_head, n_kv, tcap, scale_log2,
+                                         window);
+}
 
 int attention_decode_cluster_ncta(int total_len) {
   const int blocks = (total_len + 31) / 32;
@@ -520,13 +576,17 @@ int attention_decode_cluster_ncta(int total_len) {
 }
 
 cudaError_t attention_decode_cluster_init() {
-  return cudaFuncSetAttribute(attention_decode_cluster_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  cudaError_t e = cudaFuncSetAttribute(attention_decode_cluster_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (kDecWarps + 1) * (32 + 16 * 128) * (int)sizeof(float));
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(attention_decode_cluster_rows_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               (kDecWarps + 1) * (32 + 16 * 128) * (int)sizeof(float));
 }
 
 cudaError_t launch_attention_decode_cluster(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache,
                                             bf16* out, const GenState* state, int batch, int n_head, int n_kv, int d,
-                                            int tcap, int ncta, int window, bool pdl, cudaStream_t st) {
+                                            int tcap, int ncta, int window, bool pdl, cudaStream_t st,
+                                            const RowState* rows) {
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)d);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(ncta, n_kv, batch); cfg.blockDim = dim3(kDecWarps * 32);
@@ -537,8 +597,10 @@ cudaError_t launch_attention_decode_cluster(const bf16* qkv, int q_cols_total, c
   at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at; cfg.numAttrs = pdl ? 2 : 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, attention_decode_cluster_kernel<128>, qkv, q_cols_total, kcache, vtcache, out,
-                                     state, n_head, n_kv, tcap, scale_log2, window);
+  cudaError_t e = rows ? cudaLaunchKernelEx(&cfg, attention_decode_cluster_rows_kernel<128>, qkv, q_cols_total, kcache,
+                                            vtcache, out, rows, n_head, n_kv, tcap, scale_log2, window)
+                       : cudaLaunchKernelEx(&cfg, attention_decode_cluster_kernel<128>, qkv, q_cols_total, kcache,
+                                            vtcache, out, state, n_head, n_kv, tcap, scale_log2, window);
   count_launch();
   return e;
 }

@@ -28,23 +28,33 @@ static void launch_ex(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem
 // Token selection + HF stop bookkeeping + next-token embedding in ONE single-CTA kernel.
 // Greedy without a repetition penalty reduces the lm_head's per-tile argmax partials; otherwise the
 // full bf16 logits row is scanned (penalty changes the order).  Semantics: SURVEY.md App. B.3-6.
-__global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restrict__ logits, int vocab, int batch,
-                                                            const float* __restrict__ amax_val,
-                                                            const int* __restrict__ amax_idx, int ntiles, int amax_stride,
-                                                            GenState* state, const GenParamsDev* __restrict__ p,
-                                                            uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
-                                                            int advance_len, const bf16* __restrict__ wte,
-                                                            const bf16* __restrict__ wpe, bf16* __restrict__ x, int h,
-                                                            int n_positions) {
+// ROWS (the session variant): rows that do not select this step (session_row_selects) are skipped, each selecting row
+// keeps its own bookkeeping (session_append_token) and is embedded at its own position.
+template <bool ROWS>
+SV_DEVINL void select_fused_body(const bf16* __restrict__ logits, int vocab, int batch, const float* __restrict__ amax_val,
+                                 const int* __restrict__ amax_idx, int ntiles, int amax_stride, GenState* state,
+                                 const GenParamsDev* __restrict__ p, uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
+                                 int advance_len, const bf16* __restrict__ wte, const bf16* __restrict__ wpe,
+                                 bf16* __restrict__ x, int h, int n_positions, RowState* rows, uint32_t row_mask) {
   pdl_launch_dependents();
   pdl_wait();
-  if (state->done) return;
+  if constexpr (!ROWS) {
+    if (state->done) return;
+  }
   __shared__ AmaxPair sm[32];
   __shared__ int s_tok[16];
+  __shared__ int s_sel[16];
   const int tid = threadIdx.x;
   const float rp = p->rep_penalty;
   const bool use_partials = (rp == 1.0f) && amax_val != nullptr;
+  if constexpr (ROWS) {
+    if (tid < batch) s_sel[tid] = session_row_selects(rows, row_mask, tid) ? 1 : 0;
+    __syncthreads();
+  }
   for (int b = 0; b < batch; ++b) {
+    if constexpr (ROWS) {
+      if (!s_sel[b]) continue;
+    }
     AmaxPair best{-INFINITY, 0x7fffffff};
     if (use_partials) {
       for (int i = tid; i < ntiles; i += 1024) {
@@ -75,14 +85,23 @@ __global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restri
     }
   }
   __syncthreads();
-  if (tid == 0) select_apply_tokens(s_tok, batch, vocab, state, p, seen, next_ids, out_ids, advance_len);
+  if constexpr (ROWS) {
+    if (tid < batch && s_sel[tid])
+      session_append_token(tid, s_tok[tid], rows, p, seen, vocab, next_ids, out_ids, advance_len);
+  } else {
+    if (tid == 0) select_apply_tokens(s_tok, batch, vocab, state, p, seen, next_ids, out_ids, advance_len);
+  }
   __syncthreads();
   // --- next step's input: wte[token] + wpe[position] (bf16 add), GPTBigCodeModel.forward
-  int pos = state->cur_len;
+  int pos = ROWS ? 0 : state->cur_len;
   pos = pos >= n_positions ? n_positions - 1 : pos;
   const int hv = h >> 3;
   for (int i = tid; i < batch * hv; i += 1024) {
     const int b = i / hv, c = (i % hv) * 8;
+    if constexpr (ROWS) {
+      if (!s_sel[b]) continue;
+      pos = min(rows->row_len[b], n_positions - 1);
+    }
     int id = s_tok[b];
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
     float e[8], q[8];
@@ -95,13 +114,40 @@ __global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restri
     *reinterpret_cast<uint4*>(x + (int64_t)b * h + c) = pack8(e);
   }
 }
+__global__ void __launch_bounds__(1024) select_fused_kernel(const bf16* __restrict__ logits, int vocab, int batch,
+                                                            const float* __restrict__ amax_val,
+                                                            const int* __restrict__ amax_idx, int ntiles, int amax_stride,
+                                                            GenState* state, const GenParamsDev* __restrict__ p,
+                                                            uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
+                                                            int advance_len, const bf16* __restrict__ wte,
+                                                            const bf16* __restrict__ wpe, bf16* __restrict__ x, int h,
+                                                            int n_positions) {
+  select_fused_body<false>(logits, vocab, batch, amax_val, amax_idx, ntiles, amax_stride, state, p, seen, next_ids, out_ids,
+                           advance_len, wte, wpe, x, h, n_positions, nullptr, 0u);
+}
+__global__ void __launch_bounds__(1024) select_fused_rows_kernel(const bf16* __restrict__ logits, int vocab, int batch,
+                                                                 const float* __restrict__ amax_val,
+                                                                 const int* __restrict__ amax_idx, int ntiles,
+                                                                 int amax_stride, RowState* rows, uint32_t row_mask,
+                                                                 const GenParamsDev* __restrict__ p, uint8_t* seen,
+                                                                 int32_t* next_ids, int32_t* out_ids, int advance_len,
+                                                                 const bf16* __restrict__ wte,
+                                                                 const bf16* __restrict__ wpe, bf16* __restrict__ x,
+                                                                 int h, int n_positions) {
+  select_fused_body<true>(logits, vocab, batch, amax_val, amax_idx, ntiles, amax_stride, nullptr, p, seen, next_ids, out_ids,
+                          advance_len, wte, wpe, x, h, n_positions, rows, row_mask);
+}
 
 void launch_select_fused(const bf16* logits, int vocab, int batch, const float* amax_val, const int* amax_idx,
                          int ntiles, int amax_stride, GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
                          int32_t* out_ids, int advance_len, const bf16* wte, const bf16* wpe, bf16* x, int h,
-                         int n_positions, bool pdl, cudaStream_t st) {
-  launch_ex(select_fused_kernel, dim3(1), dim3(1024), 0, st, pdl, logits, vocab, batch, amax_val, amax_idx, ntiles,
-            amax_stride, state, params, seen, next_ids, out_ids, advance_len, wte, wpe, x, h, n_positions);
+                         int n_positions, bool pdl, cudaStream_t st, RowState* rows, uint32_t row_mask) {
+  if (rows)
+    launch_ex(select_fused_rows_kernel, dim3(1), dim3(1024), 0, st, pdl, logits, vocab, batch, amax_val, amax_idx, ntiles,
+              amax_stride, rows, row_mask, params, seen, next_ids, out_ids, advance_len, wte, wpe, x, h, n_positions);
+  else
+    launch_ex(select_fused_kernel, dim3(1), dim3(1024), 0, st, pdl, logits, vocab, batch, amax_val, amax_idx, ntiles,
+              amax_stride, state, params, seen, next_ids, out_ids, advance_len, wte, wpe, x, h, n_positions);
 }
 
 }  // namespace sv

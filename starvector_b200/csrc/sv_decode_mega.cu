@@ -23,7 +23,9 @@ namespace sv {
 namespace mega {
 
 
-enum { EPI_PLAIN = 0, EPI_QKV = 1, EPI_LMHEAD = 2 };
+// EPI_QKV_ROW: EPI_QKV of a continuous-batching session, each image row's K/V appended at its own position
+// (RowState::row_len); a separate instantiation, so the EPI_QKV kernels keep their code.
+enum { EPI_PLAIN = 0, EPI_QKV = 1, EPI_LMHEAD = 2, EPI_QKV_ROW = 3 };
 
 struct Ctx {
   const Args* a;
@@ -35,6 +37,7 @@ struct Ctx {
   // their HBM misses overlap the previous kernel's tail instead of sitting on this kernel's critical path
   uint32_t ln_s = 0;            // shared address of [ln_w row | ln_b row] (K bf16 each), 0 = read them from global
   const float* bias_s = nullptr;   // [tile][16] biases of this CTA's output rows
+  const int32_t* row_len = nullptr;   // EPI_QKV_ROW: per-row KV positions
 };
 
 // ---- consumer: one GEMV phase  Y[B,N] = epi( LN?(X)[B,K] . W[N,K]^T )
@@ -181,6 +184,7 @@ SV_DEVINL void gemv_phase(const Ctx& cx, Ring& r, const bf16* __restrict__ X, co
   float c[4] = {0.f, 0.f, 0.f, 0.f};
   int pos_now = 0;
   if constexpr (EPI == EPI_QKV) pos_now = __ldcg(&a.state->cur_len);         // read here, not behind the last MMA
+  if constexpr (EPI == EPI_QKV_ROW) pos_now = __ldcg(cx.row_len + min((int)(threadIdx.x >> 4), 15));   // the epilogue row's
   for (int tl = 0; tl < p.ntile; ++tl) {
     const int tile = p.tile0 + tl;
     // the epilogue thread's residual value: requested now, used after the MMAs (an L2 round trip off the tail)
@@ -285,7 +289,7 @@ SV_DEVINL void gemv_phase(const Ctx& cx, Ring& r, const bf16* __restrict__ X, co
         const bf16 vb = __float2bfloat16_rn(v);
         v_bf = __bfloat162float(vb);
         Y[(int64_t)mm * N + col] = vb;
-        if constexpr (EPI == EPI_QKV) {
+        if constexpr (EPI == EPI_QKV || EPI == EPI_QKV_ROW) {
           const int q_cols = a.n_head * D, j = col - q_cols;
           const int pos = pos_now;
           if (j >= 0 && pos < a.tcap) {
@@ -466,6 +470,7 @@ SV_DEVINL void gemv_phase_wide(const Ctx& cx, Ring& r, const bf16* __restrict__ 
   for (int gi = 0; gi < NG; ++gi) { c[gi][0] = 0.f; c[gi][1] = 0.f; c[gi][2] = 0.f; c[gi][3] = 0.f; }
   int pos_now = 0;
   if constexpr (EPI == EPI_QKV) pos_now = __ldcg(&a.state->cur_len);         // read here, not behind the last MMA
+  if constexpr (EPI == EPI_QKV_ROW) pos_now = __ldcg(cx.row_len + min((int)(threadIdx.x >> 4), 15));   // the epilogue row's
   for (int tl = 0; tl < p.ntile; ++tl) {
     const int tile = p.tile0 + tl;
     // the epilogue thread's residual value: requested now, used after the MMAs (an L2 round trip off the tail)
@@ -567,7 +572,7 @@ SV_DEVINL void gemv_phase_wide(const Ctx& cx, Ring& r, const bf16* __restrict__ 
         const bf16 vb = __float2bfloat16_rn(v);
         v_bf = __bfloat162float(vb);
         Y[(int64_t)mm * N + col] = vb;
-        if constexpr (EPI == EPI_QKV) {
+        if constexpr (EPI == EPI_QKV || EPI == EPI_QKV_ROW) {
           const int q_cols = a.n_head * D, j = col - q_cols;
           const int pos = pos_now;
           if (j >= 0 && pos < a.tcap) {
@@ -615,6 +620,7 @@ struct RingGemvArgs {
   bf16* Y;
   int N, K, act;
   int nslots;        // ring depth of THIS launch
+  const int32_t* row_len;   // EPI_QKV_ROW: RowState::row_len (KV append position and L2 prefetch range of each row)
 };
 
 // The c_attn GEMV's producer warp is idle once its two slabs are on their way: it pulls the K / V^T rows the NEXT kernel (the
@@ -634,6 +640,28 @@ SV_DEVINL void l2_prefetch_kv(const bf16* kc, const bf16* vc, int nkeys, int nbk
     uint32_t v;
     asm volatile("ld.global.cg.L2::128B.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     acc ^= v;
+  }
+  if (acc == 0x9e3779b9u && nkeys < 0) asm volatile("trap;");     // (never: keeps the loads' results alive)
+}
+// The same for a session: image row b's keys are [0, row_len[b]) (every row pulls only its own range).
+SV_DEVINL void l2_prefetch_kv_rows(const bf16* kc, const bf16* vc, const int32_t* row_len, int B, int n_kv, int tcap, int cta,
+                                   int ncta, int lane) {
+  uint32_t acc = 0;
+  int nkeys = 0;
+  for (int b = 0; b < B; ++b) {
+    nkeys = __ldcg(row_len + b);
+    if (nkeys <= 0) continue;
+    const int klines = (nkeys * D * 2 + 127) >> 7;
+    const int vlines_row = (nkeys * 2 + 127) >> 7, vlines = D * vlines_row;
+    const int per_bk = klines + vlines, total = n_kv * per_bk;
+    for (int i = cta + ncta * lane; i < total; i += ncta * 32) {
+      const int bk = b * n_kv + i / per_bk, r = i % per_bk;
+      const char* p = r < klines ? reinterpret_cast<const char*>(kc + (int64_t)bk * tcap * D) + (int64_t)r * 128
+                                 : reinterpret_cast<const char*>(vc + ((int64_t)bk * D + (r - klines) / vlines_row) * tcap) + (int64_t)((r - klines) % vlines_row) * 128;
+      uint32_t v;
+      asm volatile("ld.global.cg.L2::128B.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+      acc ^= v;
+    }
   }
   if (acc == 0x9e3779b9u && nkeys < 0) asm volatile("trap;");     // (never: keeps the loads' results alive)
 }
@@ -669,12 +697,15 @@ SV_DEVINL void gemv_ring_body(const RingGemvArgs& ra) {
     else produce_phase(ring, ra.W, ra.N, ra.K, cta, ncta, lane);     // no dependency on the previous kernel
     if constexpr (EPI == EPI_QKV)
       l2_prefetch_kv(ra.L.kc, ra.L.vc, ra.a.state->cur_len, ra.a.B * ra.a.n_kv, ra.a.tcap, cta, ncta, lane);
+    if constexpr (EPI == EPI_QKV_ROW)
+      l2_prefetch_kv_rows(ra.L.kc, ra.L.vc, ra.row_len, ra.a.B, ra.a.n_kv, ra.a.tcap, cta, ncta, lane);
     return;
   }
   Ctx cx;
   cx.a = &ra.a; cx.smem = smem; cx.cta = cta; cx.ncta = ncta; cx.warp = warp; cx.lane = lane; cx.g = lane >> 2; cx.t = lane & 3;
   cx.red = reinterpret_cast<float*>(smem + off_red);
   cx.stat = reinterpret_cast<float*>(smem + off_stat);
+  if constexpr (EPI == EPI_QKV_ROW) cx.row_len = ra.row_len;
   // immutable parameters (LayerNorm affine, biases of this CTA's rows) are staged into shared memory before the wait on the
   // previous kernel: their HBM misses (~1 us each, two per LayerNorm kernel, one per epilogue) overlap that kernel's tail
   {
@@ -748,7 +779,7 @@ cudaError_t gemv_ring_init() {   // set the shared-memory opt-in outside of any 
                            mega::ring_smem_bytes(mega::STAGES, 2));                                                   \
   if (e != cudaSuccess) return e;
   SV_RING_ATTR(true, mega::EPI_QKV) SV_RING_ATTR(true, mega::EPI_PLAIN) SV_RING_ATTR(true, mega::EPI_LMHEAD)
-  SV_RING_ATTR(false, mega::EPI_PLAIN)
+  SV_RING_ATTR(false, mega::EPI_PLAIN) SV_RING_ATTR(true, mega::EPI_QKV_ROW)
 #undef SV_RING_ATTR
   e = cudaFuncSetAttribute(mega::gemv_ring_kernel<true, mega::EPI_PLAIN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mega::SMEM_BYTES);
   if (e != cudaSuccess) return e;
@@ -785,6 +816,8 @@ void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st) {
   ra.L.kc = g.kcache; ra.L.vc = g.vtcache;
   ra.X = g.X; ra.W = g.W; ra.Wt = g.Wt; ra.bias = g.bias; ra.res = g.res; ra.ln_w = g.ln_w; ra.ln_b = g.ln_b; ra.Y = g.Y;
   ra.N = g.N; ra.K = g.K; ra.act = g.act;
+  ra.row_len = g.rows ? g.rows->row_len : nullptr;
+  const int epi = (g.rows && g.epi == mega::EPI_QKV) ? (int)mega::EPI_QKV_ROW : g.epi;
   const int nsm = gemv_ring_ncta();
   {   // ring depth: what this CTA will stream, capped so the next kernel's CTA can co-reside (227 KB per SM)
     static int cap = 0;
@@ -808,13 +841,15 @@ void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st) {
     return;
   }
   if (ring_row_groups(g.B) == 2) {           // 9-16 rows: two row groups share each weight fragment
-    if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV, false, 2>(ra, nsm, g.pdl, st);
+    if (ln && epi == mega::EPI_QKV_ROW) launch_ring_t<true, mega::EPI_QKV_ROW, false, 2>(ra, nsm, g.pdl, st);
+    else if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV, false, 2>(ra, nsm, g.pdl, st);
     else if (ln && g.epi == mega::EPI_LMHEAD) launch_ring_t<true, mega::EPI_LMHEAD, false, 2>(ra, nsm, g.pdl, st);
     else if (ln) launch_ring_t<true, mega::EPI_PLAIN, false, 2>(ra, nsm, g.pdl, st);
     else launch_ring_t<false, mega::EPI_PLAIN, false, 2>(ra, nsm, g.pdl, st);
     return;
   }
-  if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV>(ra, nsm, g.pdl, st);
+  if (ln && epi == mega::EPI_QKV_ROW) launch_ring_t<true, mega::EPI_QKV_ROW>(ra, nsm, g.pdl, st);
+  else if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV>(ra, nsm, g.pdl, st);
   else if (ln && g.epi == mega::EPI_LMHEAD) launch_ring_t<true, mega::EPI_LMHEAD>(ra, nsm, g.pdl, st);
   else if (ln) launch_ring_t<true, mega::EPI_PLAIN>(ra, nsm, g.pdl, st);
   else launch_ring_t<false, mega::EPI_PLAIN>(ra, nsm, g.pdl, st);

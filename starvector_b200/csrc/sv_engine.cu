@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cstddef>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -131,6 +132,17 @@ struct sv_engine {
   std::map<long long, GraphEntry> graphs;   // key = batch * 1000 + nsplit * 2 + do_sample
   float last_decode_ms = 0.f;
   int last_decode_steps = 0;
+
+  // continuous-batching session (sv_session_*): `sess_slots` cache rows decode with per-row positions (RowState); finished
+  // rows are refilled by admission while the others keep their caches
+  bool session = false;
+  sv_gen_params sess_p{};
+  int sess_slots = 0, sess_prompt_len = 0;   // the prompt length is fixed by the first admission
+  RowState* rows = nullptr;                  // device, allocated by the first session
+  RowState* rows_host = nullptr;             // pinned read-back of the polled fields
+  bf16* sess_logits = nullptr;               // [max_batch][vocab]: the prefill logits of admitted slots (token 0 is read there)
+  std::vector<int> sess_live;                // host: slot holds a request whose finish was not reported yet
+  std::vector<int> sess_len;                 // host: tokens of each slot at the last poll
 };
 
 namespace {
@@ -435,14 +447,18 @@ int run_encode(sv_engine* e, const bf16* pixels, int B, cudaStream_t st) {
 // ---- stage: decoder prefill -----------------------------------------------------------------
 // `prefix` is [B, q, H] embeddings (the resident visual prefix, or caller-provided inputs_embeds);
 // `prompt_ids` [B, P] are embedded through wte and appended (P may be 0).
-int run_prefill(sv_engine* e, const bf16* prefix, int q, const int32_t* prompt_ids, int B, int P, cudaStream_t st) {
+// `row0`: the prefilled images land in cache rows row0 .. row0+B-1 (a session admits into its free slots; every other row
+// of the cache is left as it is), and the last-position logits go to `logits_out` (nullptr: e->logits).
+int run_prefill(sv_engine* e, const bf16* prefix, int q, const int32_t* prompt_ids, int B, int P, cudaStream_t st,
+                int row0 = 0, bf16* logits_out = nullptr) {
   const sv_model_desc& d = e->d;
   const int H = d.hidden, T0 = q + P, M = B * T0, D = d.head_dim;
+  const int64_t row_off = (int64_t)row0 * d.n_kv_head * e->tcap * D;     // cache layout [layer][row][n_kv][tcap][D]
   launch_embed_prefix(prefix, prompt_ids, e->wte, e->wpe, e->p_x, B, q, P, H, d.vocab, 0, P, st);
   for (int i = 0; i < d.n_layer; ++i) {
     const DecLayer& L = e->dec[i];
-    bf16* kc = e->kcache + e->cache_layer_stride * i;
-    bf16* vc = e->vtcache + e->cache_layer_stride * i;
+    bf16* kc = e->kcache + e->cache_layer_stride * i + row_off;
+    bf16* vc = e->vtcache + e->cache_layer_stride * i + row_off;
     launch_layernorm(e->p_x, L.ln1_w, L.ln1_b, e->p_ln, M, H, d.ln_eps, H, st);
     LIN(e->p_ln, L.attn_w, L.attn_b, nullptr, e->p_qkv, M, e->qkv_cols, H, SV_ACT_NONE, st);
     if (e->v2)   // RoPE on q and k (positions 0..T0-1), modeling_starcoder2.py:167-168
@@ -457,7 +473,7 @@ int run_prefill(sv_engine* e, const bf16* prefix, int q, const int32_t* prompt_i
   // last-position logits only (HF computes all T0 positions; only [:, -1] is consumed)
   launch_gather_rows(e->p_x, e->d_last, B, T0, T0 - 1, H, st);
   launch_layernorm(e->d_last, e->lnf_w, e->lnf_b, e->d_ln, B, H, d.ln_eps, H, st);
-  launch_linear_rowgroup(e->d_ln, e->lm_head, nullptr, nullptr, e->logits, B, d.vocab, H, SV_ACT_NONE, st);
+  launch_linear_rowgroup(e->d_ln, e->lm_head, nullptr, nullptr, logits_out ? logits_out : e->logits, B, d.vocab, H, SV_ACT_NONE, st);
   return SV_OK;
 }
 
@@ -510,10 +526,11 @@ int run_score_chunk(sv_engine* e, const int32_t* ids, int n, int c0, int C, int 
 }
 
 // ---- one decode step: token ids (device) at position state->cur_len -> logits ----------------
-int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaStream_t st) {
+// rows != nullptr: a session step, row b at its own position rows->row_len[b]
+int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaStream_t st, const RowState* rows = nullptr) {
   const sv_model_desc& d = e->d;
   const int H = d.hidden, D = d.head_dim;
-  launch_embed_tokens(ids, e->wte, e->wpe, e->state, e->d_x, B, H, d.vocab, d.n_positions, st);
+  launch_embed_tokens(ids, e->wte, e->wpe, e->state, e->d_x, B, H, d.vocab, d.n_positions, st, rows);
   for (int i = 0; i < d.n_layer; ++i) {
     const DecLayer& L = e->dec[i];
     bf16* kc = e->kcache + e->cache_layer_stride * i;
@@ -521,10 +538,11 @@ int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaS
     launch_layernorm(e->d_x, L.ln1_w, L.ln1_b, e->d_ln, B, H, d.ln_eps, H, st);
     launch_linear_rowgroup(e->d_ln, L.attn_w, L.attn_b, nullptr, e->d_qkv, B, e->qkv_cols, H, SV_ACT_NONE, st);
     if (e->v2)
-      launch_rope(e->d_qkv, B, 1, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, e->state, d.n_positions, 0, st);
-    launch_kv_append(e->d_qkv, kc, vc, e->state, B, d.n_head * D, d.n_kv_head, D, e->tcap, st);
+      launch_rope(e->d_qkv, B, 1, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, e->state, d.n_positions, 0, st,
+                  rows);
+    launch_kv_append(e->d_qkv, kc, vc, e->state, B, d.n_head * D, d.n_kv_head, D, e->tcap, st, rows);
     launch_attention_decode(e->d_qkv, e->qkv_cols, kc, vc, e->d_attn, e->attn_partial, e->state, B, d.n_head,
-                            d.n_kv_head, D, e->tcap, nsplit, e->window, st);
+                            d.n_kv_head, D, e->tcap, nsplit, e->window, st, rows);
     launch_linear_rowgroup(e->d_attn, L.proj_w, L.proj_b, e->d_x, e->d_x, B, H, H, SV_ACT_NONE, st);
     launch_layernorm(e->d_x, L.ln2_w, L.ln2_b, e->d_ln, B, H, d.ln_eps, H, st);
     launch_linear_rowgroup(e->d_ln, L.fc_w, L.fc_b, nullptr, e->d_h, B, d.n_inner, H, SV_ACT_GELU_TANH, st);
@@ -538,14 +556,15 @@ int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaS
 // Fused decode step: 5 kernels per layer (4 weight-ring GEMVs with fused LayerNorm / bias / GELU / residual / KV append,
 // 1 cluster attention) + lm_head, chained with programmatic dependent launch.  `ids` != nullptr embeds those tokens first
 // (teacher forcing / sampling); with nullptr, d_x was already written by select_fused.
-// Leaves bf16 logits in e->logits and per-tile argmax partials in e->amax_*.
-int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st) {
+// Leaves bf16 logits in e->logits and per-tile argmax partials in e->amax_*.  rows != nullptr: a session step.
+int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st,
+                            const RowState* rows = nullptr) {
   const sv_model_desc& d = e->d;
   const int H = d.hidden, D = d.head_dim;
-  if (ids) launch_embed_tokens(ids, e->wte, e->wpe, e->state, e->d_x, B, H, d.vocab, d.n_positions, st);
+  if (ids) launch_embed_tokens(ids, e->wte, e->wpe, e->state, e->d_x, B, H, d.vocab, d.n_positions, st, rows);
   bool first = true;
   RingGemvLaunch g{};
-  g.B = B; g.ln_eps = d.ln_eps; g.n_head = d.n_head; g.n_kv = d.n_kv_head; g.tcap = e->tcap; g.state = e->state;
+  g.B = B; g.ln_eps = d.ln_eps; g.n_head = d.n_head; g.n_kv = d.n_kv_head; g.tcap = e->tcap; g.state = e->state; g.rows = rows;
   g.amax_val = e->amax_val; g.amax_idx = e->amax_idx;
   auto gemv = [&](const bf16* X, const bf16* W, const uint8_t* Wt, const bf16* bias, const bf16* res, bf16* Y, int N, int K, int act,
                   const bf16* lw, const bf16* lb, int epi, bf16* kc, bf16* vc, bool p) {
@@ -563,9 +582,9 @@ int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, b
     first = false;
     if (e->v2)   // RoPE on q,k then append (the GEMV epilogue cannot rotate: the pair element lives in another tile)
       launch_rope_append(e->d_qkv, B, e->qkv_cols, d.n_head, d.n_kv_head, D, e->rope_cos, e->rope_sin, kc, vc, e->state,
-                         e->tcap, d.n_positions, pdl, st);
+                         e->tcap, d.n_positions, pdl, st, rows);
     launch_attention_decode_cluster(e->d_qkv, e->qkv_cols, kc, vc, e->d_attn, e->state, B, d.n_head, d.n_kv_head, D, e->tcap,
-                                    std::min(ncta, 8), e->window, pdl, st);
+                                    std::min(ncta, 8), e->window, pdl, st, rows);
     gemv(e->d_attn, L.proj_w, tl ? e->t_proj[i] : nullptr, L.proj_b, e->d_x, e->d_x, H, H, SV_ACT_NONE, nullptr, nullptr, 0, nullptr, nullptr, pdl);
     gemv(e->d_x, L.fc_w, tl ? e->t_fc[i] : nullptr, L.fc_b, nullptr, e->d_h, d.n_inner, H, SV_ACT_GELU_TANH, L.ln2_w, L.ln2_b, 0, nullptr, nullptr, pdl);
     gemv(e->d_h, L.fc2_w, tl ? e->t_fc2[i] : nullptr, L.fc2_b, e->d_x, e->d_x, H, d.n_inner, SV_ACT_NONE, nullptr, nullptr, 0, nullptr, nullptr, pdl);
@@ -617,6 +636,16 @@ void launch_select(sv_engine* e, int B, int do_sample, cudaStream_t st) {
   else
     launch_select_greedy(e->logits, e->d.vocab, B, e->state, e->params, e->seen, e->next_ids, e->out_ids, st);
 }
+
+// Entry points that use the cache as one rectangle of rows refuse to run while a session holds per-row state in it.
+int session_guard(sv_engine* e, const char* what) {
+  return e->session ? fail(e, SV_ERR_STATE, "%s: a decode session is open (call sv_session_end first)", what) : SV_OK;
+}
+#define SV_NO_SESSION(e, what)                 \
+  do {                                        \
+    int _g = session_guard((e), (what));      \
+    if (_g != SV_OK) return _g;               \
+  } while (0)
 
 int check_ready(sv_engine* e) {
   for (auto& kv : e->w)
@@ -802,6 +831,7 @@ void sv_engine_destroy(sv_engine* e) {
   for (void* p : e->allocs) cudaFree(p);
   if (e->host_flag) cudaFreeHost(e->host_flag);
   if (e->host_stream) cudaFreeHost(e->host_stream);
+  if (e->rows_host) cudaFreeHost(e->rows_host);
   if (e->gen_stream) cudaStreamDestroy(e->gen_stream);
   if (e->ev_in) cudaEventDestroy(e->ev_in);
   if (e->ev_t0) cudaEventDestroy(e->ev_t0);
@@ -812,6 +842,7 @@ void sv_engine_destroy(sv_engine* e) {
 int sv_engine_load_weight(sv_engine* e, const char* hf_name, const void* data, const int64_t* shape, int32_t ndim,
                           int32_t dtype) {
   if (!e || !hf_name || !data || !shape) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_engine_load_weight");    // rows admitted earlier would continue on other weights
   SV_CK(e, cudaSetDevice(e->device));
   LaunchScope scope(e);
   std::string name = hf_name;
@@ -874,6 +905,7 @@ int sv_engine_missing_weights(sv_engine* e) {
 
 int sv_encode_images(sv_engine* e, const void* pixels, int32_t batch, void* out_embeds, void* vit_out, void* stream) {
   if (!e || !pixels) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_encode_images");
   if (batch < 1 || batch > e->d.max_batch) return fail(e, SV_ERR_INVALID, "batch %d outside [1,%d]", batch, e->d.max_batch);
   int r = check_ready(e);
   if (r != SV_OK) return r;
@@ -895,6 +927,7 @@ int sv_encode_images(sv_engine* e, const void* pixels, int32_t batch, void* out_
 int sv_prefill(sv_engine* e, const int32_t* prompt_ids, int32_t batch, int32_t prompt_len, float* last_logits,
                void* stream) {
   if (!e || !prompt_ids) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_prefill");
   if (!e->encoded || batch != e->cur_batch) return fail(e, SV_ERR_STATE, "sv_prefill needs sv_encode_images with the same batch first");
   if (prompt_len < 1 || prompt_len > kMaxPrompt) return fail(e, SV_ERR_INVALID, "prompt_len %d outside [1,%d]", prompt_len, kMaxPrompt);
   if (e->Q + prompt_len + 1 > e->d.max_len) return fail(e, SV_ERR_INVALID, "prefix longer than max_len");
@@ -909,6 +942,7 @@ int sv_prefill(sv_engine* e, const int32_t* prompt_ids, int32_t batch, int32_t p
 int sv_prefill_embeds(sv_engine* e, const void* inputs_embeds, int32_t batch, int32_t seq_len, float* last_logits,
                       void* stream) {
   if (!e || !inputs_embeds) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_prefill_embeds");
   if (batch < 1 || batch > e->d.max_batch) return fail(e, SV_ERR_INVALID, "batch %d outside [1,%d]", batch, e->d.max_batch);
   if (seq_len < 1 || seq_len > e->Q + kMaxPrompt) return fail(e, SV_ERR_INVALID, "seq_len %d outside [1,%d]", seq_len, e->Q + kMaxPrompt);
   if (seq_len + 1 > e->d.max_len) return fail(e, SV_ERR_INVALID, "prefix longer than max_len");
@@ -925,6 +959,7 @@ int sv_prefill_embeds(sv_engine* e, const void* inputs_embeds, int32_t batch, in
 
 int sv_decode_step(sv_engine* e, const int32_t* ids, float* logits, void* stream) {
   if (!e || !ids) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_decode_step");
   if (!e->prefilled) return fail(e, SV_ERR_STATE, "sv_decode_step needs sv_prefill first");
   if (e->host_cur_len + 1 > e->d.max_len) return fail(e, SV_ERR_INVALID, "KV cache full (max_len %d)", e->d.max_len);
   SV_CK(e, cudaSetDevice(e->device));
@@ -957,6 +992,7 @@ int sv_decode_step(sv_engine* e, const int32_t* ids, float* logits, void* stream
 
 int sv_score_tokens(sv_engine* e, const int32_t* ids, int32_t batch, int32_t n_tokens, float* logprobs, void* stream) {
   if (!e || !ids || !logprobs) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_score_tokens");
   if (!e->prefilled) return fail(e, SV_ERR_STATE, "sv_score_tokens needs sv_prefill first");
   if (batch != e->cur_batch) return fail(e, SV_ERR_INVALID, "batch %d != the current batch %d", batch, e->cur_batch);
   if (n_tokens < 1) return fail(e, SV_ERR_INVALID, "n_tokens must be >= 1");
@@ -994,7 +1030,9 @@ int sv_score_tokens(sv_engine* e, const int32_t* ids, int32_t batch, int32_t n_t
 // (sv_generate_stream); with cb == NULL the code path is exactly sv_generate's.
 static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids, int32_t* out_len, void* stream,
                          sv_token_callback cb, void* cb_user) {
-  if (!e || !p || !out_ids) return fail(e, SV_ERR_INVALID, "null argument");
+  if (!e) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_generate");
+  if (!p || !out_ids) return fail(e, SV_ERR_INVALID, "null argument");
   if (!e->prefilled) return fail(e, SV_ERR_STATE, "sv_generate needs sv_prefill first");
   if (e->host_cur_len != e->prefix_len) return fail(e, SV_ERR_STATE, "sv_generate must directly follow sv_prefill");
   const int B = e->cur_batch, max_new = p->max_new_tokens;
@@ -1175,6 +1213,7 @@ int sv_generate_im2svg_host(sv_engine* e, const void* pixels_host, int32_t batch
                             int32_t prompt_len, const sv_gen_params* p, int32_t* out_ids_host, int32_t* out_len_host,
                             void* stream) {
   if (!e || !pixels_host || !prompt_ids_host || !p || !out_ids_host) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_generate_im2svg_host");
   if (batch < 1 || batch > e->d.max_batch) return fail(e, SV_ERR_INVALID, "batch %d outside [1,%d]", batch, e->d.max_batch);
   if (prompt_len < 1 || prompt_len > kMaxPrompt) return fail(e, SV_ERR_INVALID, "prompt_len outside [1,%d]", kMaxPrompt);
   SV_CK(e, cudaSetDevice(e->device));
@@ -1211,6 +1250,7 @@ int sv_generate_im2svg_host(sv_engine* e, const void* pixels_host, int32_t batch
 // candidates -> bookkeeping (+ next-token embeddings) -> KV suffix copies; the host replays it and polls `done`.
 int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_t* out_ids, int32_t* out_len, void* stream) {
   if (!e || !bp || !out_ids) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_beam_search");
   if (sv_beam_params_check_rows(bp, batch, e->d.max_batch) != SV_OK)
     return fail(e, SV_ERR_INVALID, "bad beam parameters (need num_beams >= 2, batch * num_beams <= max_batch (%d), max_new_tokens >= 1, "
                                    "n_stop_ids in [0,8], early_stopping in {0,1,2}, temperature > 0, repetition_penalty > 0)", e->d.max_batch);
@@ -1341,6 +1381,7 @@ int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_
 
 int sv_reorder_cache(sv_engine* e, const int32_t* src_rows, void* stream) {
   if (!e || !src_rows) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_reorder_cache");
   if (!e->prefilled) return fail(e, SV_ERR_STATE, "sv_reorder_cache needs a prefilled cache");
   SV_CK(e, cudaSetDevice(e->device));
   LaunchScope scope(e);
@@ -1359,6 +1400,7 @@ int sv_reorder_cache(sv_engine* e, const int32_t* src_rows, void* stream) {
 
 int sv_expand_batch(sv_engine* e, const int32_t* src_rows_host, int32_t new_batch, void* stream) {
   if (!e || !src_rows_host) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_expand_batch");
   if (!e->prefilled || e->host_cur_len != e->prefix_len) return fail(e, SV_ERR_STATE, "sv_expand_batch must directly follow sv_prefill");
   if (new_batch < 1 || new_batch > e->d.max_batch) return fail(e, SV_ERR_INVALID, "new_batch %d outside [1,%d]", new_batch, e->d.max_batch);
   for (int r = 0; r < new_batch; ++r)
@@ -1385,6 +1427,262 @@ int sv_expand_batch(sv_engine* e, const int32_t* src_rows_host, int32_t new_batc
   return finish_prefill_impl(e, new_batch, e->prefix_len, nullptr, st);     // fresh GenState for the new rows, exchange buffers cleared
 }
 
+// ---- continuous batching --------------------------------------------------------------------------------------------
+int sv_session_begin(sv_engine* e, const sv_gen_params* p, int32_t slots) {
+  if (!e || !p) return fail(e, SV_ERR_INVALID, "null argument");
+  if (e->session) return fail(e, SV_ERR_STATE, "a decode session is already open");
+  if (slots < 1 || slots > e->d.max_batch) return fail(e, SV_ERR_INVALID, "slots %d outside [1,%d]", slots, e->d.max_batch);
+  if (p->max_new_tokens < 1 || p->max_new_tokens > e->d.max_len)
+    return fail(e, SV_ERR_INVALID, "max_new_tokens %d outside [1,%d]", p->max_new_tokens, e->d.max_len);
+  if (p->n_stop_ids < 0 || p->n_stop_ids > 8) return fail(e, SV_ERR_INVALID, "n_stop_ids outside [0,8]");
+  if (p->do_sample && !(p->temperature > 0.f)) return fail(e, SV_ERR_INVALID, "temperature must be > 0");
+  if (!(p->repetition_penalty > 0.f)) return fail(e, SV_ERR_INVALID, "repetition_penalty must be > 0");
+  int r = check_ready(e);
+  if (r != SV_OK) return r;
+  SV_CK(e, cudaSetDevice(e->device));
+  LaunchScope scope(e);
+  const sv_model_desc& d = e->d;
+  if (!e->rows) {
+    bool ok = dev_alloc(e, &e->rows, 1) == cudaSuccess && dev_alloc(e, &e->sess_logits, (int64_t)d.max_batch * d.vocab) == cudaSuccess;
+    if (ok && !e->rows_host) ok = cudaMallocHost(reinterpret_cast<void**>(&e->rows_host), sizeof(RowState)) == cudaSuccess;
+    if (!ok) { e->rows = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the session state failed: %s", cudaGetErrorString(cudaGetLastError())); }
+  }
+  cudaStream_t st = e->gen_stream;
+  GenParamsDev hp;
+  memset(&hp, 0, sizeof(hp));
+  hp.max_new = p->max_new_tokens; hp.do_sample = p->do_sample; hp.eos_id = p->eos_token_id; hp.pad_id = p->pad_token_id;
+  hp.n_stop = p->n_stop_ids;
+  for (int i = 0; i < p->n_stop_ids; ++i) hp.stop_ids[i] = p->stop_ids[i];
+  hp.stop_row0_only = 0; hp.out_stride = d.max_len;
+  hp.temperature = p->temperature; hp.top_p = p->top_p; hp.rep_penalty = p->repetition_penalty; hp.seed = p->seed;
+  SV_CK(e, cudaMemcpyAsync(e->params, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));   // pageable: staged synchronously
+  SV_CK(e, cudaMemsetAsync(e->rows, 0, sizeof(RowState), st));
+  ensure_flow_tiles(e, st);      // SV_TILED=1: the ring GEMVs stream the slab-tiled weights, rebuilt after a weight load
+  SV_CK(e, cudaStreamSynchronize(st));
+  e->sess_p = *p;
+  e->sess_slots = slots;
+  e->sess_prompt_len = 0;
+  e->sess_live.assign(slots, 0);
+  e->sess_len.assign(slots, 0);
+  e->session = true;
+  e->encoded = false;        // admission overwrites the resident visual prefix and the cache rows
+  e->prefilled = false;
+  return SV_OK;
+}
+
+int sv_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t* prompt_ids, int32_t prompt_len,
+                     const int32_t* slots_host, const int32_t* max_new_host, const uint64_t* seeds_host,
+                     const int32_t* src_host, void* stream) {
+  if (!e || !pixels || !prompt_ids || !slots_host) return fail(e, SV_ERR_INVALID, "null argument");
+  if (!e->session) return fail(e, SV_ERR_STATE, "sv_session_admit needs sv_session_begin first");
+  const sv_model_desc& d = e->d;
+  const int S = e->sess_slots, cap = e->sess_p.max_new_tokens;
+  if (k < 1 || k > S) return fail(e, SV_ERR_INVALID, "k %d outside [1,%d]", k, S);
+  if (prompt_len < 1 || prompt_len > kMaxPrompt) return fail(e, SV_ERR_INVALID, "prompt_len %d outside [1,%d]", prompt_len, kMaxPrompt);
+  if (e->sess_prompt_len != 0 && prompt_len != e->sess_prompt_len)
+    return fail(e, SV_ERR_INVALID, "prompt_len %d differs from the session's %d (the split count of the decode graph is fixed by "
+                                   "prefix + max_new_tokens)", prompt_len, e->sess_prompt_len);
+  const int prefix = e->Q + prompt_len;
+  if (prefix + cap > d.max_len)
+    return fail(e, SV_ERR_INVALID, "prefix %d + max_new_tokens %d exceeds max_len %d", prefix, cap, d.max_len);
+  std::vector<int> used(S, 0);
+  int n_img = 0;
+  for (int j = 0; j < k; ++j) {
+    const int s = slots_host[j];
+    if (s < 0 || s >= S) return fail(e, SV_ERR_INVALID, "slot %d outside [0,%d)", s, S);
+    if (used[s] || e->sess_live[s]) return fail(e, SV_ERR_INVALID, "slot %d is busy or listed twice", s);
+    used[s] = 1;
+    if (max_new_host && (max_new_host[j] < 1 || max_new_host[j] > cap))
+      return fail(e, SV_ERR_INVALID, "max_new[%d] = %d outside [1,%d] (the session cap)", j, max_new_host[j], cap);
+    const int src = src_host ? src_host[j] : j;
+    if (src < 0 || src >= k) return fail(e, SV_ERR_INVALID, "src[%d] = %d outside [0,%d)", j, src, k);
+    n_img = std::max(n_img, src + 1);
+  }
+  SV_CK(e, cudaSetDevice(e->device));
+  LaunchScope scope(e);
+  cudaStream_t caller = (cudaStream_t)stream, st = e->gen_stream;
+  SV_CK(e, cudaEventRecord(e->ev_in, caller));
+  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  const int64_t img = (int64_t)3 * d.image_size * d.image_size, row_stride = (int64_t)d.n_kv_head * e->tcap * d.head_dim;
+  const size_t lrow = (size_t)d.vocab * sizeof(bf16);
+  uint32_t mask = 0;
+  // On an error below, the slots touched so far hold a partial admission; they are not marked live, so the caller may
+  // admit into them again (or end the session).
+  // Every image is encoded and prefilled on its own (B = 1): the same kernels, tilings and bits as a one-image generate.
+  // Batching the admitted images would change M-dependent tile choices of the prefill GEMMs and of the last-logits GEMV.
+  for (int i = 0; i < n_img; ++i) {
+    int first = -1;
+    for (int j = 0; j < k; ++j)
+      if ((src_host ? src_host[j] : j) == i) { first = slots_host[j]; break; }
+    if (first < 0) continue;
+    int r = run_encode(e, (const bf16*)pixels + i * img, 1, st);
+    if (r == SV_OK) r = run_prefill(e, e->visual, e->Q, prompt_ids + (int64_t)i * prompt_len, 1, prompt_len, st, first,
+                                    e->sess_logits + (int64_t)first * d.vocab);
+    if (r != SV_OK) return r;
+    for (int j = 0; j < k; ++j) {      // n completions of one image: its prefilled rows copied into the other slots
+      const int s = slots_host[j];
+      if ((src_host ? src_host[j] : j) != i || s == first) continue;
+      for (int l = 0; l < d.n_layer; ++l) {
+        bf16* kc = e->kcache + e->cache_layer_stride * l;
+        bf16* vc = e->vtcache + e->cache_layer_stride * l;
+        launch_kv_gather(kc + first * row_stride, vc + first * row_stride, kc + s * row_stride, vc + s * row_stride, nullptr, 1,
+                         d.n_kv_head, e->tcap, d.head_dim, prefix, st);
+      }
+      SV_CK(e, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(e->sess_logits) + s * lrow,
+                               reinterpret_cast<uint8_t*>(e->sess_logits) + first * lrow, lrow, cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  // the slots' own rows of the carried state (repetition-penalty set, output row, per-row fields), in one launch
+  SessionAdmit adm;
+  memset(&adm, 0, sizeof(adm));
+  adm.n = k;
+  for (int j = 0; j < k; ++j) {
+    const int s = slots_host[j];
+    adm.slot[j] = s;
+    adm.len[j] = prefix;
+    adm.max_new[j] = max_new_host ? max_new_host[j] : cap;
+    adm.seed[j] = seeds_host ? seeds_host[j] : e->sess_p.seed;
+    mask |= 1u << s;
+  }
+  launch_session_admit(e->rows, adm, e->seen, d.vocab, e->out_ids, d.max_len, e->sess_p.pad_token_id, st);
+  // token 0 of the admitted slots from their prefill logits (generate_impl's first select, no position advance)
+  if (e->sess_p.do_sample)
+    launch_select_sample(e->sess_logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, e->logits_f32, st,
+                         e->rows, mask, 0);
+  else if (e->fused_decode)
+    launch_select_fused(e->sess_logits, d.vocab, S, nullptr, e->amax_idx, gemv_ring_ntiles(d.vocab), 8 * ring_row_groups(S),
+                        e->state, e->params, e->seen, e->next_ids, e->out_ids, 0, e->wte, e->wpe, e->d_x, d.hidden,
+                        d.n_positions, false, st, e->rows, mask);
+  else
+    launch_select_greedy(e->sess_logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, st, e->rows, mask, 0);
+  SV_CK(e, cudaGetLastError());
+  SV_CK(e, cudaStreamSynchronize(st));     // the caller may release pixels / prompt_ids on return
+  for (int j = 0; j < k; ++j) e->sess_live[slots_host[j]] = 1;
+  e->sess_prompt_len = prompt_len;
+  return SV_OK;
+}
+
+int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int32_t* len_host, void* stream) {
+  if (!e) return fail(e, SV_ERR_INVALID, "null argument");
+  if (!e->session) return fail(e, SV_ERR_STATE, "sv_session_run needs sv_session_begin first");
+  if (max_steps < 0) return fail(e, SV_ERR_INVALID, "max_steps must be >= 0");
+  SV_CK(e, cudaSetDevice(e->device));
+  LaunchScope scope(e);
+  const sv_model_desc& d = e->d;
+  const int S = e->sess_slots;
+  cudaStream_t caller = (cudaStream_t)stream, st = e->gen_stream;
+  SV_CK(e, cudaEventRecord(e->ev_in, caller));
+  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  // the select kernels raise RowState::event when a row finishes (at admission too: a first token may end a row), so a
+  // poll reads that one word; the per-row fields are read once, at the end, and the event is cleared with them
+  auto poll_event = [&](bool& fin) -> int {
+    SV_CK(e, cudaMemcpyAsync(&e->rows_host->event, &e->rows->event, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    SV_CK(e, cudaStreamSynchronize(st));
+    fin = e->rows_host->event != 0;
+    return SV_OK;
+  };
+  bool any_live = false, any_fin = false;
+  for (int s = 0; s < S; ++s) any_live = any_live || e->sess_live[s];
+  int r = poll_event(any_fin);
+  if (r != SV_OK) return r;
+  int steps = 0;
+  if (!any_fin && any_live && max_steps > 0) {
+    ensure_flow_tiles(e, st);    // (no-op unless a weight was loaded since the tiles were built)
+    const bool fused = e->fused_decode, fused_select = fused && !e->sess_p.do_sample;
+    const int total = e->Q + e->sess_prompt_len + e->sess_p.max_new_tokens;     // the session cap fixes the split count
+    const int nsplit = fused ? attention_decode_cluster_ncta(total) : nsplit_for(e, total);
+    const long long key = (1LL << 40) + (long long)S * 100000 + nsplit * 8 + (e->sess_p.do_sample ? 1 : 0) + (fused ? 2 : 0) +
+                          (e->use_pdl ? 4 : 0);
+    GraphEntry& ge = e->graphs[key];
+    for (int attempt = 0; attempt < 2 && !ge.exec; ++attempt) {
+      const bool pdl = e->use_pdl && fused && attempt == 0;
+      int64_t counted = 0;
+      g_launch_counter = &counted;
+      cudaGraph_t graph = nullptr;
+      SV_CK(e, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+      int rr;
+      if (fused) rr = run_decode_layers_fused(e, fused_select ? nullptr : e->next_ids, S, nsplit, pdl, st, e->rows);
+      else rr = run_decode_layers(e, e->next_ids, S, nsplit, st, e->rows);
+      const uint32_t all = (1u << S) - 1u;
+      if (fused_select)
+        launch_select_fused(e->logits, d.vocab, S, e->amax_val, e->amax_idx, gemv_ring_ntiles(d.vocab), 8 * ring_row_groups(S),
+                            e->state, e->params, e->seen, e->next_ids, e->out_ids, 1, e->wte, e->wpe, e->d_x, d.hidden,
+                            d.n_positions, pdl, st, e->rows, all);
+      else if (e->sess_p.do_sample)
+        launch_select_sample(e->logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, e->logits_f32, st,
+                             e->rows, all, 1);
+      else
+        launch_select_greedy(e->logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, st, e->rows, all, 1);
+      cudaError_t ce = cudaStreamEndCapture(st, &graph);
+      g_launch_counter = &e->launches;
+      if (rr != SV_OK) { if (graph) cudaGraphDestroy(graph); return rr; }
+      if (ce == cudaSuccess) ce = cudaGraphInstantiate(&ge.exec, graph, 0);
+      if (graph) cudaGraphDestroy(graph);
+      if (ce != cudaSuccess) {
+        ge.exec = nullptr;
+        cudaGetLastError();
+        if (!pdl) SV_CK(e, ce);
+        e->use_pdl = false;
+        continue;
+      }
+      ge.kernels = (int)counted;
+    }
+    const int every = e->sess_p.poll_interval > 0 ? e->sess_p.poll_interval : 16;
+    while (steps < max_steps && !any_fin && any_live) {
+      const int n = std::min(every, max_steps - steps);
+      for (int i = 0; i < n; ++i) {
+        SV_CK(e, cudaGraphLaunch(ge.exec, st));
+        e->launches += ge.kernels;
+      }
+      steps += n;
+      r = poll_event(any_fin);
+      if (r != SV_OK) return r;
+    }
+  }
+  {
+    const size_t off = offsetof(RowState, row_step), n = offsetof(RowState, event) - off;   // row_step, row_active
+    SV_CK(e, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(e->rows_host) + off, reinterpret_cast<uint8_t*>(e->rows) + off, n,
+                             cudaMemcpyDeviceToHost, st));
+    SV_CK(e, cudaMemsetAsync(&e->rows->event, 0, sizeof(int32_t), st));
+    SV_CK(e, cudaStreamSynchronize(st));
+  }
+  SV_CK(e, cudaGetLastError());
+  for (int s = 0; s < S; ++s) {
+    const bool fin = e->sess_live[s] && !e->rows_host->row_active[s];
+    e->sess_len[s] = e->rows_host->row_step[s];
+    if (fin) e->sess_live[s] = 0;
+    if (finished_host) finished_host[s] = fin ? 1 : 0;
+    if (len_host) len_host[s] = e->sess_len[s];
+  }
+  return steps;
+}
+
+int sv_session_read(sv_engine* e, int32_t slot, int32_t* ids, void* stream) {
+  if (!e || !ids) return fail(e, SV_ERR_INVALID, "null argument");
+  if (!e->session) return fail(e, SV_ERR_STATE, "sv_session_read needs an open session");
+  if (slot < 0 || slot >= e->sess_slots) return fail(e, SV_ERR_INVALID, "slot %d outside [0,%d)", slot, e->sess_slots);
+  SV_CK(e, cudaSetDevice(e->device));
+  cudaStream_t st = e->gen_stream;
+  SV_CK(e, cudaEventRecord(e->ev_in, (cudaStream_t)stream));
+  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  const int n = e->sess_len[slot];
+  if (n > 0) SV_CK(e, cudaMemcpyAsync(ids, e->out_ids + (int64_t)slot * e->d.max_len, (size_t)n * 4, cudaMemcpyDefault, st));
+  SV_CK(e, cudaStreamSynchronize(st));
+  return n;
+}
+
+int sv_session_end(sv_engine* e) {
+  if (!e) return SV_ERR_INVALID;
+  if (!e->session) return fail(e, SV_ERR_STATE, "no decode session is open");
+  SV_CK(e, cudaSetDevice(e->device));
+  SV_CK(e, cudaStreamSynchronize(e->gen_stream));
+  e->session = false;
+  e->sess_slots = 0;
+  e->sess_live.clear();
+  e->sess_len.clear();
+  return SV_OK;
+}
+
 int64_t sv_launch_count(const sv_engine* e) { return e ? e->launches : 0; }
 
 int sv_debug_read_timeline(sv_engine* e, long long* out_host, int32_t n) {
@@ -1396,10 +1694,11 @@ int sv_debug_read_timeline(sv_engine* e, long long* out_host, int32_t n) {
 const char* sv_engine_describe(sv_engine* e) {
   if (!e) return "";
   char buf[512];
-  snprintf(buf, sizeof(buf), "decode=%s weights=%s attn=cluster-dsmem pdl=%d linear_impl=%d max_batch=%d flow[%s]%s",
+  snprintf(buf, sizeof(buf), "decode=%s weights=%s attn=cluster-dsmem pdl=%d linear_impl=%d max_batch=%d flow[%s]%s%s",
            !e->fused_decode ? "legacy-kernels" : e->use_flow ? (e->flow_realloc ? "dataflow-kernel-setmaxnreg" : "dataflow-kernel") : "ring-gemv-graph",
            e->ring_tiles ? "slab-tiled" : "row-major", (int)e->use_pdl, e->linear_impl, e->d.max_batch, decode_flow_status(),
-           e->flow_requested && !e->use_flow && e->d.max_batch > 8 ? " SV_FLOW ignored: the dataflow kernel holds 8 rows, max_batch > 8 runs the graph path" : "");
+           e->flow_requested && !e->use_flow && e->d.max_batch > 8 ? " SV_FLOW ignored: the dataflow kernel holds 8 rows, max_batch > 8 runs the graph path" : "",
+           e->use_flow ? " sessions: graph path (the dataflow kernel has no per-row positions)" : "");
   e->describe = buf;
   return e->describe.c_str();
 }

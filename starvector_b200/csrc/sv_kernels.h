@@ -28,6 +28,26 @@ struct GenParamsDev {
   unsigned long long seed;
 };
 
+// Per-row state of a continuous-batching session (sv_session_*): every cache row ("slot") has its own position, step,
+// token cap and Philox seed, and finishes on its own.  The kernels' session variants (the `rows` argument of the
+// launchers below) read positions from here instead of GenState::cur_len; GenState itself is left as it is (the
+// dataflow kernel copies it into shared memory).
+constexpr int kSessionRows = 16;
+struct RowState {
+  int32_t row_len[kSessionRows];      // tokens in the row's KV cache == position of the token fed next
+  int32_t row_step[kSessionRows];     // tokens generated == next free column of the row's out_ids
+  int32_t row_active[kSessionRows];   // 1 while the row decodes; the select kernels skip rows with 0
+  int32_t event;                      // set to 1 by the select kernels when a row finishes; the host polls and clears it
+  int32_t pad_;
+  int32_t row_max_new[kSessionRows];
+  unsigned long long row_seed[kSessionRows];
+};
+// The per-row fields of the slots one admission fills, passed by value to launch_session_admit.
+struct SessionAdmit {
+  int32_t n, slot[kSessionRows], len[kSessionRows], max_new[kSessionRows];
+  unsigned long long seed[kSessionRows];
+};
+
 // ---- sv_kernels_basic.cu
 void launch_layernorm(const bf16* x, const bf16* w, const bf16* b, bf16* y, int rows, int cols, float eps,
                       int64_t x_row_stride, cudaStream_t st);
@@ -44,22 +64,34 @@ void launch_batchnorm_tokens(const bf16* z, const bf16* w, const bf16* b, const 
 // rows [b][t] of x: visual[b][t] for t < q, else wte[prompt_ids[b * id_stride + t - q]]; + wpe[pos0 + t] when wpe != nullptr
 void launch_embed_prefix(const bf16* visual, const int32_t* prompt_ids, const bf16* wte, const bf16* wpe, bf16* x,
                          int batch, int q, int p, int h, int vocab, int pos0, int id_stride, cudaStream_t st);
+// rows != nullptr (here and below): the session variant, row b at position rows->row_len[b]
 void launch_embed_tokens(const int32_t* ids, const bf16* wte, const bf16* wpe, const GenState* state, bf16* x,
-                         int batch, int h, int vocab, int n_positions, cudaStream_t st);
+                         int batch, int h, int vocab, int n_positions, cudaStream_t st, const RowState* rows = nullptr);
 // K/V of qkv rows [b][0, seq) -> cache positions t0 .. t0+seq-1
 void launch_kv_scatter(const bf16* qkv, bf16* kcache, bf16* vtcache, int batch, int seq, int q_cols, int n_kv, int d,
                        int tcap, int t0, cudaStream_t st);
 void launch_kv_append(const bf16* qkv, bf16* kcache, bf16* vtcache, const GenState* state, int batch, int q_cols,
-                      int n_kv, int d, int tcap, cudaStream_t st);
+                      int n_kv, int d, int tcap, cudaStream_t st, const RowState* rows = nullptr);
 void launch_kv_gather(const bf16* ksrc, const bf16* vsrc, bf16* kdst, bf16* vdst, const int32_t* idx, int rows, int n_kv,
                       int tcap, int d, int len, cudaStream_t st);
 void launch_gather_rows(const bf16* x, bf16* y, int batch, int seq, int row, int h, cudaStream_t st);
 void launch_logits_to_float(const bf16* logits, float* out, int64_t n, cudaStream_t st);
+// Session variants (rows != nullptr): only rows b with bit b of row_mask set and rows->row_active[b] select a token; each
+// keeps its own bookkeeping (out_ids[b][row_step[b]], stop sequence over its own history, EOS / stop / row_max_new finish
+// the row and set rows->event, row_step += 1, row_len += advance_len); sampling draws from Philox(row_seed[b], 0,
+// row_step[b]), the stream a one-row generate with that seed uses.  GenState is not touched.
 void launch_select_greedy(const bf16* logits, int vocab, int batch, GenState* state, const GenParamsDev* params,
-                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, cudaStream_t st);
+                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, cudaStream_t st, RowState* rows = nullptr,
+                          uint32_t row_mask = 0, int advance_len = 0);
 void launch_select_sample(const bf16* logits, int vocab, int batch, GenState* state, const GenParamsDev* params,
-                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, float* probs, cudaStream_t st);
+                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, float* probs, cudaStream_t st,
+                          RowState* rows = nullptr, uint32_t row_mask = 0, int advance_len = 0);
 void launch_gen_finalize(GenState* state, const GenParamsDev* params, int batch, int advance_len, cudaStream_t st);
+// Admission of a.n session slots in one launch: for each slot a.slot[j], its repetition-penalty row seen[slot] is cleared,
+// its output row out_ids[slot][0, out_stride) filled with pad_id, and its RowState fields set (row_len = a.len[j],
+// row_step = 0, row_active = 1, row_max_new, row_seed).  Every other slot's rows are left as they are.
+void launch_session_admit(RowState* rows, const SessionAdmit& a, uint8_t* seen, int vocab, int32_t* out_ids, int out_stride,
+                          int pad_id, cudaStream_t st);
 void launch_advance_len(GenState* state, cudaStream_t st);
 void launch_fill_i32(int32_t* p, int32_t v, int n, cudaStream_t st);
 
@@ -105,14 +137,15 @@ cudaError_t launch_attention_chunk(const bf16* qkv, int q_cols_total, int q_rows
                                    int tcap, int window, cudaStream_t st);
 void launch_attention_decode(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache, bf16* out,
                              float* partial, const GenState* state, int batch, int n_head, int n_kv, int d, int tcap,
-                             int nsplit, int window, cudaStream_t st);
+                             int nsplit, int window, cudaStream_t st, const RowState* rows = nullptr);
 // RoPE in place on the q and k parts of packed qkv rows [rows][qkv_cols] (StarCoder2, rotate_half convention);
-// cos/sin tables are bf16 [max_pos][D/2]; position of row r = pos0 + (r % seq) or state->cur_len when state != nullptr.
+// cos/sin tables are bf16 [max_pos][D/2]; position of row r = pos0 + (r % seq) or state->cur_len when state != nullptr
+// (or row_pos->row_len[r] when row_pos != nullptr: the session variant, one token per row).
 void launch_rope(bf16* qkv, int rows, int seq, int qkv_cols, int n_rot_heads, int d, const bf16* cos_t, const bf16* sin_t,
-                 const GenState* state, int max_pos, int pos0, cudaStream_t st);
+                 const GenState* state, int max_pos, int pos0, cudaStream_t st, const RowState* row_pos = nullptr);
 void launch_rope_append(bf16* qkv, int batch, int qkv_cols, int n_head, int n_kv, int d, const bf16* cos_t,
                         const bf16* sin_t, bf16* kcache, bf16* vtcache, const GenState* state, int tcap, int max_pos,
-                        bool pdl, cudaStream_t st);
+                        bool pdl, cudaStream_t st, const RowState* rows = nullptr);
 void launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int d, float theta, cudaStream_t st);
 
 // decode attention (PDL-ready): the ncta <= 8 CTAs of one image form a thread-block cluster
@@ -120,13 +153,15 @@ int attention_decode_cluster_ncta(int total_len);
 cudaError_t attention_decode_cluster_init();
 cudaError_t launch_attention_decode_cluster(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache,
                                             bf16* out, const GenState* state, int batch, int n_head, int n_kv, int d,
-                                            int tcap, int ncta, int window, bool pdl, cudaStream_t st);
+                                            int tcap, int ncta, int window, bool pdl, cudaStream_t st,
+                                            const RowState* rows = nullptr);
 
 // ---- sv_decode_fused.cu : token selection fused with the next step's embedding, PDL-ready
+// rows != nullptr: the session variant (see launch_select_greedy); only the selecting rows' embeddings are written.
 void launch_select_fused(const bf16* logits, int vocab, int batch, const float* amax_val, const int* amax_idx,
                          int ntiles, int amax_stride, GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
                          int32_t* out_ids, int advance_len, const bf16* wte, const bf16* wpe, bf16* x, int h,
-                         int n_positions, bool pdl, cudaStream_t st);
+                         int n_positions, bool pdl, cudaStream_t st, RowState* rows = nullptr, uint32_t row_mask = 0);
 
 // ---- sv_decode_mega.cu : per-phase weight-ring decode GEMV; layer descriptor shared with sv_decode_flow.cu
 struct MegaLayer {
@@ -147,6 +182,7 @@ struct RingGemvLaunch {
   float* amax_val;
   int* amax_idx;
   bool pdl;
+  const RowState* rows;           // != nullptr with epi 1: the session variant, KV appended at rows->row_len[row]
 };
 cudaError_t gemv_ring_init();
 bool gemv_ring_supported(int K, bool has_ln);

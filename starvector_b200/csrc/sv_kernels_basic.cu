@@ -1,6 +1,7 @@
 // Elementwise / normalisation / layout kernels of the im2svg path (all HBM-bound, bf16 storage,
 // fp32 math).  Reference semantics are cited per kernel; rounding points follow DESIGN.md.
 #include "sv_kernels.h"
+#include "sv_select.cuh"
 
 namespace sv {
 
@@ -267,13 +268,16 @@ void launch_embed_prefix(const bf16* visual, const int32_t* prompt_ids, const bf
   count_launch();
 }
 
-__global__ void embed_tokens_kernel(const int32_t* __restrict__ ids, const bf16* __restrict__ wte,
-                                    const bf16* __restrict__ wpe, const GenState* __restrict__ state,
-                                    bf16* __restrict__ x, int h, int vocab, int n_positions) {
+// ROWS: the session variant (position of row b = rows->row_len[b]); the plain kernels instantiate ROWS = false.
+template <bool ROWS>
+SV_DEVINL void embed_tokens_body(const int32_t* __restrict__ ids, const bf16* __restrict__ wte,
+                                 const bf16* __restrict__ wpe, const GenState* __restrict__ state,
+                                 const RowState* __restrict__ rows, bf16* __restrict__ x, int h, int vocab,
+                                 int n_positions) {
   const int b = blockIdx.x;
   int id = ids[b];
   id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
-  int pos = state->cur_len;
+  int pos = ROWS ? rows->row_len[b] : state->cur_len;
   pos = pos >= n_positions ? n_positions - 1 : pos;
   const bf16* src = wte + (int64_t)id * h;
   const bf16* pe = wpe ? wpe + (int64_t)pos * h : nullptr;
@@ -288,9 +292,20 @@ __global__ void embed_tokens_kernel(const int32_t* __restrict__ ids, const bf16*
     *reinterpret_cast<uint4*>(x + (int64_t)b * h + c) = pack8(a);
   }
 }
+__global__ void embed_tokens_kernel(const int32_t* __restrict__ ids, const bf16* __restrict__ wte,
+                                    const bf16* __restrict__ wpe, const GenState* __restrict__ state,
+                                    bf16* __restrict__ x, int h, int vocab, int n_positions) {
+  embed_tokens_body<false>(ids, wte, wpe, state, nullptr, x, h, vocab, n_positions);
+}
+__global__ void embed_tokens_rows_kernel(const int32_t* __restrict__ ids, const bf16* __restrict__ wte,
+                                         const bf16* __restrict__ wpe, const RowState* __restrict__ rows,
+                                         bf16* __restrict__ x, int h, int vocab, int n_positions) {
+  embed_tokens_body<true>(ids, wte, wpe, nullptr, rows, x, h, vocab, n_positions);
+}
 void launch_embed_tokens(const int32_t* ids, const bf16* wte, const bf16* wpe, const GenState* state, bf16* x,
-                         int batch, int h, int vocab, int n_positions, cudaStream_t st) {
-  embed_tokens_kernel<<<batch, 128, 0, st>>>(ids, wte, wpe, state, x, h, vocab, n_positions);
+                         int batch, int h, int vocab, int n_positions, cudaStream_t st, const RowState* rows) {
+  if (rows) embed_tokens_rows_kernel<<<batch, 128, 0, st>>>(ids, wte, wpe, rows, x, h, vocab, n_positions);
+  else embed_tokens_kernel<<<batch, 128, 0, st>>>(ids, wte, wpe, state, x, h, vocab, n_positions);
   count_launch();
 }
 
@@ -316,9 +331,24 @@ void launch_kv_scatter(const bf16* qkv, bf16* kcache, bf16* vtcache, int batch, 
   kv_write_kernel<<<dim3(seq, batch), 128, 0, st>>>(qkv, kcache, vtcache, nullptr, t0, seq, q_cols, n_kv, d, tcap);
   count_launch();
 }
+// Session variant of the decode-step append: row b's K/V go to position rows->row_len[b].
+__global__ void kv_append_rows_kernel(const bf16* __restrict__ qkv, bf16* __restrict__ kcache, bf16* __restrict__ vtcache,
+                                      const RowState* __restrict__ rows, int q_cols, int n_kv, int d, int tcap) {
+  const int b = blockIdx.y;
+  const int t = rows->row_len[b];
+  if (t >= tcap) return;
+  const int cols = q_cols + 2 * n_kv * d;
+  const bf16* row = qkv + (int64_t)b * cols;
+  for (int i = threadIdx.x; i < n_kv * d; i += blockDim.x) {
+    int kvh = i / d, dim = i % d;
+    kcache[(((int64_t)b * n_kv + kvh) * tcap + t) * d + dim] = row[q_cols + i];
+    vtcache[(((int64_t)b * n_kv + kvh) * d + dim) * tcap + t] = row[q_cols + n_kv * d + i];
+  }
+}
 void launch_kv_append(const bf16* qkv, bf16* kcache, bf16* vtcache, const GenState* state, int batch, int q_cols,
-                      int n_kv, int d, int tcap, cudaStream_t st) {
-  kv_write_kernel<<<dim3(1, batch), 128, 0, st>>>(qkv, kcache, vtcache, state, 0, 1, q_cols, n_kv, d, tcap);
+                      int n_kv, int d, int tcap, cudaStream_t st, const RowState* rows) {
+  if (rows) kv_append_rows_kernel<<<dim3(1, batch), 128, 0, st>>>(qkv, kcache, vtcache, rows, q_cols, n_kv, d, tcap);
+  else kv_write_kernel<<<dim3(1, batch), 128, 0, st>>>(qkv, kcache, vtcache, state, 0, 1, q_cols, n_kv, d, tcap);
   count_launch();
 }
 
@@ -397,12 +427,17 @@ SV_DEVINL void append_token(int b, int tok, GenState* state, const GenParamsDev*
   }
 }
 
-__global__ void __launch_bounds__(1024) select_greedy_kernel(const bf16* __restrict__ logits, int vocab,
-                                                             GenState* state, const GenParamsDev* __restrict__ p,
-                                                             uint8_t* seen, int32_t* next_ids, int32_t* out_ids) {
-  if (state->done) return;
-  __shared__ ArgMax sm[32];
+template <bool ROWS>
+SV_DEVINL void select_greedy_body(const bf16* __restrict__ logits, int vocab, GenState* state,
+                                  const GenParamsDev* __restrict__ p, uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
+                                  RowState* rows, uint32_t row_mask, int advance_len) {
   const int b = blockIdx.x;
+  if constexpr (ROWS) {
+    if (!session_row_selects(rows, row_mask, b)) return;
+  } else {
+    if (state->done) return;
+  }
+  __shared__ ArgMax sm[32];
   const bf16* lr = logits + (int64_t)b * vocab;
   const uint8_t* sr = seen + (int64_t)b * vocab;
   const float rp = p->rep_penalty;
@@ -423,12 +458,28 @@ __global__ void __launch_bounds__(1024) select_greedy_kernel(const bf16* __restr
   if (threadIdx.x == 0) {
     for (int w = 1; w < 32; ++w) best = better(best, sm[w]);
     int tok = best.i == 0x7fffffff ? 0 : best.i;
-    append_token(b, tok, state, p, seen, vocab, next_ids, out_ids);
+    if constexpr (ROWS) session_append_token(b, tok, rows, p, seen, vocab, next_ids, out_ids, advance_len);
+    else append_token(b, tok, state, p, seen, vocab, next_ids, out_ids);
   }
 }
+__global__ void __launch_bounds__(1024) select_greedy_kernel(const bf16* __restrict__ logits, int vocab,
+                                                             GenState* state, const GenParamsDev* __restrict__ p,
+                                                             uint8_t* seen, int32_t* next_ids, int32_t* out_ids) {
+  select_greedy_body<false>(logits, vocab, state, p, seen, next_ids, out_ids, nullptr, 0u, 0);
+}
+__global__ void __launch_bounds__(1024) select_greedy_rows_kernel(const bf16* __restrict__ logits, int vocab,
+                                                                  RowState* rows, const GenParamsDev* __restrict__ p,
+                                                                  uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
+                                                                  uint32_t row_mask, int advance_len) {
+  select_greedy_body<true>(logits, vocab, nullptr, p, seen, next_ids, out_ids, rows, row_mask, advance_len);
+}
 void launch_select_greedy(const bf16* logits, int vocab, int batch, GenState* state, const GenParamsDev* params,
-                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, cudaStream_t st) {
-  select_greedy_kernel<<<batch, 1024, 0, st>>>(logits, vocab, state, params, seen, next_ids, out_ids);
+                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, cudaStream_t st, RowState* rows,
+                          uint32_t row_mask, int advance_len) {
+  if (rows)
+    select_greedy_rows_kernel<<<batch, 1024, 0, st>>>(logits, vocab, rows, params, seen, next_ids, out_ids, row_mask, advance_len);
+  else
+    select_greedy_kernel<<<batch, 1024, 0, st>>>(logits, vocab, state, params, seen, next_ids, out_ids);
   count_launch();
 }
 
@@ -455,16 +506,19 @@ SV_DEVINL float philox_uniform(unsigned long long seed, uint32_t c0, uint32_t c1
 
 constexpr int kSampleThreads = 1024;
 // `probs` is an fp32 scratch row [B][vocab] (L2 resident): the kernel makes ~34 passes over it.
-__global__ void __launch_bounds__(kSampleThreads) select_sample_kernel(const bf16* __restrict__ logits, int vocab,
-                                                                       GenState* state,
-                                                                       const GenParamsDev* __restrict__ p,
-                                                                       uint8_t* seen, int32_t* next_ids,
-                                                                       int32_t* out_ids, float* __restrict__ probs) {
-  if (state->done) return;
+template <bool ROWS>
+SV_DEVINL void select_sample_body(const bf16* __restrict__ logits, int vocab, GenState* state,
+                                  const GenParamsDev* __restrict__ p, uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
+                                  float* __restrict__ probs, RowState* rows, uint32_t row_mask, int advance_len) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  if constexpr (ROWS) {
+    if (!session_row_selects(rows, row_mask, b)) return;
+  } else {
+    if (state->done) return;
+  }
   __shared__ float smf[32];
   __shared__ float s_bcast;
   __shared__ int s_tok;
-  const int b = blockIdx.x, tid = threadIdx.x;
   const bf16* lr = logits + (int64_t)b * vocab;
   const uint8_t* sr = seen + (int64_t)b * vocab;
   float* pr = probs + (int64_t)b * vocab;
@@ -514,7 +568,12 @@ __global__ void __launch_bounds__(kSampleThreads) select_sample_kernel(const bf1
   __syncthreads();
   float base = 0.f, total = 0.f;
   for (int w = 0; w < 32; ++w) { if (w < (tid >> 5)) base += smf[w]; total += smf[w]; }
-  if (tid == 0) { s_bcast = philox_uniform(p->seed, (uint32_t)b, (uint32_t)state->step) * total; s_tok = -1; }
+  if (tid == 0) {
+    // session rows: the counter of a one-row generate with the row's own seed (the slot index does not enter it)
+    if constexpr (ROWS) s_bcast = philox_uniform(rows->row_seed[b], 0u, (uint32_t)rows->row_step[b]) * total;
+    else s_bcast = philox_uniform(p->seed, (uint32_t)b, (uint32_t)state->step) * total;
+    s_tok = -1;
+  }
   __syncthreads();
   const float target = s_bcast;
   const float excl = base + incl - own;
@@ -533,12 +592,33 @@ __global__ void __launch_bounds__(kSampleThreads) select_sample_kernel(const bf1
       for (int i = vocab - 1; i >= 0; --i) if (pr[i] * invz > lo) { tok = i; break; }
       if (tok < 0) tok = 0;
     }
-    append_token(b, tok, state, p, seen, vocab, next_ids, out_ids);
+    if constexpr (ROWS) session_append_token(b, tok, rows, p, seen, vocab, next_ids, out_ids, advance_len);
+    else append_token(b, tok, state, p, seen, vocab, next_ids, out_ids);
   }
 }
+__global__ void __launch_bounds__(kSampleThreads) select_sample_kernel(const bf16* __restrict__ logits, int vocab,
+                                                                       GenState* state,
+                                                                       const GenParamsDev* __restrict__ p,
+                                                                       uint8_t* seen, int32_t* next_ids,
+                                                                       int32_t* out_ids, float* __restrict__ probs) {
+  select_sample_body<false>(logits, vocab, state, p, seen, next_ids, out_ids, probs, nullptr, 0u, 0);
+}
+__global__ void __launch_bounds__(kSampleThreads) select_sample_rows_kernel(const bf16* __restrict__ logits, int vocab,
+                                                                            RowState* rows,
+                                                                            const GenParamsDev* __restrict__ p,
+                                                                            uint8_t* seen, int32_t* next_ids,
+                                                                            int32_t* out_ids, float* __restrict__ probs,
+                                                                            uint32_t row_mask, int advance_len) {
+  select_sample_body<true>(logits, vocab, nullptr, p, seen, next_ids, out_ids, probs, rows, row_mask, advance_len);
+}
 void launch_select_sample(const bf16* logits, int vocab, int batch, GenState* state, const GenParamsDev* params,
-                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, float* probs, cudaStream_t st) {
-  select_sample_kernel<<<batch, kSampleThreads, 0, st>>>(logits, vocab, state, params, seen, next_ids, out_ids, probs);
+                          uint8_t* seen, int32_t* next_ids, int32_t* out_ids, float* probs, cudaStream_t st,
+                          RowState* rows, uint32_t row_mask, int advance_len) {
+  if (rows)
+    select_sample_rows_kernel<<<batch, kSampleThreads, 0, st>>>(logits, vocab, rows, params, seen, next_ids, out_ids, probs,
+                                                                row_mask, advance_len);
+  else
+    select_sample_kernel<<<batch, kSampleThreads, 0, st>>>(logits, vocab, state, params, seen, next_ids, out_ids, probs);
   count_launch();
 }
 
@@ -557,6 +637,25 @@ __global__ void gen_finalize_kernel(GenState* state, const GenParamsDev* __restr
 }
 void launch_gen_finalize(GenState* state, const GenParamsDev* params, int batch, int advance_len, cudaStream_t st) {
   gen_finalize_kernel<<<1, 32, 0, st>>>(state, params, batch, advance_len);
+  count_launch();
+}
+__global__ void session_admit_kernel(RowState* rows, const SessionAdmit a, uint8_t* seen, int vocab, int32_t* out_ids,
+                                     int out_stride, int pad_id) {
+  const int j = blockIdx.x, s = a.slot[j];
+  for (int i = threadIdx.x; i < vocab; i += blockDim.x) seen[(int64_t)s * vocab + i] = 0;
+  for (int i = threadIdx.x; i < out_stride; i += blockDim.x) out_ids[(int64_t)s * out_stride + i] = pad_id;
+  if (threadIdx.x == 0) {
+    rows->row_len[s] = a.len[j];
+    rows->row_step[s] = 0;
+    rows->row_active[s] = 1;
+    rows->row_max_new[s] = a.max_new[j];
+    rows->row_seed[s] = a.seed[j];
+  }
+}
+void launch_session_admit(RowState* rows, const SessionAdmit& a, uint8_t* seen, int vocab, int32_t* out_ids, int out_stride,
+                          int pad_id, cudaStream_t st) {
+  if (a.n <= 0) return;
+  session_admit_kernel<<<a.n, 256, 0, st>>>(rows, a, seen, vocab, out_ids, out_stride, pad_id);
   count_launch();
 }
 __global__ void advance_len_kernel(GenState* state) {
@@ -584,11 +683,12 @@ void launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int d, float theta
   rope_table_kernel<<<(n + 255) / 256, 256, 0, st>>>(cos_t, sin_t, max_pos, d / 2, theta);
   count_launch();
 }
-__global__ void rope_kernel(bf16* __restrict__ qkv, int seq, int qkv_cols, int n_rot_heads, int d,
-                            const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
-                            const GenState* __restrict__ state, int max_pos, int pos0) {
+template <bool ROWS>
+SV_DEVINL void rope_body(bf16* __restrict__ qkv, int seq, int qkv_cols, int n_rot_heads, int d,
+                         const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                         const GenState* __restrict__ state, const RowState* __restrict__ rows, int max_pos, int pos0) {
   const int row = blockIdx.x, half = d >> 1;
-  int pos = state ? state->cur_len : pos0 + (row % seq);
+  int pos = ROWS ? rows->row_len[row] : (state ? state->cur_len : pos0 + (row % seq));
   pos = pos >= max_pos ? max_pos - 1 : pos;
   bf16* base = qkv + (int64_t)row * qkv_cols;
   for (int i = threadIdx.x; i < n_rot_heads * half; i += blockDim.x) {
@@ -600,16 +700,28 @@ __global__ void rope_kernel(bf16* __restrict__ qkv, int seq, int qkv_cols, int n
     v[j + half] = __float2bfloat16_rn(bf16_round(x2 * c) + bf16_round(x1 * s));
   }
 }
+__global__ void rope_kernel(bf16* __restrict__ qkv, int seq, int qkv_cols, int n_rot_heads, int d,
+                            const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                            const GenState* __restrict__ state, int max_pos, int pos0) {
+  rope_body<false>(qkv, seq, qkv_cols, n_rot_heads, d, cos_t, sin_t, state, nullptr, max_pos, pos0);
+}
+__global__ void rope_rows_kernel(bf16* __restrict__ qkv, int qkv_cols, int n_rot_heads, int d,
+                                 const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                                 const RowState* __restrict__ rows, int max_pos) {
+  rope_body<true>(qkv, 1, qkv_cols, n_rot_heads, d, cos_t, sin_t, nullptr, rows, max_pos, 0);
+}
 // Decode-step companion of the fused QKV GEMV for RoPE models: rotate q in place, rotate k and append it (and v) to the
-// KV cache at position cur_len.  One block per image.
-__global__ void rope_append_kernel(bf16* __restrict__ qkv, int qkv_cols, int n_head, int n_kv, int d,
-                                   const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
-                                   bf16* __restrict__ kcache, bf16* __restrict__ vtcache,
-                                   const GenState* __restrict__ state, int tcap, int max_pos) {
+// KV cache at position cur_len (ROWS: rows->row_len[b]).  One block per image.
+template <bool ROWS>
+SV_DEVINL void rope_append_body(bf16* __restrict__ qkv, int qkv_cols, int n_head, int n_kv, int d,
+                                const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                                bf16* __restrict__ kcache, bf16* __restrict__ vtcache,
+                                const GenState* __restrict__ state, const RowState* __restrict__ rows, int tcap,
+                                int max_pos) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
   const int b = blockIdx.x, half = d >> 1;
-  const int pos = state->cur_len;
+  const int pos = ROWS ? rows->row_len[b] : state->cur_len;
   const int tp = pos >= max_pos ? max_pos - 1 : pos;
   bf16* base = qkv + (int64_t)b * qkv_cols;
   for (int i = threadIdx.x; i < (n_head + n_kv) * half; i += blockDim.x) {
@@ -635,23 +747,40 @@ __global__ void rope_append_kernel(bf16* __restrict__ qkv, int qkv_cols, int n_h
     }
   }
 }
+__global__ void rope_append_kernel(bf16* __restrict__ qkv, int qkv_cols, int n_head, int n_kv, int d,
+                                   const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                                   bf16* __restrict__ kcache, bf16* __restrict__ vtcache,
+                                   const GenState* __restrict__ state, int tcap, int max_pos) {
+  rope_append_body<false>(qkv, qkv_cols, n_head, n_kv, d, cos_t, sin_t, kcache, vtcache, state, nullptr, tcap, max_pos);
+}
+__global__ void rope_append_rows_kernel(bf16* __restrict__ qkv, int qkv_cols, int n_head, int n_kv, int d,
+                                        const bf16* __restrict__ cos_t, const bf16* __restrict__ sin_t,
+                                        bf16* __restrict__ kcache, bf16* __restrict__ vtcache,
+                                        const RowState* __restrict__ rows, int tcap, int max_pos) {
+  rope_append_body<true>(qkv, qkv_cols, n_head, n_kv, d, cos_t, sin_t, kcache, vtcache, nullptr, rows, tcap, max_pos);
+}
 void launch_rope_append(bf16* qkv, int batch, int qkv_cols, int n_head, int n_kv, int d, const bf16* cos_t,
                         const bf16* sin_t, bf16* kcache, bf16* vtcache, const GenState* state, int tcap, int max_pos,
-                        bool pdl, cudaStream_t st) {
+                        bool pdl, cudaStream_t st, const RowState* rows) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(batch); cfg.blockDim = dim3(256); cfg.stream = st;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, rope_append_kernel, qkv, qkv_cols, n_head, n_kv, d, cos_t, sin_t, kcache, vtcache, state, tcap,
-                     max_pos);
+  if (rows)
+    cudaLaunchKernelEx(&cfg, rope_append_rows_kernel, qkv, qkv_cols, n_head, n_kv, d, cos_t, sin_t, kcache, vtcache, rows,
+                       tcap, max_pos);
+  else
+    cudaLaunchKernelEx(&cfg, rope_append_kernel, qkv, qkv_cols, n_head, n_kv, d, cos_t, sin_t, kcache, vtcache, state, tcap,
+                       max_pos);
   count_launch();
 }
 
 void launch_rope(bf16* qkv, int rows, int seq, int qkv_cols, int n_rot_heads, int d, const bf16* cos_t, const bf16* sin_t,
-                 const GenState* state, int max_pos, int pos0, cudaStream_t st) {
-  rope_kernel<<<rows, 256, 0, st>>>(qkv, seq, qkv_cols, n_rot_heads, d, cos_t, sin_t, state, max_pos, pos0);
+                 const GenState* state, int max_pos, int pos0, cudaStream_t st, const RowState* row_pos) {
+  if (row_pos) rope_rows_kernel<<<rows, 256, 0, st>>>(qkv, qkv_cols, n_rot_heads, d, cos_t, sin_t, row_pos, max_pos);
+  else rope_kernel<<<rows, 256, 0, st>>>(qkv, seq, qkv_cols, n_rot_heads, d, cos_t, sin_t, state, max_pos, pos0);
   count_launch();
 }
 

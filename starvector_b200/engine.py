@@ -8,7 +8,7 @@ from __future__ import annotations
 import ctypes as C
 import dataclasses
 import threading
-from typing import Dict, Iterable, Optional, Sequence, Tuple
+from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -310,6 +310,70 @@ class Engine:
             self._batch = B
         n_gen = int(olen[0])
         return out[:, :n_gen], n_gen
+
+    # -- continuous batching (sv_session_*) -----------------------------------------------------
+    def generate_requests(self, pixels: torch.Tensor, prompt_ids: torch.Tensor, params: GenerationParams, *,
+                          max_new_tokens: Optional[Sequence[int]] = None, seeds: Optional[Sequence[int]] = None, n: int = 1,
+                          on_finish=None, slots: Optional[int] = None) -> List[torch.Tensor]:
+        """Continuous batching over any number of images: a decode session of `slots` (default `max_batch`) cache rows,
+        refilled with the next queued image whenever a row finishes (`ContinuousScheduler`).  Completion j of image i
+        (index i * n + j of the returned list, int32 on the CPU) holds exactly the tokens a one-image `generate` of image i
+        with `params` (seed `seeds[i * n + j]`, default `params.seed + i * n + j`, and `max_new_tokens[i]` new tokens at most)
+        returns.  `params.max_new_tokens` is the session cap; `on_finish(index, ids)` streams results as they complete."""
+        from .continuous import ContinuousScheduler
+
+        return ContinuousScheduler(self, slots).run(pixels, prompt_ids, params, max_new_tokens=max_new_tokens, seeds=seeds,
+                                                    n=n, on_finish=on_finish)
+
+    def session_begin(self, params: GenerationParams, slots: int) -> None:
+        cp = params.to_c()
+        with self._lock:
+            self._ck(self._lib.sv_session_begin(self._h, C.byref(cp), int(slots)))
+            self._session_slots = int(slots)
+            self._batch = 0
+
+    def session_admit(self, pixels: torch.Tensor, prompt_ids: torch.Tensor, slots: Sequence[int], *,
+                      max_new_tokens: Optional[Sequence[int]] = None, seeds: Optional[Sequence[int]] = None,
+                      src: Optional[Sequence[int]] = None) -> None:
+        """Encode and prefill images `[n_img, 3, S, S]` (prompts `[n_img, P]`) into free `slots`; `src[j]` is the image of
+        slots[j] (default j), so one image may fill several slots (n completions, prefilled once)."""
+        d = self.dims
+        if pixels.dim() != 4 or tuple(pixels.shape[1:]) != (3, d.image_size, d.image_size):
+            raise ValueError(f"image batch must be [B,3,{d.image_size},{d.image_size}], got {tuple(pixels.shape)}")
+        px = self._dev(pixels, torch.bfloat16)
+        ids = self._dev(prompt_ids, torch.int32)
+        k = len(slots)
+        def arr(t, v, mask=None):
+            return None if v is None else (t * k)(*[int(x) & mask if mask else int(x) for x in v])
+
+        sl, mx, sr = arr(C.c_int32, slots), arr(C.c_int32, max_new_tokens), arr(C.c_int32, src)
+        sd = arr(C.c_uint64, seeds, 2 ** 64 - 1)
+        with self._lock:
+            self._ck(self._lib.sv_session_admit(self._h, C.c_void_p(px.data_ptr()), k, C.c_void_p(ids.data_ptr()), ids.shape[1],
+                                                sl, mx, sd, sr, _stream_ptr(self.device)))
+
+    def session_run(self, max_steps: int) -> Tuple[int, List[bool], List[int]]:
+        """Replay decode steps until a slot finishes: (steps run, finished flag per slot, tokens per slot)."""
+        S = self._session_slots
+        fin, ln = (C.c_int32 * S)(), (C.c_int32 * S)()
+        with self._lock:
+            r = self._lib.sv_session_run(self._h, int(max_steps), fin, ln, _stream_ptr(self.device))
+            if r < 0:
+                self._ck(r)
+        return int(r), [bool(v) for v in fin], [int(v) for v in ln]
+
+    def session_read(self, slot: int) -> torch.Tensor:
+        """The tokens of `slot` as of the last `session_run` (int32, CPU)."""
+        out = torch.empty(self.dims.max_len, dtype=torch.int32)
+        with self._lock:
+            r = self._lib.sv_session_read(self._h, int(slot), C.c_void_p(out.data_ptr()), _stream_ptr(self.device))
+            if r < 0:
+                self._ck(r)
+        return out[:r].clone()
+
+    def session_end(self) -> None:
+        with self._lock:
+            self._ck(self._lib.sv_session_end(self._h))
 
     # -- introspection -------------------------------------------------------------------
     def launch_count(self) -> int:

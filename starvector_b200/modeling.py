@@ -296,6 +296,31 @@ class StarVectorStarCoder:
         ids = self.generate_im2svg_ids(batch, **kwargs)
         return self.svg_transformer.tokenizer.batch_decode(ids, skip_special_tokens=True)          # :257
 
+    @torch.no_grad()
+    def generate_im2svg_continuous(self, batch: Dict[str, torch.Tensor], **kwargs) -> List[str]:
+        """`generate_im2svg` over any number of images with continuous batching (`Engine.generate_requests`): the engine's
+        `max_batch` cache rows are refilled with the next image as soon as a row finishes, instead of running groups of
+        `max_batch` that each last as long as their longest member.  Takes the kwargs of `generate_im2svg` (max_length,
+        use_nucleus_sampling, temperature, top_p, repetition_penalty, prompt, seed, num_return_sequences).  Every image's
+        completion is what `generate_im2svg({"image": image[k:k+1]}, num_beams=1, seed=seed + k, ...)` returns (the
+        `</svg>` stop and EOS end each row on its own); completion j of image i (num_return_sequences = G) is request
+        k = i * G + j.  Returns prompt + completion strings in that order."""
+        num_beams = int(kwargs.get("num_beams", 1))
+        if num_beams > 1:
+            raise NotImplementedError("generate_im2svg_continuous decodes one beam per request; beam search has no "
+                                      "continuous-batching form (pass num_beams=1 or use generate_im2svg)")
+        image = batch["image"]
+        N = image.shape[0]
+        G = int(kwargs.get("num_return_sequences", 1))
+        if G < 1:
+            raise ValueError("num_return_sequences must be >= 1")
+        prompt_ids = self._tokenize_prompt(kwargs.get("prompt"), 1)
+        params = self._gen_params(kwargs, prefix_len=self.query_length + prompt_ids.shape[1])
+        outs = self.engine.generate_requests(image, prompt_ids[0], params, n=G)
+        tok = self.svg_transformer.tokenizer
+        p0 = prompt_ids[0].cpu().long()
+        return tok.batch_decode([torch.cat([p0, o.long()]) for o in outs], skip_special_tokens=True)
+
     def generate_im2svg_grpo(self, batch, **kwargs):                                               # :261-286
         """`num_return_sequences` completions per image (sampled independently, `num_beams` forced to 1, :277-280):
         HF's `_expand_inputs_for_generation` = every image row repeated G times, adjacent — here the image is encoded and
@@ -486,6 +511,9 @@ class StarVectorForCausalLM:
     # -- the surface ---------------------------------------------------------------------
     def generate_im2svg(self, batch, **kwargs) -> List[str]:                  # starvector_arch.py:186-187
         return self.model.generate_im2svg(batch, **kwargs)
+
+    def generate_im2svg_continuous(self, batch, **kwargs) -> List[str]:
+        return self.model.generate_im2svg_continuous(batch, **kwargs)
 
     def generate_im2text(self, batch, **kwargs):                              # :189-190 (dangling in the reference too)
         raise AttributeError("generate_im2text has no implementation in the reference model core either")
