@@ -292,6 +292,44 @@ SV_API int sv_op_attention_chunk(const void* qkv, void* out, int32_t batch, int3
 SV_API int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets, float* logprob, int32_t M, int32_t N,
                             int32_t K, void* stream);
 
+/* The decode-step kernels one at a time, over caches the caller fills (D = 128; kcache [batch][n_kv][tcap][D], vtcache
+ * [batch][n_kv][D][tcap], packed qkv rows [batch][(n_head + 2 n_kv) * D]).  Every argument is checked on the host:
+ * SV_ERR_INVALID before any launch.  Synchronous on `stream`. */
+enum { SV_ATTN_DECODE_SPLIT = 0 /* split + merge, nsplit in [1, 128] */, SV_ATTN_DECODE_CLUSTER = 1 /* nsplit = CTAs in [1, 8] */ };
+/* Decode attention: row b's query (qkv row b) attends to keys [0, lens_host[b]) of its cache (the last, lens - 1, is the
+ * new token; keys > lens - 1 - window when window > 0) -> out [batch][n_head * D].  per_row = 0: the plain kernels
+ * (equal lengths); 1: the session kernels.  1 <= lens <= tcap, tcap % 32 == 0, batch <= 16, n_head / n_kv <= 16. */
+SV_API int sv_op_attention_decode(int32_t impl, int32_t per_row, const void* qkv, const void* kcache, const void* vtcache,
+                                  void* out, const int32_t* lens_host, int32_t batch, int32_t n_head, int32_t n_kv,
+                                  int32_t tcap, int32_t nsplit, int32_t window, void* stream);
+/* One weight-ring GEMV launch: y[B,N] = epi(LN?(x)[B,K] . w[N,K]^T) with the decode step's rounding points. */
+typedef struct sv_op_ring {
+  const void *x, *w, *bias, *residual; /* residual may alias y (in place) */
+  const void *ln_w, *ln_b;             /* both NULL: no LayerNorm */
+  void* y;
+  int32_t B, N, K, act;
+  int32_t epi;                         /* 0 plain, 1 QKV + KV append (needs LN), 2 lm_head + argmax partials (needs LN) */
+  int32_t tiled;                       /* 1: stream a slab-tiled copy of w (built by the call) instead of w's rows */
+  float ln_eps;
+  void *kcache, *vtcache;              /* epi 1 */
+  int32_t n_head, n_kv, tcap, per_row;
+  const int32_t* pos_host;             /* epi 1: the append position (per_row = 0: [0] for every row; 1: one per row) */
+  float* amax_val;                     /* epi 2: [sv_op_ring_ntiles(N)][sv_op_ring_row_stride(B)] */
+  int32_t* amax_idx;
+} sv_op_ring;
+SV_API int sv_op_gemv_ring(const sv_op_ring* args, void* stream);
+SV_API int32_t sv_op_ring_ntiles(int32_t N);
+SV_API int32_t sv_op_ring_row_stride(int32_t B);
+/* The bf16 RoPE tables cos/sin [max_pos][d / 2] the engine builds for theta. */
+SV_API int sv_op_rope_table(void* cos_t, void* sin_t, int32_t max_pos, int32_t d, float theta, void* stream);
+/* RoPE in place on the q and k heads of packed qkv [rows][(n_head + 2 n_kv) * D] (positions >= max_pos use max_pos - 1).
+ * pos_host == NULL: the prefill kernel, row r at pos0 + r % seq.  Otherwise one token per row at pos_host[0] (per_row = 0,
+ * equal positions) or pos_host[r] (per_row = 1); with kcache != NULL the append kernel: q rotated in place, rotated k
+ * and v written to the caches at the row's position when it is < tcap. */
+SV_API int sv_op_rope(void* qkv, const void* cos_t, const void* sin_t, int32_t rows, int32_t seq, int32_t n_head,
+                      int32_t n_kv, int32_t max_pos, int32_t pos0, const int32_t* pos_host, int32_t per_row, void* kcache,
+                      void* vtcache, int32_t tcap, void* stream);
+
 /* ---- image preprocessing (SURVEY.md §8f-2) ------------------------------------------------ */
 /* Replaces `ImageTrainProcessor.__call__` (reference starvector/data/util.py:40-66: RGBA pasted on white, pad to
  * square with 255, `transforms.Resize(size, BICUBIC)` on the PIL image, ToTensor, Normalize) and

@@ -56,7 +56,18 @@ class ImageU8(C.Structure):
                 ("row_stride", C.c_int32)]
 
 
-TOKEN_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32)   # sv_token_callback
+SV_ATTN_DECODE_SPLIT, SV_ATTN_DECODE_CLUSTER = 0, 1
+
+
+class OpRing(C.Structure):   # sv_op_ring
+    _fields_ = [(n, C.c_void_p) for n in ("x", "w", "bias", "residual", "ln_w", "ln_b", "y")] + [
+        (n, C.c_int32) for n in ("B", "N", "K", "act", "epi", "tiled")] + [
+        ("ln_eps", C.c_float), ("kcache", C.c_void_p), ("vtcache", C.c_void_p)] + [
+        (n, C.c_int32) for n in ("n_head", "n_kv", "tcap", "per_row")] + [
+        ("pos_host", C.POINTER(C.c_int32)), ("amax_val", C.c_void_p), ("amax_idx", C.c_void_p)]
+
+
+TOKEN_CALLBACK =C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32)   # sv_token_callback
 
 # name -> (restype, argtypes); must list every SV_API symbol of the header (tests check this)
 _P, _I, _F = C.c_void_p, C.c_int32, C.c_float
@@ -104,6 +115,12 @@ SIGNATURES = {
     "sv_op_attention_mqa": (C.c_int, [_P, _P, _I, _I, _I, _P]),
     "sv_op_attention_chunk": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "sv_op_lm_logprob": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "sv_op_attention_decode": (C.c_int, [_I, _I, _P, _P, _P, _P, C.POINTER(_I), _I, _I, _I, _I, _I, _I, _P]),
+    "sv_op_gemv_ring": (C.c_int, [C.POINTER(OpRing), _P]),
+    "sv_op_ring_ntiles": (C.c_int32, [_I]),
+    "sv_op_ring_row_stride": (C.c_int32, [_I]),
+    "sv_op_rope_table": (C.c_int, [_P, _P, _I, _I, _F, _P]),
+    "sv_op_rope": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, C.POINTER(_I), _I, _P, _P, _I, _P]),
     "sv_preproc_create": (C.c_int, [C.POINTER(PreprocDesc), C.c_int, C.POINTER(_P)]),
     "sv_preproc_destroy": (None, [_P]),
     "sv_preproc_last_error": (C.c_char_p, [_P]),

@@ -790,6 +790,10 @@ cudaError_t gemv_ring_init() {   // set the shared-memory opt-in outside of any 
 
 bool gemv_ring_supported(int K, bool has_ln) { (void)has_ln; return K >= 32 && K % 32 == 0; }
 
+// The register-resident LayerNorm prologue holds two slabs of x; with more (K > 2048, but also K = 96, 640 or 1280, whose
+// slabs are narrower) the statistics are streamed by the LN_BIGK instantiations.
+bool gemv_ring_ln_streamed(int K) { return K / mega::slab_width(K) > 2; }
+
 // The 16-row kernels' epilogue gives one (weight row, image row) pair of a 16 x 16 tile to each consumer thread.
 int gemv_ring_max_rows() { return mega::NCT >= 256 ? 16 : 8; }
 
@@ -823,15 +827,13 @@ void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st) {
     static int cap = 0;
     if (cap == 0) { const char* c = getenv("SV_RING_SLOTS"); cap = c ? atoi(c) : mega::STAGES; if (cap < 1 || cap > 6) cap = mega::STAGES; }
     const int rows_per_cta = (g.N + nsm - 1) / nsm, tpc = (rows_per_cta + 15) / 16;
-    int ks = 32;
-    for (int c : {1024, 768, 512, 256, 128, 64}) if (c <= g.K && g.K % c == 0) { ks = c; break; }
-    const int need = tpc * (g.K / ks);
+    const int need = tpc * (g.K / mega::slab_width(g.K));
     ra.nslots = need < cap ? need : cap;
     if (ring_row_groups(g.B) == 2 && ra.nslots > mega::STAGES) ra.nslots = mega::STAGES;   // + 32 KB of fragments must fit
     if (ra.nslots < 1) ra.nslots = 1;
   }
   const bool ln = g.ln_w != nullptr;
-  if (ln && g.K > 2 * mega::KS_MAX) {       // LayerNorm over K > 2048 (v2): separate instantiations, 8 rows only
+  if (ln && gemv_ring_ln_streamed(g.K)) {   // streamed LayerNorm (v2's K = 4608): separate instantiations, 8 rows only
     if (ring_row_groups(g.B) != 1) {          // sv_engine_create keeps such engines off this path above 8 rows
       fprintf(stderr, "starvector_b200: LayerNorm GEMV with K = %d over %d rows has no ring kernel\n", g.K, g.B);
       abort();

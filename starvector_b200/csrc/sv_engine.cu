@@ -749,12 +749,14 @@ int sv_engine_create(const sv_model_desc* desc, int device, sv_engine** out) {
     const char* la = getenv("SV_FLOW_L2AHEAD");
     if (la) e->flow_l2_ahead = std::max(0, std::min(64, atoi(la))); }
   if (!gemv_ring_supported(d.hidden, true) || !gemv_ring_supported(d.n_inner, false)) e->fused_decode = false;
+  // v1 appends K/V in the c_attn GEMV's epilogue, which the streamed-LayerNorm kernels do not have
+  if (!e->v2 && gemv_ring_ln_streamed(d.hidden)) e->fused_decode = false;
   // v2 at full size: the per-op kernels measure faster (4.4 vs 5.8 ms/token at 8B; 768-wide slabs + per-slab LayerNorm
   // on the consumer path), so the fused ring step is opt-in for v2 (SV_DECODE=fused) until that is fixed.
   if (e->v2 && !(dec && !strcmp(dec, "fused"))) e->fused_decode = false;
-  // above 8 rows the fused step needs the 16-row ring kernels: v1 with hidden <= 2048 (they have no K > 2048 LayerNorm
-  // path) and 8 consumer warps
-  if (d.max_batch > 8 && (e->v2 || d.hidden > 2048 || d.max_batch > gemv_ring_max_rows())) e->fused_decode = false;
+  // above 8 rows the fused step needs the 16-row ring kernels: v1 without a streamed LayerNorm (they have none) and
+  // 8 consumer warps
+  if (d.max_batch > 8 && (e->v2 || gemv_ring_ln_streamed(d.hidden) || d.max_batch > gemv_ring_max_rows())) e->fused_decode = false;
   if (!build_weights(e) || !build_buffers(e)) {
     std::string msg = std::string("device allocation failed: ") + cudaGetErrorString(cudaGetLastError());
     sv_engine_destroy(e);
@@ -1804,6 +1806,180 @@ int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets, float
   }
   cudaFree(buf);
   return r == cudaSuccess ? SV_OK : op_fail("lm_logprob", r);
+}
+
+// ---- the decode-step kernels one at a time, over caches the caller owns -------------------------------------------
+// Every argument is checked on the host before anything is allocated or launched: a shape the kernels were not built
+// for returns SV_ERR_INVALID instead of reaching a device trap (the ring's bounded waits) or an abort.
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+constexpr size_t kOpState = 512;     // scratch header holding the GenState / RowState the kernels read
+static_assert(sizeof(GenState) <= kOpState && sizeof(RowState) <= kOpState, "the state structs fit the scratch header");
+
+int sv_op_attention_decode(int32_t impl, int32_t per_row, const void* qkv, const void* kcache, const void* vtcache, void* out,
+                           const int32_t* lens_host, int32_t batch, int32_t n_head, int32_t n_kv, int32_t tcap,
+                           int32_t nsplit, int32_t window, void* stream) {
+  const char* bad = nullptr;
+  if (!qkv || !kcache || !vtcache || !out || !lens_host) bad = "null pointer";
+  else if (impl != SV_ATTN_DECODE_SPLIT && impl != SV_ATTN_DECODE_CLUSTER) bad = "unknown impl";
+  else if (per_row != 0 && per_row != 1) bad = "per_row is 0 or 1";
+  else if (batch < 1 || batch > kSessionRows) bad = "batch not in [1, 16]";
+  else if (n_head < 1 || n_kv < 1 || n_head % n_kv || n_head / n_kv > 16) bad = "n_head % n_kv != 0 or group > 16";
+  else if (tcap < 32 || tcap % 32) bad = "tcap % 32 != 0";
+  else if (nsplit < 1 || nsplit > (impl == SV_ATTN_DECODE_CLUSTER ? 8 : kMaxSplit)) bad = "nsplit not in [1, 128] (split) / [1, 8] (cluster)";
+  else if (window < 0) bad = "window < 0";
+  else if (!aligned16(qkv) || !aligned16(kcache) || !aligned16(vtcache)) bad = "qkv and the caches must be 16-byte aligned";
+  for (int b = 0; !bad && b < batch; ++b) {
+    if (lens_host[b] < 1 || lens_host[b] > tcap) bad = "a length is not in [1, tcap]";
+    else if (!per_row && lens_host[b] != lens_host[0]) bad = "per_row = 0 needs equal lengths";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad attention_decode arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = 128, cols = (n_head + 2 * n_kv) * D;
+  const size_t part_floats = impl == SV_ATTN_DECODE_SPLIT ? (size_t)batch * n_kv * nsplit * (32 + 16 * D) : 0;
+  GenState gs{};
+  RowState rs{};
+  gs.cur_len = lens_host[0] - 1;
+  for (int b = 0; b < batch; ++b) rs.row_len[b] = lens_host[b] - 1;    // the new token's key sits at lens - 1
+  void* buf = nullptr;
+  cudaError_t r = cudaMalloc(&buf, kOpState + part_floats * sizeof(float));
+  if (r != cudaSuccess) return op_fail("attention_decode alloc", r);
+  GenState* d_gs = reinterpret_cast<GenState*>(buf);
+  RowState* d_rs = reinterpret_cast<RowState*>(buf);
+  float* partial = reinterpret_cast<float*>(static_cast<char*>(buf) + kOpState);
+  if (per_row) r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
+  else r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) {
+    if (impl == SV_ATTN_DECODE_SPLIT) {
+      launch_attention_decode((const bf16*)qkv, cols, (const bf16*)kcache, (const bf16*)vtcache, (bf16*)out, partial, d_gs,
+                              batch, n_head, n_kv, D, tcap, nsplit, window, st, per_row ? d_rs : nullptr);
+      r = cudaGetLastError();
+    } else {
+      r = attention_decode_cluster_init();
+      if (r == cudaSuccess)
+        r = launch_attention_decode_cluster((const bf16*)qkv, cols, (const bf16*)kcache, (const bf16*)vtcache, (bf16*)out, d_gs,
+                                            batch, n_head, n_kv, D, tcap, nsplit, window, false, st, per_row ? d_rs : nullptr);
+    }
+  }
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  return r == cudaSuccess ? SV_OK : op_fail("attention_decode", r);
+}
+
+int32_t sv_op_ring_ntiles(int32_t N) { return N < 1 ? 0 : gemv_ring_ntiles(N); }
+int32_t sv_op_ring_row_stride(int32_t B) { return 8 * ring_row_groups(B); }
+
+int sv_op_gemv_ring(const sv_op_ring* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad gemv_ring arguments: null descriptor");
+  const sv_op_ring& o = *args;
+  const bool ln = o.ln_w != nullptr;
+  const char* bad = nullptr;
+  if (!o.x || !o.w || !o.y) bad = "x, w and y are required";
+  else if (o.B < 1 || o.B > gemv_ring_max_rows()) bad = "B not in [1, gemv_ring_max_rows()]";
+  else if (o.N < 1 || !gemv_ring_supported(o.K, ln)) bad = "N < 1 or K % 32 != 0";
+  else if (ln != (o.ln_b != nullptr)) bad = "ln_w and ln_b go together";
+  else if (!aligned16(o.x) || !aligned16(o.w) || (ln && (!aligned16(o.ln_w) || !aligned16(o.ln_b))))
+    bad = "x, w, ln_w and ln_b must be 16-byte aligned";
+  else if (o.act < SV_ACT_NONE || o.act > SV_ACT_SILU) bad = "unknown act";
+  else if (o.tiled != 0 && o.tiled != 1) bad = "tiled is 0 or 1";
+  else if (o.epi < 0 || o.epi > 2 || (o.epi != 0 && !ln)) bad = "epi is 0 (plain), 1 (QKV) or 2 (lm_head); 1 and 2 need the LayerNorm";
+  else if (ln && gemv_ring_ln_streamed(o.K) && (o.B > 8 || o.epi == 1))
+    bad = "a LayerNorm over more than two slabs of K has ring kernels for <= 8 rows and no QKV epilogue";
+  else if (o.epi == 2 && (!o.amax_val || !o.amax_idx)) bad = "lm_head needs amax_val and amax_idx";
+  else if (o.epi == 1) {
+    if (!o.kcache || !o.vtcache || !o.pos_host) bad = "QKV needs kcache, vtcache and pos_host";
+    else if (o.n_head < 1 || o.n_kv < 1 || o.n_head % o.n_kv || o.N != (o.n_head + 2 * o.n_kv) * 128) bad = "N != (n_head + 2 n_kv) * 128";
+    else if (o.tcap < 32 || o.tcap % 32) bad = "tcap % 32 != 0";
+    else if (o.per_row != 0 && o.per_row != 1) bad = "per_row is 0 or 1";
+    for (int b = 0; !bad && b < (o.per_row ? o.B : 1); ++b)
+      if (o.pos_host[b] < 0 || o.pos_host[b] > o.tcap) bad = "a position is not in [0, tcap]";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad gemv_ring arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ncta = gemv_ring_ncta();
+  const size_t tiled_bytes = o.tiled ? flow_tiled_bytes(o.N, o.K, ncta) : 0;
+  void* buf = nullptr;
+  cudaError_t r = cudaMalloc(&buf, kOpState + tiled_bytes);
+  if (r != cudaSuccess) return op_fail("gemv_ring alloc", r);
+  GenState gs{};
+  RowState rs{};
+  if (o.epi == 1) {
+    gs.cur_len = o.pos_host[0];
+    for (int b = 0; o.per_row && b < o.B; ++b) rs.row_len[b] = o.pos_host[b];
+  }
+  GenState* d_gs = reinterpret_cast<GenState*>(buf);
+  RowState* d_rs = reinterpret_cast<RowState*>(buf);
+  uint8_t* wt = static_cast<uint8_t*>(buf) + kOpState;
+  if (o.per_row) r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
+  else r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = gemv_ring_init();
+  if (r == cudaSuccess) {
+    if (o.tiled) launch_flow_repack((const bf16*)o.w, (const bf16*)o.bias, wt, o.N, o.K, ncta, st);
+    RingGemvLaunch g{};
+    g.X = (const bf16*)o.x; g.W = (const bf16*)o.w; g.Wt = o.tiled ? wt : nullptr; g.bias = (const bf16*)o.bias;
+    g.res = (const bf16*)o.residual; g.ln_w = (const bf16*)o.ln_w; g.ln_b = (const bf16*)o.ln_b; g.Y = (bf16*)o.y;
+    g.B = o.B; g.N = o.N; g.K = o.K; g.act = o.act; g.epi = o.epi; g.ln_eps = o.ln_eps;
+    g.n_head = o.n_head; g.n_kv = o.n_kv; g.tcap = o.tcap; g.state = d_gs;
+    g.kcache = (bf16*)o.kcache; g.vtcache = (bf16*)o.vtcache; g.amax_val = o.amax_val; g.amax_idx = o.amax_idx;
+    g.pdl = false; g.rows = (o.epi == 1 && o.per_row) ? d_rs : nullptr;
+    launch_gemv_ring(g, st);
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  return r == cudaSuccess ? SV_OK : op_fail("gemv_ring", r);
+}
+
+int sv_op_rope_table(void* cos_t, void* sin_t, int32_t max_pos, int32_t d, float theta, void* stream) {
+  if (!cos_t || !sin_t || max_pos < 1 || d < 2 || d % 2 || d / 2 > kRopeMaxHalf || !(theta > 0.f))
+    return fail(nullptr, SV_ERR_INVALID, "bad rope_table arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  launch_rope_table((bf16*)cos_t, (bf16*)sin_t, max_pos, d, theta, st);
+  cudaError_t r = cudaGetLastError();
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  return r == cudaSuccess ? SV_OK : op_fail("rope_table", r);
+}
+
+int sv_op_rope(void* qkv, const void* cos_t, const void* sin_t, int32_t rows, int32_t seq, int32_t n_head, int32_t n_kv,
+               int32_t max_pos, int32_t pos0, const int32_t* pos_host, int32_t per_row, void* kcache, void* vtcache,
+               int32_t tcap, void* stream) {
+  const char* bad = nullptr;
+  if (!qkv || !cos_t || !sin_t) bad = "null pointer";
+  else if (rows < 1 || seq < 1 || n_head < 1 || n_kv < 1 || max_pos < 1 || pos0 < 0) bad = "rows, seq, n_head, n_kv, max_pos >= 1, pos0 >= 0";
+  else if (kcache && (!vtcache || !pos_host || tcap < 32 || tcap % 32)) bad = "the KV append needs vtcache, pos_host and tcap % 32 == 0";
+  else if (pos_host && (rows > kSessionRows || (per_row != 0 && per_row != 1))) bad = "one token per row: rows <= 16, per_row is 0 or 1";
+  for (int b = 0; !bad && pos_host && b < rows; ++b) {
+    if (pos_host[b] < 0) bad = "a position is < 0";
+    else if (!per_row && pos_host[b] != pos_host[0]) bad = "per_row = 0 needs equal positions";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad rope arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = 128, cols = (n_head + 2 * n_kv) * D;
+  void* buf = nullptr;
+  cudaError_t r = cudaSuccess;
+  GenState* d_gs = nullptr;
+  RowState* d_rs = nullptr;
+  if (pos_host) {
+    r = cudaMalloc(&buf, kOpState);
+    if (r != cudaSuccess) return op_fail("rope alloc", r);
+    GenState gs{};
+    RowState rs{};
+    gs.cur_len = pos_host[0];
+    for (int b = 0; b < rows; ++b) rs.row_len[b] = pos_host[b];
+    if (per_row) { d_rs = reinterpret_cast<RowState*>(buf); r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st); }
+    else { d_gs = reinterpret_cast<GenState*>(buf); r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st); }
+  }
+  if (r == cudaSuccess) {
+    if (kcache)
+      launch_rope_append((bf16*)qkv, rows, cols, n_head, n_kv, D, (const bf16*)cos_t, (const bf16*)sin_t, (bf16*)kcache,
+                         (bf16*)vtcache, d_gs, tcap, max_pos, false, st, d_rs);
+    else
+      launch_rope((bf16*)qkv, rows, pos_host ? 1 : seq, cols, n_head + n_kv, D, (const bf16*)cos_t, (const bf16*)sin_t, d_gs,
+                  max_pos, pos0, st, d_rs);
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  if (buf) cudaFree(buf);
+  return r == cudaSuccess ? SV_OK : op_fail("rope", r);
 }
 
 }  // extern "C"

@@ -146,6 +146,7 @@ void launch_rope(bf16* qkv, int rows, int seq, int qkv_cols, int n_rot_heads, in
 void launch_rope_append(bf16* qkv, int batch, int qkv_cols, int n_head, int n_kv, int d, const bf16* cos_t,
                         const bf16* sin_t, bf16* kcache, bf16* vtcache, const GenState* state, int tcap, int max_pos,
                         bool pdl, cudaStream_t st, const RowState* rows = nullptr);
+constexpr int kRopeMaxHalf = 256;     // d / 2 of a RoPE table
 void launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int d, float theta, cudaStream_t st);
 
 // decode attention (PDL-ready): the ncta <= 8 CTAs of one image form a thread-block cluster
@@ -186,6 +187,8 @@ struct RingGemvLaunch {
 };
 cudaError_t gemv_ring_init();
 bool gemv_ring_supported(int K, bool has_ln);
+// LayerNorm GEMVs over such K stream their statistics: kernels for <= 8 rows and the plain / lm_head epilogues only
+bool gemv_ring_ln_streamed(int K);
 int gemv_ring_ntiles(int N);
 int gemv_ring_ncta();
 int gemv_ring_max_rows();

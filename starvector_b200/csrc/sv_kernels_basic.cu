@@ -669,18 +669,29 @@ void launch_advance_len(GenState* state, cudaStream_t st) {
 // ------------------------------------------------------------------------------------------
 // Rotary position embedding of StarCoder2 (transformers modeling_starcoder2.py:72-107,265-329): cos/sin are computed
 // in fp32, CAST TO bf16, and  q*cos + rotate_half(q)*sin  runs as three bf16 tensor ops (two products, one sum).
-__global__ void rope_table_kernel(bf16* __restrict__ cos_t, bf16* __restrict__ sin_t, int max_pos, int half, float theta) {
+// inv_freq comes from the host, computed as transformers does in fp32 (1.0 / theta ** (arange(0, d, 2) / d): the exponent,
+// the power and the reciprocal each rounded to fp32 once).  The device's powf may be an ulp or two off; at positions in the
+// thousands that moves the angle enough to change bf16 entries by up to hundreds of ulps where cos / sin cross zero.
+struct RopeInvFreq {
+  float v[kRopeMaxHalf];
+};
+__global__ void rope_table_kernel(bf16* __restrict__ cos_t, bf16* __restrict__ sin_t, int max_pos, int half,
+                                  const RopeInvFreq inv_freq) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= max_pos * half) return;
   const int pos = i / half, j = i % half;
-  const float inv_freq = 1.0f / powf(theta, (float)(2 * j) / (float)(2 * half));
-  const float ang = (float)pos * inv_freq;
+  const float ang = (float)pos * inv_freq.v[j];
   cos_t[i] = __float2bfloat16_rn(cosf(ang));
   sin_t[i] = __float2bfloat16_rn(sinf(ang));
 }
 void launch_rope_table(bf16* cos_t, bf16* sin_t, int max_pos, int d, float theta, cudaStream_t st) {
+  RopeInvFreq f{};
+  for (int j = 0; j < d / 2 && j < kRopeMaxHalf; ++j) {
+    const float e = (float)(2 * j) / (float)d;
+    f.v[j] = 1.0f / (float)std::pow((double)theta, (double)e);      // the fp32 power, correctly rounded
+  }
   const int n = max_pos * (d / 2);
-  rope_table_kernel<<<(n + 255) / 256, 256, 0, st>>>(cos_t, sin_t, max_pos, d / 2, theta);
+  rope_table_kernel<<<(n + 255) / 256, 256, 0, st>>>(cos_t, sin_t, max_pos, d / 2, f);
   count_launch();
 }
 template <bool ROWS>

@@ -113,6 +113,12 @@ SV_DEVINL Plan make_plan(int N, int K, int cta, int ncta) {
   return p;
 }
 
+// make_plan's slab width on the host
+inline int slab_width(int K) {
+  for (int ks : {1024, 768, 512, 256, 128, 64}) if (ks <= K && K % ks == 0) return ks;
+  return 32;
+}
+
 struct Ring {
   uint32_t base, full0, empty0;      // shared addresses
   uint32_t slot, phase, nslots;

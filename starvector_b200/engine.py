@@ -446,3 +446,75 @@ def op_lm_logprob(x: torch.Tensor, w: torch.Tensor, targets: torch.Tensor) -> to
     out = torch.empty(M, dtype=torch.float32, device=x.device)
     _lib.check(lib, lib.sv_op_lm_logprob(_p(x), _p(w), _p(tg), _p(out), M, w.shape[0], K, _stream_ptr(x.device)))
     return out
+
+
+def _i32s(v) -> C.Array:
+    v = [int(a) for a in v]
+    return (C.c_int32 * max(1, len(v)))(*v)
+
+
+def op_attention_decode(qkv: torch.Tensor, kcache: torch.Tensor, vtcache: torch.Tensor, lens, n_head: int, n_kv: int,
+                        nsplit: int, window: int = 0, impl: int = _lib.SV_ATTN_DECODE_SPLIT, per_row: bool = False) -> torch.Tensor:
+    """One decode-attention launch over caller-filled caches `kcache [B, n_kv, tcap, 128]`, `vtcache [B, n_kv, 128, tcap]`:
+    row b's query (qkv row b) attends to keys `[0, lens[b])` -> `[B, n_head * 128]`."""
+    lib = _lib.load()
+    B, tcap = kcache.shape[0], kcache.shape[2]
+    out = torch.empty(B, n_head * 128, dtype=torch.bfloat16, device=qkv.device)
+    _lib.check(lib, lib.sv_op_attention_decode(impl, int(per_row), _p(qkv), _p(kcache), _p(vtcache), _p(out), _i32s(lens), B,
+                                               n_head, n_kv, tcap, nsplit, window, _stream_ptr(qkv.device)))
+    return out
+
+
+def op_gemv_ring(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
+                 ln: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, act: int = 0, epi: int = 0, tiled: bool = False,
+                 ln_eps: float = 1e-5, y: Optional[torch.Tensor] = None, kcache: Optional[torch.Tensor] = None,
+                 vtcache: Optional[torch.Tensor] = None, n_head: int = 0, n_kv: int = 0, pos=None, per_row: bool = False):
+    """One weight-ring GEMV launch (the decode step's): `y [B, N]`; with `epi=2` also the argmax partials
+    `(amax_val, amax_idx)`, `[ntiles, row_stride]`.  `y` may be `residual` (in place)."""
+    lib = _lib.load()
+    B, K = x.shape
+    N = w.shape[0]
+    if y is None:
+        y = torch.empty(B, N, dtype=torch.bfloat16, device=x.device)
+    a = _lib.OpRing(x=x.data_ptr(), w=w.data_ptr(), y=y.data_ptr(), B=B, N=N, K=K, act=act, epi=epi, tiled=int(tiled),
+                    ln_eps=ln_eps, n_head=n_head, n_kv=n_kv, per_row=int(per_row))
+    if bias is not None:
+        a.bias = bias.data_ptr()
+    if residual is not None:
+        a.residual = residual.data_ptr()
+    if ln is not None:
+        a.ln_w, a.ln_b = ln[0].data_ptr(), ln[1].data_ptr()
+    if kcache is not None:
+        a.kcache, a.vtcache, a.tcap = kcache.data_ptr(), vtcache.data_ptr(), kcache.shape[2]
+    if pos is not None:
+        posv = _i32s(pos)
+        a.pos_host = C.cast(posv, C.POINTER(C.c_int32))
+    amax = None
+    if epi == 2:
+        nt, rs = lib.sv_op_ring_ntiles(N), lib.sv_op_ring_row_stride(B)
+        amax = (torch.full((nt, rs), float("nan"), dtype=torch.float32, device=x.device),
+                torch.full((nt, rs), -1, dtype=torch.int32, device=x.device))
+        a.amax_val, a.amax_idx = amax[0].data_ptr(), amax[1].data_ptr()
+    _lib.check(lib, lib.sv_op_gemv_ring(C.byref(a), _stream_ptr(x.device)))
+    return (y, amax) if epi == 2 else y
+
+
+def op_rope_table(max_pos: int, d: int, theta: float, device="cuda") -> Tuple[torch.Tensor, torch.Tensor]:
+    """The engine's bf16 RoPE tables `cos, sin [max_pos, d / 2]`."""
+    lib = _lib.load()
+    cos = torch.empty(max_pos, d // 2, dtype=torch.bfloat16, device=device)
+    sin = torch.empty_like(cos)
+    _lib.check(lib, lib.sv_op_rope_table(_p(cos), _p(sin), max_pos, d, theta, _stream_ptr(cos.device)))
+    return cos, sin
+
+
+def op_rope(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_head: int, n_kv: int, seq: int = 1, pos0: int = 0,
+            pos=None, per_row: bool = False, kcache: Optional[torch.Tensor] = None,
+            vtcache: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """RoPE in place on packed qkv rows `[rows, (n_head + 2 n_kv) * 128]` (see sv_op_rope); returns qkv."""
+    lib = _lib.load()
+    tcap = kcache.shape[2] if kcache is not None else 0
+    posv = _i32s(pos) if pos is not None else None
+    _lib.check(lib, lib.sv_op_rope(_p(qkv), _p(cos), _p(sin), qkv.shape[0], seq, n_head, n_kv, cos.shape[0], pos0, posv,
+                                   int(per_row), _p(kcache), _p(vtcache), tcap, _stream_ptr(qkv.device)))
+    return qkv

@@ -49,6 +49,79 @@ def test_create_rejects_bad_descriptors_without_touching_cuda():
     assert lib.sv_engine_create(C.byref(d), 0, C.byref(h)) == _lib.SV_ERR_INVALID
 
 
+DECODE_OPS = ("sv_op_attention_decode", "sv_op_gemv_ring", "sv_op_ring_ntiles", "sv_op_ring_row_stride",
+              "sv_op_rope_table", "sv_op_rope")
+
+
+def test_decode_op_symbols_and_descriptor_layout():
+    assert _lib.ABI_VERSION == 7                       # test hooks only: no existing entry point changed
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    for name in DECODE_OPS:
+        assert name in _header_symbols() and name in _lib.SIGNATURES and name in exported, name
+    # sv_op_ring: 7 pointers, 6 int32, float (+4 padding), 2 pointers, 4 int32, 3 pointers
+    assert C.sizeof(_lib.OpRing) == 144
+    assert (_lib.OpRing.ln_eps.offset, _lib.OpRing.kcache.offset, _lib.OpRing.n_head.offset,
+            _lib.OpRing.pos_host.offset, _lib.OpRing.amax_idx.offset) == (80, 88, 104, 120, 136)
+
+
+def _bad_decode_attention(**kw):
+    a = dict(impl=0, per_row=0, lens=[5], n_head=16, n_kv=1, tcap=64, nsplit=2, window=0, ptr=0x10000)
+    a.update(kw)
+    lens = a["lens"]
+    arr = (C.c_int32 * len(lens))(*lens)
+    p = C.c_void_p(a["ptr"])
+    lib = _lib.load()
+    return lib.sv_op_attention_decode(a["impl"], a["per_row"], p, p, p, p, arr, len(lens), a["n_head"], a["n_kv"], a["tcap"],
+                                      a["nsplit"], a["window"], None)
+
+
+@pytest.mark.parametrize("kw", [dict(n_head=6, n_kv=4), dict(n_head=17, n_kv=1), dict(tcap=48), dict(lens=[0]),
+                                dict(lens=[65]), dict(lens=[5, 6]), dict(lens=[1] * 17, per_row=1), dict(nsplit=0),
+                                dict(nsplit=129), dict(impl=1, nsplit=9), dict(impl=2), dict(window=-1), dict(ptr=0x10008),
+                                dict(ptr=0)], ids=str)
+def test_decode_attention_op_rejects_on_the_host(kw):
+    """Checked before any CUDA call: these return SV_ERR_INVALID on a machine without a GPU too."""
+    assert _bad_decode_attention(**kw) == _lib.SV_ERR_INVALID
+    assert b"attention_decode" in _lib.load().sv_last_error(None)
+
+
+@pytest.mark.parametrize("kw", [dict(K=48), dict(K=0), dict(B=0), dict(B=17), dict(N=0), dict(x=0x10008),
+                                dict(w=0x10004), dict(ln=True, ln_b=0x10008), dict(ln=False, epi=1), dict(ln=False, epi=2),
+                                dict(ln=True, K=4608, B=9), dict(ln=True, K=640, B=9), dict(ln=True, K=4608, epi=1),
+                                dict(ln=True, epi=2, amax=False), dict(ln=True, epi=1, N=2304, tcap=40),
+                                dict(ln=True, epi=1, N=2300), dict(ln=True, epi=1, N=2304, pos=[65]),
+                                dict(ln=True, epi=1, N=2304, pos=[3, -1], per_row=1, B=2), dict(act=4), dict(epi=3)], ids=str)
+def test_gemv_ring_op_rejects_on_the_host(kw):
+    """Among them the LayerNorm GEMV over K > 2048 with more than 8 rows, which has no ring kernel (the launcher would abort)."""
+    a = dict(B=1, N=2304, K=2048, ln=False, epi=0, act=0, tcap=64, pos=[3], per_row=0, amax=True)
+    a.update(kw)
+    pos = (C.c_int32 * len(a["pos"]))(*a["pos"])
+    o = _lib.OpRing(x=a.get("x", 0x10000), w=a.get("w", 0x20000), y=0x30000, B=a["B"], N=a["N"], K=a["K"], act=a["act"],
+                    epi=a["epi"], n_head=16, n_kv=1, tcap=a["tcap"], per_row=a["per_row"], kcache=0x40000, vtcache=0x50000,
+                    pos_host=C.cast(pos, C.POINTER(C.c_int32)))
+    if a["ln"]:
+        o.ln_w, o.ln_b = 0x60000, a.get("ln_b", 0x70000)
+    if a["amax"]:
+        o.amax_val, o.amax_idx = 0x80000, 0x90000
+    lib = _lib.load()
+    assert lib.sv_op_gemv_ring(C.byref(o), None) == _lib.SV_ERR_INVALID
+    assert b"gemv_ring" in lib.sv_last_error(None)
+
+
+def test_rope_ops_reject_on_the_host():
+    lib = _lib.load()
+    p = C.c_void_p(0x10000)
+    assert lib.sv_op_rope_table(p, p, 16, 127, 1e4, None) == _lib.SV_ERR_INVALID
+    assert lib.sv_op_rope_table(p, p, 0, 128, 1e4, None) == _lib.SV_ERR_INVALID
+    assert lib.sv_op_rope_table(p, p, 16, 128, 0.0, None) == _lib.SV_ERR_INVALID
+    two = (C.c_int32 * 2)(3, 4)
+    assert lib.sv_op_rope(p, p, p, 2, 1, 4, 2, 16, 0, two, 0, None, None, 0, None) == _lib.SV_ERR_INVALID   # unequal, per_row 0
+    assert lib.sv_op_rope(p, p, p, 2, 1, 4, 2, 16, 0, two, 1, p, p, 40, None) == _lib.SV_ERR_INVALID        # tcap % 32
+    assert lib.sv_op_rope(p, p, p, 2, 1, 4, 2, 16, 0, None, 0, p, p, 64, None) == _lib.SV_ERR_INVALID      # append without pos
+    assert lib.sv_op_rope(p, p, p, 2, 1, 4, 2, 16, -1, None, 0, None, None, 0, None) == _lib.SV_ERR_INVALID
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
 def test_engine_fails_loudly_without_gpu():
     from starvector_b200.engine import Engine

@@ -88,24 +88,61 @@ def test_linear_tcgen05_agrees_with_rowgroup():
     assert (a == c).float().mean() > 0.98
 
 
-@pytest.mark.parametrize("B,L,H", [(1, 17, 2), (2, 257, 16), (3, 40, 4)])
-def test_attention_vit(B, L, H):
+def _close_attn(got, ref, dim, ulps=1.0, c=0.02):
+    """Scale-aware attention tolerance: 1 bf16 ulp + 2 % of the rms of that (row, head) output.  Attention outputs shrink
+    as the context grows, so a fixed atol would end up larger than the output itself and pass a key range off by one."""
+    got, ref = got.double().reshape(-1, dim), ref.double().reshape(-1, dim)
+    rms = ref.pow(2).mean(-1, keepdim=True).sqrt()
+    ulp = torch.exp2(torch.floor(torch.log2(ref.abs().clamp(min=2.0 ** -126))) - 7)
+    err = (got - ref).abs()
+    bad = err > ulps * ulp + c * rms
+    assert not bool(bad.any()), f"{int(bad.sum())} / {bad.numel()} mismatches, worst err/rms {(err / rms).max().item():.4f}"
+
+
+def plant_strong_keys(x, B, L, groups, dim, positions, seed):
+    """In packed rows x [B*L, cols] (CPU): aim every query of each group's heads along its own direction u_h (orthonormal in
+    the group) and make the keys at `positions` score 20 for all of them, with V = 4 N(0,1).  Where such a key is visible it
+    dominates the output; where it is masked, reading it would.  groups: [(q column offsets, k offset, v offset)]."""
+    g = torch.Generator().manual_seed(seed)
+    x = x.view(B, L, -1)
+    for qo, ko, vo in groups:
+        u = torch.linalg.qr(torch.randn(dim, len(qo), generator=g, dtype=torch.float64)).Q.T
+        for j, o in enumerate(qo):
+            x[:, :, o:o + dim] = (u[j] * math.sqrt(dim) + 0.3 * torch.randn(B, L, dim, generator=g, dtype=torch.float64)).to(x.dtype)
+        for p in positions:
+            x[:, p, ko:ko + dim] = (20.0 * u.sum(0)).to(x.dtype)
+            x[:, p, vo:vo + dim] = (4.0 * torch.randn(B, dim, generator=g)).to(x.dtype)
+
+
+@pytest.mark.parametrize("B,L,H,strong", [(1, 17, 2, False), (2, 257, 16, False), (3, 40, 4, False), (2, 257, 4, True)],
+                         ids=["1-17-2", "2-257-16", "3-40-4", "2-257-4-strong"])
+def test_attention_vit(B, L, H, strong):
     W = H * 64
     qkv = _bf(B * L, 3 * W, seed=14)
+    if strong:
+        x = qkv.cpu()
+        plant_strong_keys(x, B, L, [([h * 64], W + h * 64, 2 * W + h * 64) for h in range(H)], 64, [0, 31, 32, L - 1], seed=1)
+        qkv = x.to(DEV)
     out = E.op_attention_vit(qkv, B, L, H)
-    q, k, v = qkv.float().view(B, L, 3, H, 64).permute(2, 0, 3, 1, 4)
+    q, k, v = qkv.double().view(B, L, 3, H, 64).permute(2, 0, 3, 1, 4)
     ref = torch.nn.functional.scaled_dot_product_attention(q, k, v).permute(0, 2, 1, 3).reshape(B * L, W)
-    _close(out, ref, ulps=2, atol=1.5e-2)
+    _close_attn(out, ref, 64)
 
 
-@pytest.mark.parametrize("B,T,H", [(1, 19, 2), (2, 259, 16), (1, 70, 9)])
-def test_attention_mqa_causal(B, T, H):
+@pytest.mark.parametrize("B,T,H,strong", [(1, 19, 2, False), (2, 259, 16, False), (1, 70, 9, False), (2, 259, 16, True)],
+                         ids=["1-19-2", "2-259-16", "1-70-9", "2-259-16-strong"])
+def test_attention_mqa_causal(B, T, H, strong):
+    """strong: keys at 0, 31, 32, 33 and T - 1 that every head scores at 20; each query must see exactly the ones <= it."""
     D = 128
     qkv = _bf(B * T, H * D + 2 * D, seed=15)
+    if strong:
+        x = qkv.cpu()
+        plant_strong_keys(x, B, T, [([h * D for h in range(H)], H * D, H * D + D)], D, [0, 31, 32, 33, T - 1], seed=2)
+        qkv = x.to(DEV)
     out = E.op_attention_mqa(qkv, B, T, H)
-    x = qkv.float().view(B, T, H * D + 2 * D)
+    x = qkv.double().view(B, T, H * D + 2 * D)
     q = x[..., : H * D].view(B, T, H, D).transpose(1, 2)
     k = x[..., H * D: H * D + D].unsqueeze(1).expand(B, H, T, D)
     v = x[..., H * D + D:].unsqueeze(1).expand(B, H, T, D)
     ref = torch.nn.functional.scaled_dot_product_attention(q, k, v, is_causal=True).transpose(1, 2).reshape(B * T, H * D)
-    _close(out, ref, ulps=2, atol=1.5e-2)
+    _close_attn(out, ref, D)

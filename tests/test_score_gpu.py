@@ -12,6 +12,7 @@ from starvector_b200.config import dims_1b, dims_8b, dims_tiny, dims_tiny_v2
 from starvector_b200.engine import Engine, GenerationParams
 from starvector_b200.modeling import StarVectorForCausalLM
 from starvector_b200.weights import synthetic_images, synthetic_state_dict
+from test_ops_gpu import _close_attn, plant_strong_keys
 from test_score_logic import oracle_im2svg_loss
 
 pytestmark = pytest.mark.gpu
@@ -77,10 +78,10 @@ def test_lm_logprob_random_within_one_ulp():
 # ---- sv_op_attention_chunk ---------------------------------------------------------------------
 def _attention_ref(qkv, B, seq, q0, nh, nkv, window):
     D = 128
-    x = qkv.float().view(B, seq, (nh + 2 * nkv), D)
+    x = qkv.double().view(B, seq, (nh + 2 * nkv), D)
     q, k, v = x[:, :, :nh], x[:, :, nh:nh + nkv], x[:, :, nh + nkv:]
     grp = nh // nkv
-    out = torch.empty(B, seq - q0, nh, D)
+    out = torch.empty(B, seq - q0, nh, D, dtype=torch.float64)
     for p in range(q0, seq):
         lo = max(0, p + 1 - window) if window > 0 else 0
         for h in range(nh):
@@ -90,14 +91,22 @@ def _attention_ref(qkv, B, seq, q0, nh, nkv, window):
     return out.reshape(B * (seq - q0), nh * D)
 
 
-@pytest.mark.parametrize("q0,nh,nkv,window", [(0, 16, 1, 0), (17, 16, 1, 0), (300, 16, 1, 0), (17, 4, 2, 0),
-                                              (300, 4, 2, 24), (40, 18, 2, 24)])
-def test_attention_chunk(q0, nh, nkv, window):
+@pytest.mark.parametrize("q0,nh,nkv,window,strong", [(0, 16, 1, 0, False), (17, 16, 1, 0, False), (300, 16, 1, 0, False),
+                                                     (17, 4, 2, 0, False), (300, 4, 2, 24, False), (40, 18, 2, 24, False),
+                                                     (300, 4, 2, 24, True)],
+                         ids=["0-16-1-0", "17-16-1-0", "300-16-1-0", "17-4-2-0", "300-4-2-24", "40-18-2-24", "300-4-2-24-strong"])
+def test_attention_chunk(q0, nh, nkv, window, strong):
+    """strong: keys every head scores at 20 at the window edges of the chunk's queries (and 31/32/33, the last position):
+    each must count exactly for the queries whose window holds it."""
     B, seq = 2, q0 + 45
     g = torch.Generator().manual_seed(q0 * 7 + nh)
     qkv = torch.randn(B * seq, (nh + 2 * nkv) * 128, generator=g).to(torch.bfloat16)
+    if strong:
+        grp, D = nh // nkv, 128
+        groups = [([(k * grp + j) * D for j in range(grp)], (nh + k) * D, (nh + nkv + k) * D) for k in range(nkv)]
+        plant_strong_keys(qkv, B, seq, groups, D, [q0 - window, q0 - window + 1, q0 + 10 - window, 31, 32, 33, seq - 1], seed=3)
     got = E.op_attention_chunk(qkv.cuda(), B, seq, q0, nh, nkv, window).cpu()
-    _close(got, _attention_ref(qkv, B, seq, q0, nh, nkv, window), ulps=2, atol=1.5e-2)
+    _close_attn(got, _attention_ref(qkv, B, seq, q0, nh, nkv, window), 128)
 
 
 # ---- Engine.score against the oracle -----------------------------------------------------------
