@@ -330,6 +330,49 @@ SV_API int sv_op_rope(void* qkv, const void* cos_t, const void* sin_t, int32_t r
                       int32_t n_kv, int32_t max_pos, int32_t pos0, const int32_t* pos_host, int32_t per_row, void* kcache,
                       void* vtcache, int32_t tcap, void* stream);
 
+/* The token-selection kernels one launch at a time: what follows the logits of a decode step.  The caller owns the device
+ * tensors; the generation state travels as HOST arrays that are read on entry and written back on return.  The same
+ * logits are selected from `nsteps` times in one call, the bookkeeping advancing between the launches (B x nsteps draws
+ * of the sampler).  Every argument is checked on the host: SV_ERR_INVALID before any launch.  Synchronous on `stream`. */
+enum {
+  SV_SELECT_GREEDY = 0, /* select_greedy(_rows)_kernel; per_row = 0: followed by gen_finalize_kernel */
+  SV_SELECT_SAMPLE = 1, /* select_sample(_rows)_kernel; per_row = 0: followed by gen_finalize_kernel (fp32 scratch allocated here) */
+  SV_SELECT_FUSED = 2   /* select_fused(_rows)_kernel: greedy + bookkeeping + the next token's embedding in one launch */
+};
+typedef struct sv_op_select_args {
+  int32_t impl;                 /* SV_SELECT_* */
+  int32_t per_row;              /* 0: the rectangle-batch kernels; 1: the session kernels (every row has its own state) */
+  const void* logits;           /* bf16 [B][vocab] */
+  int32_t vocab, B;             /* vocab >= 1, B in [1, 16] */
+  sv_gen_params params;         /* max_new_tokens is the plain kernels' cap; poll_interval is ignored */
+  void* seen;                   /* uint8 [B][vocab]: ids generated so far (repetition penalty), updated */
+  int32_t* out_ids;             /* [B][out_stride] */
+  int32_t* next_ids;            /* [B] */
+  int32_t out_stride, advance_len, nsteps;
+  /* per_row = 0 (GenState) */
+  int32_t* counters_host;       /* [3]: step, cur_len, done */
+  int32_t* unfinished_host;     /* [B] */
+  /* per_row = 1 (RowState): rows b with bit b of row_mask set and row_active[b] != 0 select */
+  int32_t *row_len_host, *row_step_host, *row_active_host, *row_max_new_host;   /* [B] each */
+  uint64_t* row_seed_host;      /* [B] */
+  uint32_t row_mask;
+  int32_t* event_host;          /* [1] */
+  /* SV_SELECT_FUSED only */
+  const float* amax_val;        /* lm_head argmax partials [sv_op_ring_ntiles(vocab)][sv_op_ring_row_stride(B)], or NULL: */
+  const int32_t* amax_idx;      /*   the logits rows are scanned (always so when repetition_penalty != 1) */
+  const void *wte, *wpe;        /* bf16 [vocab][h], [n_positions][h]; wpe may be NULL (RoPE models) */
+  void* x;                      /* bf16 [B][h]: the selected tokens' embeddings at their post-advance positions */
+  int32_t h, n_positions;       /* h % 8 == 0 */
+} sv_op_select_args;
+SV_API int sv_op_select(const sv_op_select_args* args, void* stream);
+/* One beam_candidates_kernel launch over R = batch * num_beams rows: logits bf16 [R][vocab]; cur_len = tokens every
+ * running beam holds (0: no repetition penalty yet), running_scores_host float [R], run_seq int32 [R][seq_stride] (device,
+ * the beams' generated ids) -> cand_key / cand_val float and cand_tok int32 [R][2 * num_beams] (device).  p is checked as
+ * sv_beam_params_check_rows(p, batch, 16) does; a vocab whose row does not fit the SM's shared memory is SV_ERR_INVALID. */
+SV_API int sv_op_beam_candidates(const void* logits, int32_t vocab, const sv_beam_params* p, int32_t batch, int32_t cur_len,
+                                 const float* running_scores_host, const int32_t* run_seq, int32_t seq_stride,
+                                 float* cand_key, float* cand_val, int32_t* cand_tok, void* stream);
+
 /* ---- image preprocessing (SURVEY.md §8f-2) ------------------------------------------------ */
 /* Replaces `ImageTrainProcessor.__call__` (reference starvector/data/util.py:40-66: RGBA pasted on white, pad to
  * square with 255, `transforms.Resize(size, BICUBIC)` on the PIL image, ToTensor, Normalize) and

@@ -67,6 +67,21 @@ class OpRing(C.Structure):   # sv_op_ring
         ("pos_host", C.POINTER(C.c_int32)), ("amax_val", C.c_void_p), ("amax_idx", C.c_void_p)]
 
 
+SV_SELECT_GREEDY, SV_SELECT_SAMPLE, SV_SELECT_FUSED = 0, 1, 2
+
+
+class OpSelect(C.Structure):   # sv_op_select_args
+    _fields_ = [("impl", C.c_int32), ("per_row", C.c_int32), ("logits", C.c_void_p), ("vocab", C.c_int32), ("B", C.c_int32),
+                ("params", GenParams), ("seen", C.c_void_p), ("out_ids", C.c_void_p), ("next_ids", C.c_void_p),
+                ("out_stride", C.c_int32), ("advance_len", C.c_int32), ("nsteps", C.c_int32),
+                ("counters_host", C.POINTER(C.c_int32)), ("unfinished_host", C.POINTER(C.c_int32)),
+                ("row_len_host", C.POINTER(C.c_int32)), ("row_step_host", C.POINTER(C.c_int32)),
+                ("row_active_host", C.POINTER(C.c_int32)), ("row_max_new_host", C.POINTER(C.c_int32)),
+                ("row_seed_host", C.POINTER(C.c_uint64)), ("row_mask", C.c_uint32), ("event_host", C.POINTER(C.c_int32)),
+                ("amax_val", C.c_void_p), ("amax_idx", C.c_void_p), ("wte", C.c_void_p), ("wpe", C.c_void_p),
+                ("x", C.c_void_p), ("h", C.c_int32), ("n_positions", C.c_int32)]
+
+
 TOKEN_CALLBACK =C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32)   # sv_token_callback
 
 # name -> (restype, argtypes); must list every SV_API symbol of the header (tests check this)
@@ -121,6 +136,8 @@ SIGNATURES = {
     "sv_op_ring_row_stride": (C.c_int32, [_I]),
     "sv_op_rope_table": (C.c_int, [_P, _P, _I, _I, _F, _P]),
     "sv_op_rope": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, C.POINTER(_I), _I, _P, _P, _I, _P]),
+    "sv_op_select": (C.c_int, [C.POINTER(OpSelect), _P]),
+    "sv_op_beam_candidates": (C.c_int, [_P, _I, C.POINTER(BeamParams), _I, _I, C.POINTER(C.c_float), _P, _I, _P, _P, _P, _P]),
     "sv_preproc_create": (C.c_int, [C.POINTER(PreprocDesc), C.c_int, C.POINTER(_P)]),
     "sv_preproc_destroy": (None, [_P]),
     "sv_preproc_last_error": (C.c_char_p, [_P]),

@@ -373,9 +373,9 @@ int sv_beam_row_candidates_host(const sv_beam_params* bp, const float* logits, i
   for (int i = 0; i < seq_len; ++i) if (seq[i] >= 0 && seq[i] < vocab) seen[seq[i]] = 1;
   float mx = -INFINITY;
   for (int i = 0; i < vocab; ++i) mx = std::max(mx, logits[i]);
-  float z = 0.f;
+  double z = 0.0;                       // the device sums in a tree: a serial fp32 sum of 49k terms is off by ~1e-4
   for (int i = 0; i < vocab; ++i) z += expf(logits[i] - mx);
-  const float logz = logf(z);
+  const float logz = logf((float)z);
   std::vector<float> s(vocab);
   for (int i = 0; i < vocab; ++i)
     s[i] = svbeam::process_logprob((logits[i] - mx) - logz, seq_len > 0 && seen[i], bp->repetition_penalty, sample, bp->temperature);
@@ -384,8 +384,10 @@ int sv_beam_row_candidates_host(const sv_beam_params* bp, const float* logits, i
     std::vector<int> order(vocab);
     for (int i = 0; i < vocab; ++i) order[i] = i;
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return s[a] < s[b]; });    // ascending, as torch.sort
-    float m2 = s[order[vocab - 1]], z2 = 0.f;
-    for (int i = 0; i < vocab; ++i) z2 += expf(s[i] - m2);
+    const float m2 = s[order[vocab - 1]];
+    double zd = 0.0;
+    for (int i = 0; i < vocab; ++i) zd += expf(s[i] - m2);
+    const float z2 = (float)zd;
     float cum = 0.f;
     for (int j = 0; j < vocab; ++j) {
       cum += expf(s[order[j]] - m2) / z2;

@@ -1028,6 +1028,18 @@ int sv_score_tokens(sv_engine* e, const int32_t* ids, int32_t batch, int32_t n_t
   return finish_prefill_impl(e, B, pos0 + n, nullptr, st);
 }
 
+// The device-side generation parameters (n_stop_ids already checked to lie in [0, 8]).
+static GenParamsDev gen_params_dev(const sv_gen_params* p, int stop_row0_only, int out_stride) {
+  GenParamsDev hp;
+  memset(&hp, 0, sizeof(hp));
+  hp.max_new = p->max_new_tokens; hp.do_sample = p->do_sample; hp.eos_id = p->eos_token_id; hp.pad_id = p->pad_token_id;
+  hp.n_stop = p->n_stop_ids;
+  for (int i = 0; i < p->n_stop_ids; ++i) hp.stop_ids[i] = p->stop_ids[i];
+  hp.stop_row0_only = stop_row0_only; hp.out_stride = out_stride;
+  hp.temperature = p->temperature; hp.top_p = p->top_p; hp.rep_penalty = p->repetition_penalty; hp.seed = p->seed;
+  return hp;
+}
+
 // The generate loop.  `cb` (optional) receives the new tokens of every row each time the host polls the device
 // (sv_generate_stream); with cb == NULL the code path is exactly sv_generate's.
 static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids, int32_t* out_len, void* stream,
@@ -1050,13 +1062,7 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
   SV_CK(e, cudaEventRecord(e->ev_in, caller));
   SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
 
-  GenParamsDev hp;
-  memset(&hp, 0, sizeof(hp));
-  hp.max_new = max_new; hp.do_sample = p->do_sample; hp.eos_id = p->eos_token_id; hp.pad_id = p->pad_token_id;
-  hp.n_stop = p->n_stop_ids;
-  for (int i = 0; i < p->n_stop_ids; ++i) hp.stop_ids[i] = p->stop_ids[i];
-  hp.stop_row0_only = p->stop_row0_only; hp.out_stride = e->d.max_len;
-  hp.temperature = p->temperature; hp.top_p = p->top_p; hp.rep_penalty = p->repetition_penalty; hp.seed = p->seed;
+  const GenParamsDev hp = gen_params_dev(p, p->stop_row0_only, e->d.max_len);
   SV_CK(e, cudaMemcpyAsync(e->params, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
   SV_CK(e, cudaMemsetAsync(e->seen, 0, (size_t)B * e->d.vocab, st));
   launch_fill_i32(e->out_ids, p->pad_token_id, B * e->d.max_len, st);
@@ -1248,6 +1254,23 @@ int sv_generate_im2svg_host(sv_engine* e, const void* pixels_host, int32_t batch
   return r;
 }
 
+// The device-side beam parameters of a search over `batch` images (K = 2 * num_beams candidates per row).
+static svbeam::Params beam_params_dev(const sv_beam_params* bp, int batch, int vocab, int seq_stride) {
+  svbeam::Params hp;
+  memset(&hp, 0, sizeof(hp));
+  hp.B = batch; hp.nb = bp->num_beams; hp.K = 2 * bp->num_beams; hp.vocab = vocab; hp.max_length = bp->max_new_tokens;
+  hp.eos_id = bp->eos_token_id;
+  hp.pad_id = bp->pad_token_id;
+  hp.n_stop = bp->n_stop_ids;
+  for (int i = 0; i < bp->n_stop_ids; ++i) hp.stop_ids[i] = bp->stop_ids[i];
+  hp.do_sample = bp->do_sample; hp.early_stopping = bp->early_stopping;
+  hp.min_keep = std::max(2, 1 + (bp->eos_token_id >= 0 ? 1 : 0));
+  hp.seq_stride = seq_stride;
+  hp.temperature = bp->temperature; hp.top_p = bp->top_p; hp.rep_penalty = bp->repetition_penalty;
+  hp.length_penalty = bp->length_penalty; hp.seed = bp->seed;
+  return hp;
+}
+
 // Beam search with the whole loop on the device.  Graph body = one decode step over the batch * num_beams cache rows, then
 // candidates -> bookkeeping (+ next-token embeddings) -> KV suffix copies; the host replays it and polls `done`.
 int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_t* out_ids, int32_t* out_len, void* stream) {
@@ -1285,17 +1308,7 @@ int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_
   SV_CK(e, cudaEventRecord(e->ev_in, caller));
   SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
 
-  svbeam::Params hp;
-  memset(&hp, 0, sizeof(hp));
-  hp.B = batch; hp.nb = nb; hp.K = K; hp.vocab = d.vocab; hp.max_length = max_new; hp.eos_id = bp->eos_token_id;
-  hp.pad_id = bp->pad_token_id;
-  hp.n_stop = bp->n_stop_ids;
-  for (int i = 0; i < bp->n_stop_ids; ++i) hp.stop_ids[i] = bp->stop_ids[i];
-  hp.do_sample = bp->do_sample; hp.early_stopping = bp->early_stopping;
-  hp.min_keep = std::max(2, 1 + (bp->eos_token_id >= 0 ? 1 : 0));
-  hp.seq_stride = stride;
-  hp.temperature = bp->temperature; hp.top_p = bp->top_p; hp.rep_penalty = bp->repetition_penalty;
-  hp.length_penalty = bp->length_penalty; hp.seed = bp->seed;
+  const svbeam::Params hp = beam_params_dev(bp, batch, d.vocab, stride);
   svbeam::State hs;
   memset(&hs, 0, sizeof(hs));
   svbeam::init_state(hp, hs, e->prefix_len);
@@ -1450,13 +1463,7 @@ int sv_session_begin(sv_engine* e, const sv_gen_params* p, int32_t slots) {
     if (!ok) { e->rows = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the session state failed: %s", cudaGetErrorString(cudaGetLastError())); }
   }
   cudaStream_t st = e->gen_stream;
-  GenParamsDev hp;
-  memset(&hp, 0, sizeof(hp));
-  hp.max_new = p->max_new_tokens; hp.do_sample = p->do_sample; hp.eos_id = p->eos_token_id; hp.pad_id = p->pad_token_id;
-  hp.n_stop = p->n_stop_ids;
-  for (int i = 0; i < p->n_stop_ids; ++i) hp.stop_ids[i] = p->stop_ids[i];
-  hp.stop_row0_only = 0; hp.out_stride = d.max_len;
-  hp.temperature = p->temperature; hp.top_p = p->top_p; hp.rep_penalty = p->repetition_penalty; hp.seed = p->seed;
+  const GenParamsDev hp = gen_params_dev(p, /*stop_row0_only=*/0, d.max_len);
   SV_CK(e, cudaMemcpyAsync(e->params, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));   // pageable: staged synchronously
   SV_CK(e, cudaMemsetAsync(e->rows, 0, sizeof(RowState), st));
   ensure_flow_tiles(e, st);      // SV_TILED=1: the ring GEMVs stream the slab-tiled weights, rebuilt after a weight load
@@ -1980,6 +1987,146 @@ int sv_op_rope(void* qkv, const void* cos_t, const void* sin_t, int32_t rows, in
   if (r == cudaSuccess) r = cudaStreamSynchronize(st);
   if (buf) cudaFree(buf);
   return r == cudaSuccess ? SV_OK : op_fail("rope", r);
+}
+
+// ---- the token-selection kernels one at a time ---------------------------------------------------------------------
+int sv_op_select(const sv_op_select_args* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad select arguments: null descriptor");
+  const sv_op_select_args& o = *args;
+  const sv_gen_params& p = o.params;
+  const bool sampling = o.impl == SV_SELECT_SAMPLE || p.do_sample != 0, fused = o.impl == SV_SELECT_FUSED;
+  const char* bad = nullptr;
+  if (o.impl != SV_SELECT_GREEDY && o.impl != SV_SELECT_SAMPLE && o.impl != SV_SELECT_FUSED) bad = "unknown impl";
+  else if (o.per_row != 0 && o.per_row != 1) bad = "per_row is 0 or 1";
+  else if (!o.logits || !o.seen || !o.out_ids || !o.next_ids) bad = "logits, seen, out_ids and next_ids are required";
+  else if (o.B < 1 || o.B > kSessionRows) bad = "B not in [1, 16]";
+  else if (o.vocab < 1) bad = "vocab < 1";
+  else if (o.nsteps < 1 || o.out_stride < 1) bad = "nsteps and out_stride must be >= 1";
+  else if (o.advance_len != 0 && o.advance_len != 1) bad = "advance_len is 0 or 1";
+  else if (sampling && !(p.temperature > 0.f)) bad = "temperature must be > 0";
+  else if (sampling && !(p.top_p > 0.f && p.top_p <= 1.f)) bad = "top_p not in (0, 1]";
+  else if (!(p.repetition_penalty > 0.f)) bad = "repetition_penalty must be > 0";
+  else if (p.n_stop_ids < 0 || p.n_stop_ids > 8) bad = "n_stop_ids outside [0, 8]";
+  else if (!o.per_row) {
+    if (!o.counters_host || !o.unfinished_host) bad = "per_row = 0 needs counters_host and unfinished_host";
+    else if (o.counters_host[0] < 0 || o.counters_host[1] < 0) bad = "step and cur_len must be >= 0";
+    else if (o.counters_host[0] + o.nsteps > o.out_stride) bad = "step + nsteps > out_stride";
+  } else {
+    if (!o.row_len_host || !o.row_step_host || !o.row_active_host || !o.row_max_new_host || !o.row_seed_host || !o.event_host)
+      bad = "per_row = 1 needs the row_*_host arrays and event_host";
+    for (int b = 0; !bad && b < o.B; ++b) {
+      if (o.row_len_host[b] < 0 || o.row_step_host[b] < 0) bad = "row_len and row_step must be >= 0";
+      else if (o.row_step_host[b] + o.nsteps > o.out_stride) bad = "row_step + nsteps > out_stride";
+    }
+  }
+  if (!bad && fused) {
+    if (!o.wte || !o.x) bad = "fused needs wte and x";
+    else if (o.h < 8 || o.h % 8) bad = "h % 8 != 0";
+    else if (o.n_positions < 1) bad = "n_positions < 1";
+    else if (!aligned16(o.wte) || !aligned16(o.wpe) || !aligned16(o.x)) bad = "wte, wpe and x must be 16-byte aligned";
+    else if ((o.amax_val != nullptr) != (o.amax_idx != nullptr)) bad = "amax_val and amax_idx go together";
+    else if (o.amax_val && o.nsteps > 1) bad = "the argmax partials describe one step: nsteps > 1 needs amax_val = NULL";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad select arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const GenParamsDev hp = gen_params_dev(&p, p.stop_row0_only, o.out_stride);
+  GenState gs{};
+  RowState rs{};
+  if (o.per_row) {
+    for (int b = 0; b < o.B; ++b) {
+      rs.row_len[b] = o.row_len_host[b]; rs.row_step[b] = o.row_step_host[b]; rs.row_active[b] = o.row_active_host[b];
+      rs.row_max_new[b] = o.row_max_new_host[b]; rs.row_seed[b] = o.row_seed_host[b];
+    }
+    rs.event = o.event_host[0];
+  } else {
+    gs.step = o.counters_host[0]; gs.cur_len = o.counters_host[1]; gs.done = o.counters_host[2];
+    for (int b = 0; b < o.B; ++b) gs.unfinished[b] = o.unfinished_host[b];
+  }
+  const size_t probs_bytes = o.impl == SV_SELECT_SAMPLE ? (size_t)o.B * o.vocab * sizeof(float) : 0;
+  char* buf = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&buf), 3 * kOpState + probs_bytes);
+  if (r != cudaSuccess) return op_fail("select alloc", r);
+  GenState* d_gs = reinterpret_cast<GenState*>(buf);
+  RowState* d_rs = reinterpret_cast<RowState*>(buf + kOpState);
+  GenParamsDev* d_p = reinterpret_cast<GenParamsDev*>(buf + 2 * kOpState);
+  float* probs = reinterpret_cast<float*>(buf + 3 * kOpState);
+  static_assert(sizeof(GenParamsDev) <= kOpState, "the parameters fit a scratch slot");
+  r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_p, &hp, sizeof(hp), cudaMemcpyHostToDevice, st);
+  RowState* rows = o.per_row ? d_rs : nullptr;
+  const bf16* lg = (const bf16*)o.logits;
+  uint8_t* seen = (uint8_t*)o.seen;
+  for (int s = 0; r == cudaSuccess && s < o.nsteps; ++s) {
+    if (fused) {
+      launch_select_fused(lg, o.vocab, o.B, o.amax_val, o.amax_idx, gemv_ring_ntiles(o.vocab), 8 * ring_row_groups(o.B), d_gs,
+                          d_p, seen, o.next_ids, o.out_ids, o.advance_len, (const bf16*)o.wte, (const bf16*)o.wpe, (bf16*)o.x,
+                          o.h, o.n_positions, false, st, rows, o.row_mask);
+    } else {
+      if (o.impl == SV_SELECT_SAMPLE)
+        launch_select_sample(lg, o.vocab, o.B, d_gs, d_p, seen, o.next_ids, o.out_ids, probs, st, rows, o.row_mask, o.advance_len);
+      else
+        launch_select_greedy(lg, o.vocab, o.B, d_gs, d_p, seen, o.next_ids, o.out_ids, st, rows, o.row_mask, o.advance_len);
+      if (!o.per_row) launch_gen_finalize(d_gs, d_p, o.B, o.advance_len, st);
+    }
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&gs, d_gs, sizeof(gs), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&rs, d_rs, sizeof(rs), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  if (r != cudaSuccess) return op_fail("select", r);
+  if (o.per_row) {
+    for (int b = 0; b < o.B; ++b) {
+      o.row_len_host[b] = rs.row_len[b]; o.row_step_host[b] = rs.row_step[b]; o.row_active_host[b] = rs.row_active[b];
+      o.row_max_new_host[b] = rs.row_max_new[b]; o.row_seed_host[b] = rs.row_seed[b];
+    }
+    o.event_host[0] = rs.event;
+  } else {
+    o.counters_host[0] = gs.step; o.counters_host[1] = gs.cur_len; o.counters_host[2] = gs.done;
+    for (int b = 0; b < o.B; ++b) o.unfinished_host[b] = gs.unfinished[b];
+  }
+  return SV_OK;
+}
+
+int sv_op_beam_candidates(const void* logits, int32_t vocab, const sv_beam_params* p, int32_t batch, int32_t cur_len,
+                          const float* running_scores_host, const int32_t* run_seq, int32_t seq_stride, float* cand_key,
+                          float* cand_val, int32_t* cand_tok, void* stream) {
+  const char* bad = nullptr;
+  if (!logits || !p || !running_scores_host || !run_seq || !cand_key || !cand_val || !cand_tok) bad = "null pointer";
+  else if (sv_beam_params_check_rows(p, batch, svbeam::kMaxRows) != SV_OK)
+    bad = "beam parameters (num_beams in [2, 8], batch * num_beams <= 16, max_new_tokens >= 1, n_stop_ids in [0, 8], "
+          "early_stopping in {0, 1, 2}, temperature > 0, repetition_penalty > 0)";
+  else if (p->do_sample && !(p->top_p > 0.f && p->top_p <= 1.f)) bad = "top_p not in (0, 1]";
+  else if (vocab < 1) bad = "vocab < 1";
+  else if (seq_stride < 1 || cur_len < 0 || cur_len > seq_stride) bad = "cur_len not in [0, seq_stride]";
+  cudaError_t r = bad ? cudaSuccess : beam_init(vocab);      // the last check: it sizes the kernel's shared memory
+  if (r == cudaErrorInvalidValue) bad = "a logits row of this vocab does not fit the SM's shared memory";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad beam_candidates arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int R = batch * p->num_beams;
+  const svbeam::Params hp = beam_params_dev(p, batch, vocab, seq_stride);
+  svbeam::State hs;
+  memset(&hs, 0, sizeof(hs));
+  svbeam::init_state(hp, hs, 0);
+  hs.cur_len = cur_len;
+  for (int r = 0; r < R; ++r) hs.running_scores[r] = running_scores_host[r];
+  if (r != cudaSuccess) { cudaGetLastError(); return op_fail("beam_candidates setup", r); }
+  char* buf = nullptr;
+  r = cudaMalloc(reinterpret_cast<void**>(&buf), sizeof(svbeam::Params) + sizeof(svbeam::State));
+  if (r != cudaSuccess) return op_fail("beam_candidates alloc", r);
+  svbeam::Params* d_p = reinterpret_cast<svbeam::Params*>(buf);
+  svbeam::State* d_s = reinterpret_cast<svbeam::State*>(buf + sizeof(svbeam::Params));
+  static_assert(sizeof(svbeam::Params) % 8 == 0, "State follows Params at its alignment");
+  r = cudaMemcpyAsync(d_p, &hp, sizeof(hp), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_s, &hs, sizeof(hs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) {
+    launch_beam_candidates((const bf16*)logits, vocab, R, d_p, d_s, run_seq, cand_key, cand_val, cand_tok, st);
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  return r == cudaSuccess ? SV_OK : op_fail("beam_candidates", r);
 }
 
 }  // extern "C"

@@ -552,9 +552,7 @@ SV_DEVINL void select_sample_body(const bf16* __restrict__ logits, int vocab, Ge
       m = block_sum<kSampleThreads>(m, smf);
       if (m < top_p) hi = mid; else lo = mid;
     }
-  } else {
-    lo = -1.f;
-  }
+  }                                                                   // top_p == 1: lo stays 0, every id with p > 0 is kept
   // kept set = { p > lo }.  Thread `tid` owns ids [tid*per, tid*per+per) so the scan runs in id order.
   const int per = (vocab + kSampleThreads - 1) / kSampleThreads;
   const int i0 = tid * per, i1 = min(i0 + per, vocab);
@@ -576,8 +574,12 @@ SV_DEVINL void select_sample_body(const bf16* __restrict__ logits, int vocab, Ge
   }
   __syncthreads();
   const float target = s_bcast;
+  // torch.multinomial(probs, 1): every thread whose interval starts at or below the target proposes the id its scan stops
+  // at, or its last kept id when the scan runs off its end; ids rise with the thread index, so the maximum is the proposal
+  // of the last such thread.  (Also requiring `target < excl + own` leaves gaps: a thread's upper end and its neighbour's
+  // lower end are different fp32 expressions, and a target between them was claimed by nobody.)
   const float excl = base + incl - own;
-  if (own > 0.f && target >= excl && target < excl + own) {            // torch.multinomial(probs, 1)
+  if (own > 0.f && target >= excl) {
     float acc = excl; int tok = -1;
     for (int i = i0; i < i1; ++i) {
       float q = pr[i] * invz;
@@ -588,7 +590,7 @@ SV_DEVINL void select_sample_body(const bf16* __restrict__ logits, int vocab, Ge
   __syncthreads();
   if (tid == 0) {
     int tok = s_tok;
-    if (tok < 0) {                                                     // fp rounding fell off the end: last kept id
+    if (tok < 0) {                                                     // no id has any mass (a row of -inf): last kept id
       for (int i = vocab - 1; i >= 0; --i) if (pr[i] * invz > lo) { tok = i; break; }
       if (tok < 0) tok = 0;
     }

@@ -518,3 +518,66 @@ def op_rope(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_head: int
     _lib.check(lib, lib.sv_op_rope(_p(qkv), _p(cos), _p(sin), qkv.shape[0], seq, n_head, n_kv, cos.shape[0], pos0, posv,
                                    int(per_row), _p(kcache), _p(vtcache), tcap, _stream_ptr(qkv.device)))
     return qkv
+
+
+def op_select(impl: int, logits: torch.Tensor, params: GenerationParams, seen: torch.Tensor, out_ids: torch.Tensor,
+              next_ids: torch.Tensor, state: dict, per_row: bool = False, advance_len: int = 1, nsteps: int = 1,
+              amax: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, wte: Optional[torch.Tensor] = None,
+              wpe: Optional[torch.Tensor] = None, x: Optional[torch.Tensor] = None, n_positions: int = 0) -> dict:
+    """`nsteps` token selections from bf16 `logits [B, vocab]` (see sv_op_select); `seen` uint8 `[B, vocab]`, `out_ids` int32
+    `[B, out_stride]`, `next_ids` int32 `[B]` and (fused) `x` are updated in place.  `state` holds the generation state and
+    is updated too: `step, cur_len, done, unfinished[B]`, or with `per_row` `row_len, row_step, row_active, row_max_new,
+    row_seed` (`[B]` each), `row_mask, event`."""
+    lib = _lib.load()
+    B, vocab = logits.shape
+    a = _lib.OpSelect(impl=impl, per_row=int(per_row), logits=logits.data_ptr(), vocab=vocab, B=B, params=params.to_c(),
+                      seen=seen.data_ptr(), out_ids=out_ids.data_ptr(), next_ids=next_ids.data_ptr(),
+                      out_stride=out_ids.shape[1], advance_len=advance_len, nsteps=nsteps)
+    i32p = C.POINTER(C.c_int32)
+    if per_row:
+        keys = ("row_len", "row_step", "row_active", "row_max_new")
+        arrs = {k: _i32s(state[k]) for k in keys}
+        seeds = (C.c_uint64 * B)(*[int(s) & (2 ** 64 - 1) for s in state["row_seed"]])
+        event = _i32s([state["event"]])
+        for k in keys:
+            setattr(a, k + "_host", C.cast(arrs[k], i32p))
+        a.row_seed_host, a.event_host = C.cast(seeds, C.POINTER(C.c_uint64)), C.cast(event, i32p)
+        a.row_mask = int(state["row_mask"])
+    else:
+        counters = _i32s([state["step"], state["cur_len"], state["done"]])
+        unfinished = _i32s(state["unfinished"])
+        a.counters_host, a.unfinished_host = C.cast(counters, i32p), C.cast(unfinished, i32p)
+    if amax is not None:
+        a.amax_val, a.amax_idx = amax[0].data_ptr(), amax[1].data_ptr()
+    if wte is not None:
+        a.wte, a.h = wte.data_ptr(), wte.shape[1]
+    if wpe is not None:
+        a.wpe = wpe.data_ptr()
+    if x is not None:
+        a.x = x.data_ptr()
+    a.n_positions = n_positions
+    _lib.check(lib, lib.sv_op_select(C.byref(a), _stream_ptr(logits.device)))
+    if per_row:
+        for k in keys:
+            state[k] = list(arrs[k])[:B]
+        state["row_seed"], state["event"] = list(seeds), int(event[0])
+    else:
+        state["step"], state["cur_len"], state["done"] = (int(v) for v in counters)
+        state["unfinished"] = list(unfinished)[:B]
+    return state
+
+
+def op_beam_candidates(logits: torch.Tensor, bp: "_lib.BeamParams", batch: int, cur_len: int, running_scores,
+                       run_seq: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """One beam-candidates launch over bf16 `logits [batch * num_beams, vocab]` (see sv_op_beam_candidates); `run_seq` int32
+    `[R, seq_stride]` holds each beam's generated ids -> `(cand_key, cand_val, cand_tok)`, `[R, 2 * num_beams]` each."""
+    lib = _lib.load()
+    R, vocab = logits.shape
+    K = 2 * bp.num_beams
+    key = torch.full((R, K), float("nan"), dtype=torch.float32, device=logits.device)
+    val = torch.full_like(key, float("nan"))
+    tok = torch.full((R, K), -1, dtype=torch.int32, device=logits.device)
+    rs = (C.c_float * max(1, len(running_scores)))(*[float(v) for v in running_scores])
+    _lib.check(lib, lib.sv_op_beam_candidates(_p(logits), vocab, C.byref(bp), batch, cur_len, rs, _p(run_seq), run_seq.shape[1],
+                                              _p(key), _p(val), _p(tok), _stream_ptr(logits.device)))
+    return key, val, tok

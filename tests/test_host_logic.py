@@ -122,6 +122,82 @@ def test_rope_ops_reject_on_the_host():
     assert lib.sv_op_rope(p, p, p, 2, 1, 4, 2, 16, -1, None, 0, None, None, 0, None) == _lib.SV_ERR_INVALID
 
 
+def test_select_op_symbols_and_descriptor_layout():
+    assert _lib.ABI_VERSION == 7
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    for name in ("sv_op_select", "sv_op_beam_candidates"):
+        assert name in _header_symbols() and name in _lib.SIGNATURES and name in exported, name
+    # sv_op_select_args: 2 int32, pointer, 2 int32, sv_gen_params (88), 3 pointers, 3 int32 (+4), 7 pointers, uint32 (+4),
+    # 6 pointers, 2 int32
+    o = _lib.OpSelect
+    assert C.sizeof(o) == 272
+    assert (o.params.offset, o.seen.offset, o.out_stride.offset, o.counters_host.offset, o.row_seed_host.offset,
+            o.row_mask.offset, o.event_host.offset, o.amax_val.offset, o.x.offset, o.h.offset) == (
+        24, 112, 136, 152, 200, 208, 216, 224, 256, 264)
+
+
+def _bad_select(**kw):
+    a = dict(impl=0, per_row=0, B=2, vocab=500, nsteps=1, out_stride=8, advance_len=1, step=0, cur_len=5, logits=0x10000,
+             seen=0x20000, out_ids=0x30000, next_ids=0x40000, do_sample=False, temperature=1.0, top_p=1.0, rp=1.0, stop=(),
+             row_step=None, row_len=None, h=64, n_positions=16, wte=0x50000, wpe=0x60000, x=0x70000, amax=False,
+             counters=True, event=True)
+    a.update(kw)
+    B = max(1, min(a["B"], 32))
+    o = _lib.OpSelect(impl=a["impl"], per_row=a["per_row"], logits=a["logits"], vocab=a["vocab"], B=a["B"], seen=a["seen"],
+                      out_ids=a["out_ids"], next_ids=a["next_ids"], out_stride=a["out_stride"], advance_len=a["advance_len"],
+                      nsteps=a["nsteps"], row_mask=0xffff, h=a["h"], n_positions=a["n_positions"], wte=a["wte"],
+                      wpe=a["wpe"], x=a["x"])
+    p = o.params
+    p.max_new_tokens, p.do_sample, p.temperature, p.top_p = 8, int(a["do_sample"]), a["temperature"], a["top_p"]
+    p.repetition_penalty, p.eos_token_id, p.n_stop_ids = a["rp"], 0, a["stop"] if isinstance(a["stop"], int) else len(a["stop"])
+    i32 = lambda v: C.cast((C.c_int32 * len(v))(*v), C.POINTER(C.c_int32))
+    keep = [i32([a["step"], a["cur_len"], 0]), i32([1] * B), i32(a["row_len"] or [5] * B), i32(a["row_step"] or [0] * B),
+            i32([1] * B), i32([8] * B), C.cast((C.c_uint64 * B)(), C.POINTER(C.c_uint64)), i32([0])]
+    if a["counters"]:
+        o.counters_host, o.unfinished_host = keep[0], keep[1]
+    o.row_len_host, o.row_step_host, o.row_active_host, o.row_max_new_host, o.row_seed_host = keep[2:7]
+    if a["event"]:
+        o.event_host = keep[7]
+    if a["amax"]:
+        o.amax_val, o.amax_idx = 0x80000, 0x90000
+    return _lib.load().sv_op_select(C.byref(o), None)
+
+
+@pytest.mark.parametrize("kw", [dict(impl=3), dict(per_row=2), dict(logits=0), dict(seen=0), dict(out_ids=0), dict(next_ids=0),
+                                dict(B=0), dict(B=17), dict(vocab=0), dict(nsteps=0), dict(advance_len=2),
+                                dict(impl=1, temperature=0.0), dict(do_sample=True, temperature=-1.0), dict(impl=1, top_p=0.0),
+                                dict(impl=1, top_p=1.5), dict(impl=1, top_p=float("nan")), dict(rp=0.0), dict(stop=9),
+                                dict(stop=-1), dict(step=7, nsteps=2), dict(step=-1), dict(counters=False),
+                                dict(per_row=1, row_step=[0, 8]), dict(per_row=1, row_len=[-1, 0]),
+                                dict(per_row=1, event=False), dict(impl=2, h=60), dict(impl=2, h=0), dict(impl=2, wte=0),
+                                dict(impl=2, x=0), dict(impl=2, n_positions=0), dict(impl=2, wpe=0x60008),
+                                dict(impl=2, amax=True, nsteps=2)], ids=str)
+def test_select_op_rejects_on_the_host(kw):
+    assert _bad_select(**kw) == _lib.SV_ERR_INVALID
+    assert b"bad select arguments" in _lib.load().sv_last_error(None)
+
+
+@pytest.mark.parametrize("kw", [dict(num_beams=1), dict(num_beams=9), dict(batch=9), dict(max_new_tokens=0), dict(n_stop_ids=9),
+                                dict(early_stopping=3), dict(do_sample=1, temperature=0.0), dict(do_sample=1, top_p=0.0),
+                                dict(do_sample=1, top_p=1.01), dict(repetition_penalty=0.0), dict(vocab=0), dict(vocab=60000),
+                                dict(cur_len=-1), dict(cur_len=9), dict(logits=0), dict(run_seq=0), dict(cand=0),
+                                dict(scores=False)], ids=str)
+def test_beam_candidates_op_rejects_on_the_host(kw):
+    """Among them a vocabulary whose fp32 row plus seen-bits exceed the shared memory the kernel may ask for."""
+    a = dict(num_beams=2, batch=2, max_new_tokens=8, n_stop_ids=0, early_stopping=1, do_sample=0, temperature=1.0, top_p=1.0,
+             repetition_penalty=1.0, vocab=500, cur_len=3, logits=0x10000, run_seq=0x20000, cand=0x30000, scores=True)
+    a.update(kw)
+    bp = _lib.BeamParams(**{k: a[k] for k in ("num_beams", "max_new_tokens", "n_stop_ids", "early_stopping", "do_sample",
+                                              "temperature", "top_p", "repetition_penalty")}, length_penalty=1.0)
+    scores = (C.c_float * 16)() if a["scores"] else None
+    lib = _lib.load()
+    c = C.c_void_p(a["cand"])
+    assert lib.sv_op_beam_candidates(C.c_void_p(a["logits"]), a["vocab"], C.byref(bp), a["batch"], a["cur_len"], scores,
+                                     C.c_void_p(a["run_seq"]), 8, c, c, c, None) == _lib.SV_ERR_INVALID
+    assert b"bad beam_candidates arguments" in lib.sv_last_error(None)
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
 def test_engine_fails_loudly_without_gpu():
     from starvector_b200.engine import Engine
