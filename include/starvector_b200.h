@@ -281,7 +281,8 @@ SV_API int sv_op_linear(int32_t impl, const void* x, const void* w, const void* 
                  int32_t M, int32_t N, int32_t K, int32_t act, void* stream);
 /* ViT self-attention over packed qkv [B*L, 3*heads*64] -> out [B*L, heads*64]. */
 SV_API int sv_op_attention_vit(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, void* stream);
-/* Causal multi-query attention over packed qkv [B*T, heads*D + 2*D] (D=128) -> out [B*T, heads*D]. */
+/* Causal multi-query attention over packed qkv [B*T, heads*D + 2*D] (D=128) -> out [B*T, heads*D]: sv_op_attention_prefill
+ * over zeroed caches this call allocates. */
 SV_API int sv_op_attention_mqa(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, void* stream);
 /* The scoring chunk attention: packed qkv [B*seq, (n_head + 2*n_kv)*D] (D=128) fills a cache with all seq positions;
  * the queries of positions [q0, seq) attend causally (keys > pos - window when window > 0) -> out [B*(seq-q0), n_head*D]. */
@@ -372,6 +373,38 @@ SV_API int sv_op_select(const sv_op_select_args* args, void* stream);
 SV_API int sv_op_beam_candidates(const void* logits, int32_t vocab, const sv_beam_params* p, int32_t batch, int32_t cur_len,
                                  const float* running_scores_host, const int32_t* run_seq, int32_t seq_stride,
                                  float* cand_key, float* cand_val, int32_t* cand_tok, void* stream);
+
+/* The image-encoder, adapter and prefill kernels one launch at a time (the half of a request before the first decode
+ * step).  The caller owns the device tensors; every argument is checked on the host: SV_ERR_INVALID before any launch.
+ * Synchronous on `stream`.  sv_op_layernorm, sv_op_linear and sv_op_attention_vit above are the rest of that half. */
+/* pixels [batch][3][image][image] -> patches [batch * (image / patch)^2][kpad]: row = one patch, columns (c, iy, ix)
+ * row-major, zero from 3 * patch^2 to kpad (the conv as a GEMM). */
+SV_API int sv_op_im2col(const void* pixels, void* patches, int32_t batch, int32_t image, int32_t patch, int32_t kpad,
+                        void* stream);
+/* x [batch][np (+1)][width] = bf16(cat(cls, pe[b]) + pos), or bf16(pe[b] + pos) when cls == NULL (SigLIP);
+ * pe [batch][np][width], cls [width], pos [np (+1)][width]. */
+SV_API int sv_op_vit_assemble(const void* pe, const void* cls, const void* pos, void* x, int32_t batch, int32_t np,
+                              int32_t width, void* stream);
+/* The adapter norm over z [batch][q][h] -> y.  SV_ADAPTER_NORM_SLAB: LayerNorm([q, h]) per image, w and b [q][h]
+ * (rmean, rvar unused; q * h % 8 == 0).  SV_ADAPTER_NORM_TOKENS: eval BatchNorm1d(q), channel = token, w, b, rmean,
+ * rvar [q]. */
+enum { SV_ADAPTER_NORM_SLAB = 0, SV_ADAPTER_NORM_TOKENS = 1 };
+SV_API int sv_op_adapter_norm(int32_t kind, const void* z, const void* w, const void* b, const void* rmean, const void* rvar,
+                              void* y, int32_t batch, int32_t q, int32_t h, float eps, void* stream);
+/* x [batch][q + p][h]: row t = visual[b][t] for t < q, else wte[clamp(ids[b * id_stride + t - q], 0, vocab - 1)]; plus
+ * wpe[pos0 + t] unless wpe == NULL (RoPE models).  ids int32 (device); q = 0, pos0 > 0 is the scoring chunk's form. */
+SV_API int sv_op_embed_prefix(const void* visual, const int32_t* ids, const void* wte, const void* wpe, void* x,
+                              int32_t batch, int32_t q, int32_t p, int32_t h, int32_t vocab, int32_t pos0, int32_t id_stride,
+                              void* stream);
+/* The prefill attention over caches the caller owns (D = 128; kcache [batch][n_kv][tcap][D], vtcache
+ * [batch][n_kv][D][tcap]): the K/V columns of packed qkv [batch * seq][(n_head + 2 n_kv) * D] are written to slots
+ * [0, seq), then token t of each image attends to keys [0, t] (keys > t - window when window > 0) -> out
+ * [batch * seq][n_head * D].  Slots >= seq are not written.  seq <= tcap, tcap % 32 == 0, n_head / n_kv <= 16. */
+SV_API int sv_op_attention_prefill(const void* qkv, void* kcache, void* vtcache, void* out, int32_t batch, int32_t seq,
+                                   int32_t n_head, int32_t n_kv, int32_t tcap, int32_t window, void* stream);
+/* y [M][N] = bf16(x[M,K] . w[N,K]^T) for any N: the resident last-position logits of a scoring call, with the tiling and
+ * rounding of sv_op_lm_logprob.  Only the M * N outputs are written; K % 64 == 0. */
+SV_API int sv_op_lm_logits(const void* x, const void* w, void* y, int32_t M, int32_t N, int32_t K, void* stream);
 
 /* ---- image preprocessing (SURVEY.md §8f-2) ------------------------------------------------ */
 /* Replaces `ImageTrainProcessor.__call__` (reference starvector/data/util.py:40-66: RGBA pasted on white, pad to

@@ -68,6 +68,7 @@ class OpRing(C.Structure):   # sv_op_ring
 
 
 SV_SELECT_GREEDY, SV_SELECT_SAMPLE, SV_SELECT_FUSED = 0, 1, 2
+SV_ADAPTER_NORM_SLAB, SV_ADAPTER_NORM_TOKENS = 0, 1
 
 
 class OpSelect(C.Structure):   # sv_op_select_args
@@ -138,6 +139,12 @@ SIGNATURES = {
     "sv_op_rope": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, C.POINTER(_I), _I, _P, _P, _I, _P]),
     "sv_op_select": (C.c_int, [C.POINTER(OpSelect), _P]),
     "sv_op_beam_candidates": (C.c_int, [_P, _I, C.POINTER(BeamParams), _I, _I, C.POINTER(C.c_float), _P, _I, _P, _P, _P, _P]),
+    "sv_op_im2col": (C.c_int, [_P, _P, _I, _I, _I, _I, _P]),
+    "sv_op_vit_assemble": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "sv_op_adapter_norm": (C.c_int, [_I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _P]),
+    "sv_op_embed_prefix": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "sv_op_attention_prefill": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "sv_op_lm_logits": (C.c_int, [_P, _P, _P, _I, _I, _I, _P]),
     "sv_preproc_create": (C.c_int, [C.POINTER(PreprocDesc), C.c_int, C.POINTER(_P)]),
     "sv_preproc_destroy": (None, [_P]),
     "sv_preproc_last_error": (C.c_char_p, [_P]),

@@ -1726,9 +1726,16 @@ static int op_fail(const char* what, cudaError_t r) {
   return SV_ERR_CUDA;
 }
 
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 int sv_op_layernorm(const void* x, const void* w, const void* b, void* y, int32_t rows, int32_t cols, float eps,
                     void* stream) {
-  if (!x || !w || !b || !y || cols % 8) return fail(nullptr, SV_ERR_INVALID, "bad layernorm arguments");
+  const char* bad = nullptr;
+  if (!x || !w || !b || !y) bad = "null pointer";
+  else if (rows < 1 || cols < 8 || cols % 8) bad = "rows >= 1, cols >= 8 and cols % 8 == 0";
+  else if (!(eps >= 0.f)) bad = "eps < 0";
+  else if (!aligned16(x) || !aligned16(w) || !aligned16(b) || !aligned16(y)) bad = "x, w, b and y must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad layernorm arguments: %s", bad);
   launch_layernorm((const bf16*)x, (const bf16*)w, (const bf16*)b, (bf16*)y, rows, cols, eps, cols, (cudaStream_t)stream);
   cudaError_t r = cudaGetLastError();
   return r == cudaSuccess ? SV_OK : op_fail("layernorm", r);
@@ -1736,7 +1743,18 @@ int sv_op_layernorm(const void* x, const void* w, const void* b, void* y, int32_
 
 int sv_op_linear(int32_t impl, const void* x, const void* w, const void* bias, const void* residual, void* y, int32_t M,
                  int32_t N, int32_t K, int32_t act, void* stream) {
-  if (!x || !w || !y || M < 1 || N < 1 || K < 32) return fail(nullptr, SV_ERR_INVALID, "bad linear arguments");
+  const char* bad = nullptr;
+  const bool wg_ok = wgmma_supported(M, N, K), rg_ok = K >= 32 && K % 32 == 0;
+  if (!x || !w || !y) bad = "x, w and y are required";
+  else if (impl != SV_LINEAR_AUTO && impl != SV_LINEAR_ROWGROUP && impl != SV_LINEAR_TCGEN05) bad = "unknown impl";
+  else if (act < SV_ACT_NONE || act > SV_ACT_SILU) bad = "unknown act";
+  else if (M < 1 || N < 1 || K < 1) bad = "M, N and K must be >= 1";
+  else if (impl == SV_LINEAR_ROWGROUP && !rg_ok) bad = "rowgroup needs K % 32 == 0";
+  else if (impl == SV_LINEAR_TCGEN05 && !wg_ok) bad = "wgmma needs N % 8 == 0 and K % 64 == 0";
+  else if (impl == SV_LINEAR_AUTO && !rg_ok && !(M > 32 && wg_ok)) bad = "no kernel for this shape (AUTO)";
+  else if (!aligned16(x) || !aligned16(w) || !aligned16(y) || !aligned16(bias) || !aligned16(residual))
+    bad = "x, w, bias, residual and y must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad linear arguments: %s (M=%d N=%d K=%d)", bad, M, N, K);
   int r = do_linear(nullptr, impl, (const bf16*)x, (const bf16*)w, (const bf16*)bias, (const bf16*)residual, (bf16*)y, M,
                     N, K, act, (cudaStream_t)stream);
   if (r != SV_OK) return r;
@@ -1745,7 +1763,11 @@ int sv_op_linear(int32_t impl, const void* x, const void* w, const void* bias, c
 }
 
 int sv_op_attention_vit(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, void* stream) {
-  if (!qkv || !out || batch < 1 || seq < 1 || heads < 1) return fail(nullptr, SV_ERR_INVALID, "bad attention arguments");
+  const char* bad = nullptr;
+  if (!qkv || !out) bad = "null pointer";
+  else if (batch < 1 || seq < 1 || heads < 1) bad = "batch, seq and heads must be >= 1";
+  else if (!aligned16(qkv) || !aligned16(out)) bad = "qkv and out must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad attention_vit arguments: %s", bad);
   cudaStream_t st = (cudaStream_t)stream;
   const int seq_pad = (seq + 31) / 32 * 32;
   bf16* vt = nullptr;
@@ -1758,6 +1780,30 @@ int sv_op_attention_vit(const void* qkv, void* out, int32_t batch, int32_t seq, 
   return r == cudaSuccess ? SV_OK : op_fail("attention_vit", r);
 }
 
+// The decoder prefill's attention as run_prefill issues it: the K/V columns of qkv rows [b][0, seq) go to cache slots
+// [0, seq) of image b (kv_write_kernel), then every token attends causally to the cache (attention_heads_kernel).
+int sv_op_attention_prefill(const void* qkv, void* kcache, void* vtcache, void* out, int32_t batch, int32_t seq,
+                            int32_t n_head, int32_t n_kv, int32_t tcap, int32_t window, void* stream) {
+  const char* bad = nullptr;
+  if (!qkv || !kcache || !vtcache || !out) bad = "null pointer";
+  else if (batch < 1 || seq < 1) bad = "batch and seq must be >= 1";
+  else if (n_head < 1 || n_kv < 1 || n_head % n_kv || n_head / n_kv > 16) bad = "n_head % n_kv != 0 or group > 16";
+  else if (tcap < 32 || tcap % 32) bad = "tcap % 32 != 0";
+  else if (seq > tcap) bad = "seq > tcap";
+  else if (window < 0) bad = "window < 0";
+  else if (!aligned16(qkv) || !aligned16(kcache) || !aligned16(vtcache) || !aligned16(out))
+    bad = "qkv, the caches and out must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad attention_prefill arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = 128;
+  launch_kv_scatter((const bf16*)qkv, (bf16*)kcache, (bf16*)vtcache, batch, seq, n_head * D, n_kv, D, tcap, 0, st);
+  launch_attention_heads((const bf16*)qkv, (n_head + 2 * n_kv) * D, (const bf16*)kcache, (const bf16*)vtcache, (bf16*)out,
+                         batch, seq, n_head, n_kv, D, tcap, window, st);
+  cudaError_t r = cudaGetLastError();
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  return r == cudaSuccess ? SV_OK : op_fail("attention_prefill", r);
+}
+
 int sv_op_attention_mqa(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, void* stream) {
   if (!qkv || !out || batch < 1 || seq < 1 || heads < 1 || heads > 16) return fail(nullptr, SV_ERR_INVALID, "bad attention arguments");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1766,13 +1812,11 @@ int sv_op_attention_mqa(const void* qkv, void* out, int32_t batch, int32_t seq, 
   bf16* kc = nullptr;
   cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&kc), 2 * n * 2);
   if (r != cudaSuccess) return op_fail("attention_mqa alloc", r);
-  bf16* vc = kc + n;
-  cudaMemsetAsync(kc, 0, 2 * n * 2, st);
-  launch_kv_scatter((const bf16*)qkv, kc, vc, batch, seq, heads * D, 1, D, tcap, 0, st);
-  launch_attention_heads((const bf16*)qkv, heads * D + 2 * D, kc, vc, (bf16*)out, batch, seq, heads, 1, D, tcap, 0, st);
-  r = cudaStreamSynchronize(st);
+  r = cudaMemsetAsync(kc, 0, 2 * n * 2, st);
+  const int rc = r == cudaSuccess ? sv_op_attention_prefill(qkv, kc, kc + n, out, batch, seq, heads, 1, tcap, 0, stream)
+                                  : op_fail("attention_mqa", r);
   cudaFree(kc);
-  return r == cudaSuccess ? SV_OK : op_fail("attention_mqa", r);
+  return rc;
 }
 
 int sv_op_attention_chunk(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t q0, int32_t n_head, int32_t n_kv,
@@ -1818,7 +1862,6 @@ int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets, float
 // ---- the decode-step kernels one at a time, over caches the caller owns -------------------------------------------
 // Every argument is checked on the host before anything is allocated or launched: a shape the kernels were not built
 // for returns SV_ERR_INVALID instead of reaching a device trap (the ring's bounded waits) or an abort.
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 constexpr size_t kOpState = 512;     // scratch header holding the GenState / RowState the kernels read
 static_assert(sizeof(GenState) <= kOpState && sizeof(RowState) <= kOpState, "the state structs fit the scratch header");
 
@@ -2127,6 +2170,88 @@ int sv_op_beam_candidates(const void* logits, int32_t vocab, const sv_beam_param
   if (r == cudaSuccess) r = cudaStreamSynchronize(st);
   cudaFree(buf);
   return r == cudaSuccess ? SV_OK : op_fail("beam_candidates", r);
+}
+
+// ---- the image-encoder, adapter and prefill kernels one at a time --------------------------------------------------
+static int op_sync(const char* what, cudaStream_t st) {
+  cudaError_t r = cudaGetLastError();
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  return r == cudaSuccess ? SV_OK : op_fail(what, r);
+}
+
+int sv_op_im2col(const void* pixels, void* patches, int32_t batch, int32_t image, int32_t patch, int32_t kpad, void* stream) {
+  const char* bad = nullptr;
+  if (!pixels || !patches) bad = "null pointer";
+  else if (batch < 1 || patch < 1 || image < patch || image % patch) bad = "batch >= 1 and image a multiple of patch";
+  else if (kpad < 3 * patch * patch) bad = "kpad < 3 * patch * patch";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad im2col arguments: %s", bad);
+  launch_im2col((const bf16*)pixels, (bf16*)patches, batch, image, patch, kpad, (cudaStream_t)stream);
+  return op_sync("im2col", (cudaStream_t)stream);
+}
+
+int sv_op_vit_assemble(const void* pe, const void* cls, const void* pos, void* x, int32_t batch, int32_t np, int32_t width,
+                       void* stream) {
+  const char* bad = nullptr;
+  if (!pe || !pos || !x) bad = "pe, pos and x are required";
+  else if (batch < 1 || np < 1 || width < 1) bad = "batch, np and width must be >= 1";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad vit_assemble arguments: %s", bad);
+  launch_vit_assemble((const bf16*)pe, (const bf16*)cls, (const bf16*)pos, (bf16*)x, batch, np, width, (cudaStream_t)stream);
+  return op_sync("vit_assemble", (cudaStream_t)stream);
+}
+
+int sv_op_adapter_norm(int32_t kind, const void* z, const void* w, const void* b, const void* rmean, const void* rvar,
+                       void* y, int32_t batch, int32_t q, int32_t h, float eps, void* stream) {
+  const char* bad = nullptr;
+  if (kind != SV_ADAPTER_NORM_SLAB && kind != SV_ADAPTER_NORM_TOKENS) bad = "unknown kind";
+  else if (!z || !w || !b || !y) bad = "z, w, b and y are required";
+  else if (kind == SV_ADAPTER_NORM_TOKENS && (!rmean || !rvar)) bad = "the token BatchNorm needs rmean and rvar";
+  else if (batch < 1 || q < 1 || h < 1) bad = "batch, q and h must be >= 1";
+  else if (!(eps >= 0.f)) bad = "eps < 0";
+  else if (kind == SV_ADAPTER_NORM_SLAB && ((int64_t)q * h) % 8) bad = "q * h % 8 != 0";
+  else if (kind == SV_ADAPTER_NORM_SLAB && (!aligned16(z) || !aligned16(w) || !aligned16(b) || !aligned16(y)))
+    bad = "z, w, b and y must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad adapter_norm arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (kind == SV_ADAPTER_NORM_TOKENS) {
+    launch_batchnorm_tokens((const bf16*)z, (const bf16*)w, (const bf16*)b, (const bf16*)rmean, (const bf16*)rvar, (bf16*)y,
+                            batch, q, h, eps, st);
+    return op_sync("adapter_norm", st);
+  }
+  float* partial = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&partial), (size_t)batch * 64 * 2 * sizeof(float));
+  if (r != cudaSuccess) return op_fail("adapter_norm alloc", r);
+  launch_slab_layernorm((const bf16*)z, (const bf16*)w, (const bf16*)b, (bf16*)y, partial, batch, (int64_t)q * h, eps, st);
+  const int rc = op_sync("adapter_norm", st);
+  cudaFree(partial);
+  return rc;
+}
+
+int sv_op_embed_prefix(const void* visual, const int32_t* ids, const void* wte, const void* wpe, void* x, int32_t batch,
+                       int32_t q, int32_t p, int32_t h, int32_t vocab, int32_t pos0, int32_t id_stride, void* stream) {
+  const char* bad = nullptr;
+  if (!wte || !x) bad = "wte and x are required";
+  else if ((q > 0 && !visual) || (p > 0 && !ids)) bad = "q > 0 needs visual, p > 0 needs ids";
+  else if (batch < 1 || q < 0 || p < 0 || q + p < 1) bad = "batch >= 1, q, p >= 0 and q + p >= 1";
+  else if (h < 8 || h % 8) bad = "h % 8 != 0";
+  else if (vocab < 1 || pos0 < 0 || id_stride < p) bad = "vocab >= 1, pos0 >= 0 and id_stride >= p";
+  else if (!aligned16(visual) || !aligned16(wte) || !aligned16(wpe) || !aligned16(x))
+    bad = "visual, wte, wpe and x must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad embed_prefix arguments: %s", bad);
+  launch_embed_prefix((const bf16*)visual, ids, (const bf16*)wte, (const bf16*)wpe, (bf16*)x, batch, q, p, h, vocab, pos0,
+                      id_stride, (cudaStream_t)stream);
+  return op_sync("embed_prefix", (cudaStream_t)stream);
+}
+
+int sv_op_lm_logits(const void* x, const void* w, void* y, int32_t M, int32_t N, int32_t K, void* stream) {
+  const char* bad = nullptr;
+  if (!x || !w || !y) bad = "null pointer";
+  else if (M < 1 || N < 1 || K < 64 || K % 64) bad = "M, N >= 1 and K % 64 == 0";
+  else if (!aligned16(x) || !aligned16(w)) bad = "x and w must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad lm_logits arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t r = launch_lm_logits((const bf16*)x, (const bf16*)w, (bf16*)y, M, N, K, st);
+  if (r != cudaSuccess) return op_fail("lm_logits", r);
+  return op_sync("lm_logits", st);
 }
 
 }  // extern "C"

@@ -448,6 +448,74 @@ def op_lm_logprob(x: torch.Tensor, w: torch.Tensor, targets: torch.Tensor) -> to
     return out
 
 
+def op_im2col(pixels: torch.Tensor, patch: int, kpad: int) -> torch.Tensor:
+    """bf16 `pixels [B, 3, S, S]` -> patches `[B * (S / patch)^2, kpad]` (columns (c, iy, ix), zero-padded to kpad)."""
+    lib = _lib.load()
+    B, S = pixels.shape[0], pixels.shape[-1]
+    out = torch.empty(B * (S // patch) ** 2, kpad, dtype=torch.bfloat16, device=pixels.device)
+    _lib.check(lib, lib.sv_op_im2col(_p(pixels), _p(out), B, S, patch, kpad, _stream_ptr(pixels.device)))
+    return out
+
+
+def op_vit_assemble(pe: torch.Tensor, cls: Optional[torch.Tensor], pos: torch.Tensor, batch: int) -> torch.Tensor:
+    """`bf16(cat(cls, pe) + pos)` per image (`pe [batch * np, width]`), or `bf16(pe + pos)` without cls."""
+    lib = _lib.load()
+    width = pe.shape[-1]
+    np_ = pe.numel() // width // batch
+    q = np_ + (cls is not None)
+    x = torch.empty(batch * q, width, dtype=torch.bfloat16, device=pe.device)
+    _lib.check(lib, lib.sv_op_vit_assemble(_p(pe), _p(cls), _p(pos), _p(x), batch, np_, width, _stream_ptr(pe.device)))
+    return x
+
+
+def op_adapter_norm(kind: int, z: torch.Tensor, w: torch.Tensor, b: torch.Tensor, rmean: Optional[torch.Tensor] = None,
+                    rvar: Optional[torch.Tensor] = None, eps: float = 1e-5) -> torch.Tensor:
+    """The adapter norm over `z [B, Q, H]`: LayerNorm([Q, H]) (`kind` SV_ADAPTER_NORM_SLAB, w / b `[Q, H]`) or eval
+    BatchNorm1d(Q) (SV_ADAPTER_NORM_TOKENS, w / b / rmean / rvar `[Q]`)."""
+    lib = _lib.load()
+    B, Q, H = z.shape
+    y = torch.empty_like(z)
+    _lib.check(lib, lib.sv_op_adapter_norm(kind, _p(z), _p(w), _p(b), _p(rmean), _p(rvar), _p(y), B, Q, H, eps,
+                                           _stream_ptr(z.device)))
+    return y
+
+
+def op_embed_prefix(visual: Optional[torch.Tensor], ids: Optional[torch.Tensor], wte: torch.Tensor, wpe: Optional[torch.Tensor],
+                    batch: int, q: int, p: int, pos0: int = 0, id_stride: Optional[int] = None) -> torch.Tensor:
+    """`[batch * (q + p), h]`: visual rows then `wte[clamp(id)]` rows, `+ wpe[pos0 + t]` unless wpe is None.  `ids` int32
+    with row b's ids at `b * id_stride` (default p)."""
+    lib = _lib.load()
+    h, vocab = wte.shape[1], wte.shape[0]
+    x = torch.empty(batch * (q + p), h, dtype=torch.bfloat16, device=wte.device)
+    _lib.check(lib, lib.sv_op_embed_prefix(_p(visual), _p(ids), _p(wte), _p(wpe), _p(x), batch, q, p, h, vocab, pos0,
+                                           p if id_stride is None else id_stride, _stream_ptr(wte.device)))
+    return x
+
+
+def op_attention_prefill(qkv: torch.Tensor, kcache: torch.Tensor, vtcache: torch.Tensor, seq: int, n_head: int, n_kv: int,
+                         window: int = 0) -> torch.Tensor:
+    """The prefill attention over caller-owned caches `kcache [>= B, n_kv, tcap, 128]`, `vtcache [>= B, n_kv, 128, tcap]`:
+    slots `[0, seq)` of images `b < B` get the K/V of packed qkv `[B * seq, (n_head + 2 n_kv) * 128]`, then causal attention
+    -> `[B * seq, n_head * 128]`."""
+    lib = _lib.load()
+    B, tcap = qkv.shape[0] // seq, kcache.shape[2]
+    out = torch.empty(B * seq, n_head * 128, dtype=torch.bfloat16, device=qkv.device)
+    _lib.check(lib, lib.sv_op_attention_prefill(_p(qkv), _p(kcache), _p(vtcache), _p(out), B, seq, n_head, n_kv, tcap, window,
+                                                _stream_ptr(qkv.device)))
+    return out
+
+
+def op_lm_logits(x: torch.Tensor, w: torch.Tensor, y: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """`bf16(x @ w.T)` for any N on the scoring lm_head tiling; `y` (at least M * N elements) may be given."""
+    lib = _lib.load()
+    M, K = x.shape
+    N = w.shape[0]
+    if y is None:
+        y = torch.empty(M, N, dtype=torch.bfloat16, device=x.device)
+    _lib.check(lib, lib.sv_op_lm_logits(_p(x), _p(w), _p(y), M, N, K, _stream_ptr(x.device)))
+    return y
+
+
 def _i32s(v) -> C.Array:
     v = [int(a) for a in v]
     return (C.c_int32 * max(1, len(v)))(*v)

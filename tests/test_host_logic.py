@@ -122,6 +122,86 @@ def test_rope_ops_reject_on_the_host():
     assert lib.sv_op_rope(p, p, p, 2, 1, 4, 2, 16, -1, None, 0, None, None, 0, None) == _lib.SV_ERR_INVALID
 
 
+PREFILL_OPS = ("sv_op_im2col", "sv_op_vit_assemble", "sv_op_adapter_norm", "sv_op_embed_prefix", "sv_op_attention_prefill",
+               "sv_op_lm_logits")
+
+
+def test_prefill_op_symbols():
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    for name in PREFILL_OPS:
+        assert name in _header_symbols() and name in _lib.SIGNATURES and name in exported, name
+
+
+_A, _U = 0x10000, 0x10008      # a 16-byte aligned and a misaligned device address (never dereferenced: rejected first)
+
+
+def _prefill_op_calls():
+    p, u, n = C.c_void_p(_A), C.c_void_p(_U), None
+    RG, WG, AUTO = _lib.SV_LINEAR_ROWGROUP, _lib.SV_LINEAR_TCGEN05, _lib.SV_LINEAR_AUTO
+    return {
+        "layernorm null": ("sv_op_layernorm", (n, p, p, p, 4, 64, 1e-5, n)),
+        "layernorm rows 0": ("sv_op_layernorm", (p, p, p, p, 0, 64, 1e-5, n)),
+        "layernorm cols % 8": ("sv_op_layernorm", (p, p, p, p, 4, 60, 1e-5, n)),
+        "layernorm misaligned": ("sv_op_layernorm", (u, p, p, p, 4, 64, 1e-5, n)),
+        "linear null": ("sv_op_linear", (WG, p, n, n, n, p, 4, 64, 64, 0, n)),
+        "linear M 0": ("sv_op_linear", (WG, p, p, n, n, p, 0, 64, 64, 0, n)),
+        "linear N 0": ("sv_op_linear", (RG, p, p, n, n, p, 4, 0, 64, 0, n)),
+        "linear rowgroup K % 32": ("sv_op_linear", (RG, p, p, n, n, p, 4, 64, 48, 0, n)),
+        "linear wgmma N % 8": ("sv_op_linear", (WG, p, p, n, n, p, 64, 60, 64, 0, n)),
+        "linear wgmma K % 64": ("sv_op_linear", (WG, p, p, n, n, p, 64, 64, 96, 0, n)),
+        "linear auto no kernel": ("sv_op_linear", (AUTO, p, p, n, n, p, 64, 64, 48, 0, n)),
+        "linear impl": ("sv_op_linear", (3, p, p, n, n, p, 4, 64, 64, 0, n)),
+        "linear act": ("sv_op_linear", (RG, p, p, n, n, p, 4, 64, 64, 4, n)),
+        "linear misaligned bias": ("sv_op_linear", (RG, p, p, u, n, p, 4, 64, 64, 0, n)),
+        "attention_vit null": ("sv_op_attention_vit", (n, p, 1, 17, 2, n)),
+        "attention_vit heads 0": ("sv_op_attention_vit", (p, p, 1, 17, 0, n)),
+        "attention_vit seq 0": ("sv_op_attention_vit", (p, p, 1, 0, 2, n)),
+        "im2col null": ("sv_op_im2col", (n, p, 1, 224, 14, 640, n)),
+        "im2col image % patch": ("sv_op_im2col", (p, p, 1, 225, 14, 640, n)),
+        "im2col kpad": ("sv_op_im2col", (p, p, 1, 224, 14, 587, n)),
+        "im2col batch 0": ("sv_op_im2col", (p, p, 0, 224, 14, 640, n)),
+        "vit_assemble null pos": ("sv_op_vit_assemble", (p, p, n, p, 1, 256, 1024, n)),
+        "vit_assemble np 0": ("sv_op_vit_assemble", (p, p, p, p, 1, 0, 1024, n)),
+        "adapter_norm kind": ("sv_op_adapter_norm", (2, p, p, p, p, p, p, 1, 257, 2048, 1e-5, n)),
+        "adapter_norm tokens without stats": ("sv_op_adapter_norm", (1, p, p, p, n, p, p, 1, 257, 2048, 1e-5, n)),
+        "adapter_norm slab % 8": ("sv_op_adapter_norm", (0, p, p, p, n, n, p, 1, 3, 3, 1e-5, n)),
+        "adapter_norm misaligned": ("sv_op_adapter_norm", (0, u, p, p, n, n, p, 1, 257, 2048, 1e-5, n)),
+        "adapter_norm q 0": ("sv_op_adapter_norm", (1, p, p, p, p, p, p, 1, 0, 2048, 1e-5, n)),
+        "adapter_norm eps < 0": ("sv_op_adapter_norm", (0, p, p, p, n, n, p, 1, 257, 2048, -1.0, n)),
+        "embed_prefix no visual": ("sv_op_embed_prefix", (n, p, p, p, p, 1, 257, 2, 2048, 49156, 0, 2, n)),
+        "embed_prefix no ids": ("sv_op_embed_prefix", (p, n, p, p, p, 1, 257, 2, 2048, 49156, 0, 2, n)),
+        "embed_prefix h % 8": ("sv_op_embed_prefix", (p, p, p, p, p, 1, 257, 2, 2044, 49156, 0, 2, n)),
+        "embed_prefix empty": ("sv_op_embed_prefix", (p, p, p, p, p, 1, 0, 0, 2048, 49156, 0, 0, n)),
+        "embed_prefix id_stride < p": ("sv_op_embed_prefix", (n, p, p, p, p, 1, 0, 16, 2048, 49156, 300, 8, n)),
+        "embed_prefix pos0 < 0": ("sv_op_embed_prefix", (n, p, p, p, p, 1, 0, 16, 2048, 49156, -1, 16, n)),
+        "embed_prefix misaligned wpe": ("sv_op_embed_prefix", (p, p, p, u, p, 1, 257, 2, 2048, 49156, 0, 2, n)),
+        "attention_prefill null": ("sv_op_attention_prefill", (p, n, p, p, 1, 40, 16, 1, 64, 0, n)),
+        "attention_prefill group": ("sv_op_attention_prefill", (p, p, p, p, 1, 40, 6, 4, 64, 0, n)),
+        "attention_prefill group > 16": ("sv_op_attention_prefill", (p, p, p, p, 1, 40, 17, 1, 64, 0, n)),
+        "attention_prefill tcap % 32": ("sv_op_attention_prefill", (p, p, p, p, 1, 40, 16, 1, 48, 0, n)),
+        "attention_prefill seq > tcap": ("sv_op_attention_prefill", (p, p, p, p, 1, 65, 16, 1, 64, 0, n)),
+        "attention_prefill window < 0": ("sv_op_attention_prefill", (p, p, p, p, 1, 40, 16, 1, 64, -1, n)),
+        "attention_prefill misaligned": ("sv_op_attention_prefill", (p, u, p, p, 1, 40, 16, 1, 64, 0, n)),
+        "attention_prefill batch 0": ("sv_op_attention_prefill", (p, p, p, p, 0, 40, 16, 1, 64, 0, n)),
+        "attention_mqa heads > 16": ("sv_op_attention_mqa", (p, p, 1, 40, 17, n)),
+        "lm_logits K % 64": ("sv_op_lm_logits", (p, p, p, 1, 49156, 2000, n)),
+        "lm_logits M 0": ("sv_op_lm_logits", (p, p, p, 0, 49156, 2048, n)),
+        "lm_logits null": ("sv_op_lm_logits", (p, p, n, 1, 49156, 2048, n)),
+        "lm_logits misaligned": ("sv_op_lm_logits", (u, p, p, 1, 49156, 2048, n)),
+    }
+
+
+@pytest.mark.parametrize("case", sorted(_prefill_op_calls()))
+def test_prefill_ops_reject_on_the_host(case):
+    """The encoder / adapter / prefill entry points check every argument before any CUDA call: SV_ERR_INVALID here, on a
+    machine without a GPU too."""
+    name, args = _prefill_op_calls()[case]
+    lib = _lib.load()
+    assert getattr(lib, name)(*args) == _lib.SV_ERR_INVALID
+    assert b"bad" in lib.sv_last_error(None)
+
+
 def test_select_op_symbols_and_descriptor_layout():
     assert _lib.ABI_VERSION == 7
     exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
