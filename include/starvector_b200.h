@@ -225,6 +225,36 @@ SV_API int sv_generate_im2svg_host(sv_engine* e, const void* pixels_host, int32_
                             const int32_t* prompt_ids_host, int32_t prompt_len, const sv_gen_params* p,
                             int32_t* out_ids_host, int32_t* out_len_host, void* stream);
 
+/* ---- prompt-lookup speculative decoding (HF generate(prompt_lookup_num_tokens=k), DESIGN.md §7g) ------------------ */
+typedef struct sv_spec_params {
+  int32_t num_tokens;               /* k = prompt_lookup_num_tokens: drafts per verify step, 1 <= k <= max_batch - 1 (<= 15) */
+  int32_t max_matching_ngram_size;  /* >= 1 (HF default 2) */
+} sv_spec_params;
+/* sv_generate (sv_generate_stream when on_tokens != NULL) with drafts from n-gram matches in the row's own generated
+ * tokens, verified k + 1 columns of one cache row per weight stream.  Returns the same out_ids rectangle, out_len and
+ * cache length as sv_generate with the same parameters, bit for bit (greedy and sampling, every stop rule): the drafts
+ * change the speed only.  One image (batch 1), v1 engines on the fused graph decode path (SV_FLOW engines run it on the
+ * graph path).  SV_ERR_UNSUPPORTED for v2, SV_DECODE=legacy, batch > 1 or an open session; SV_ERR_INVALID for k outside
+ * [1, max_batch - 1] or an n-gram size < 1.  Synchronises `stream`. */
+SV_API int sv_generate_speculative(sv_engine* e, const sv_gen_params* p, const sv_spec_params* sp, int32_t* out_ids,
+                                   int32_t* out_len, sv_token_callback on_tokens, void* user, void* stream);
+/* Counters of the last sv_generate_speculative: verify steps, drafts proposed, drafts accepted (any pointer may be NULL). */
+SV_API int sv_last_spec_stats(const sv_engine* e, int32_t* steps, int32_t* drafted, int32_t* accepted);
+/* Teacher-forced verify step (tests): after a one-image prefill (and any sv_decode_step calls), feeds ids_host[0, ncols) as
+ * the columns of one verify forward at positions cur_len + c and writes their logits, fp32 [ncols][vocab].  Column c's
+ * logits are those the (c + 1)-th of ncols successive sv_decode_step calls with these ids returns, bit for bit, when the
+ * decode attention's cluster size (attention_decode_cluster_ncta of the length) is the same for all of them.  The K/V of
+ * the columns are written, the cache length does not advance.  Synchronises `stream`. */
+SV_API int sv_spec_verify_step(sv_engine* e, const int32_t* ids_host, int32_t ncols, float* logits, void* stream);
+/* Host replays of the device rules (tests): the drafts proposed after the history hist[0, n) (returns their count, <= k,
+ * written to out), and one accept walk: columns' selected tokens sel[0, n_live) against the column inputs cols (cols[c] =
+ * draft c for c >= 1) with the plain path's per-token bookkeeping on state {cur_len, step, done} and out_ids (returns the
+ * number of tokens emitted). */
+SV_API int sv_spec_draft_host(const int32_t* hist, int32_t n, int32_t k, int32_t max_ngram, int32_t eos_id, int32_t budget,
+                              int32_t* out);
+SV_API int sv_spec_accept_host(const sv_gen_params* p, int32_t* state, int32_t* out_ids, int32_t out_stride,
+                               const int32_t* sel, const int32_t* cols, int32_t n_live);
+
 /* ---- continuous batching (vLLM-style serving; the reference's fast validator backend,
  * starvector/validation/starvector_vllm_svg_validator.py) -------------------------------------- */
 /* A decode session keeps `slots` (<= max_batch) cache rows; every row decodes at its own position, has its own token cap

@@ -83,6 +83,10 @@ class OpSelect(C.Structure):   # sv_op_select_args
                 ("x", C.c_void_p), ("h", C.c_int32), ("n_positions", C.c_int32)]
 
 
+class SpecParams(C.Structure):   # sv_spec_params
+    _fields_ = [("num_tokens", C.c_int32), ("max_matching_ngram_size", C.c_int32)]
+
+
 TOKEN_CALLBACK =C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32)   # sv_token_callback
 
 # name -> (restype, argtypes); must list every SV_API symbol of the header (tests check this)
@@ -116,6 +120,11 @@ SIGNATURES = {
     "sv_generate": (C.c_int, [_P, C.POINTER(GenParams), _P, _P, _P]),
     "sv_generate_stream": (C.c_int, [_P, C.POINTER(GenParams), _P, _P, TOKEN_CALLBACK, _P, _P]),
     "sv_generate_im2svg_host": (C.c_int, [_P, _P, _I, _P, _I, C.POINTER(GenParams), _P, _P, _P]),
+    "sv_generate_speculative": (C.c_int, [_P, C.POINTER(GenParams), C.POINTER(SpecParams), _P, _P, TOKEN_CALLBACK, _P, _P]),
+    "sv_last_spec_stats": (C.c_int, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
+    "sv_spec_verify_step": (C.c_int, [_P, C.POINTER(_I), _I, _P, _P]),
+    "sv_spec_draft_host": (C.c_int, [C.POINTER(_I), _I, _I, _I, _I, _I, C.POINTER(_I)]),
+    "sv_spec_accept_host": (C.c_int, [C.POINTER(GenParams), C.POINTER(_I), C.POINTER(_I), _I, C.POINTER(_I), C.POINTER(_I), _I]),
     "sv_session_begin": (C.c_int, [_P, C.POINTER(GenParams), _I]),
     "sv_session_admit": (C.c_int, [_P, _P, _I, _P, _I, _P, _P, _P, _P, _P]),
     "sv_session_run": (C.c_int, [_P, _I, _P, _P, _P]),

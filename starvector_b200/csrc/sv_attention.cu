@@ -468,17 +468,19 @@ SV_DEVINL float ld_dsmem(uint32_t local_addr, uint32_t cta_rank) {
 
 // ROWS (the session variant): image b's keys are [0, rows->row_len[b]]; the cluster size stays the launch's, so CTAs
 // of a short row that get no key block still join both cluster barriers and contribute m = -inf.
-template <int D, bool ROWS>
+// MAP (a speculative verify step): query b is column b, reading cache row cmap->row[b] over keys [0, cmap->pos[b]]; the
+// key and block partition is the one plain decode uses at that length with the same cluster size.
+template <int D, bool ROWS, bool MAP = false>
 SV_DEVINL void attention_decode_cluster_body(
     const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
     bf16* __restrict__ out, const GenState* __restrict__ state, const RowState* __restrict__ rows, int n_head, int n_kv,
-    int tcap, float scale_log2, int window) {
+    int tcap, float scale_log2, int window, const svspec::ColMap* __restrict__ cmap = nullptr) {
   extern __shared__ float dsm[];                               // [kDecWarps][PSZ] warp partials | [PSZ] CTA partial
   constexpr int PSZ = 32 + 16 * D;
   float* cta_part = dsm + kDecWarps * PSZ;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   // cur_len was written by the previous token's select kernel (long complete): read it before the PDL wait
-  const int nkeys = (ROWS ? rows->row_len[blockIdx.z] : state->cur_len) + 1;
+  const int nkeys = (MAP ? cmap->pos[blockIdx.z] : ROWS ? rows->row_len[blockIdx.z] : state->cur_len) + 1;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const int cta = blockIdx.x, ncta = gridDim.x, kvh = blockIdx.y, b = blockIdx.z;
   const int group = n_head / n_kv;
@@ -486,7 +488,7 @@ SV_DEVINL void attention_decode_cluster_body(
   const int blk_lo = key_lo / 32, blk_hi = (nkeys + 31) / 32;
   const int per = (blk_hi - blk_lo + ncta - 1) / ncta;
   const int blk0 = blk_lo + cta * per, blk1 = min(blk_hi, blk0 + per);
-  const int64_t bk = (int64_t)b * n_kv + kvh;
+  const int64_t bk = (int64_t)(MAP ? cmap->row[b] : b) * n_kv + kvh;
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
   float acc[D / 8][4], mrow[2], lrow[2];
@@ -570,6 +572,15 @@ __global__ void __launch_bounds__(kDecWarps * 32, 1) attention_decode_cluster_ro
                                          window);
 }
 
+template <int D>
+__global__ void __launch_bounds__(kDecWarps * 32, 1) attention_decode_cluster_map_kernel(
+    const bf16* __restrict__ qkv, int ld, const bf16* __restrict__ kcache, const bf16* __restrict__ vtcache,
+    bf16* __restrict__ out, const svspec::ColMap* __restrict__ cmap, int n_head, int n_kv, int tcap, float scale_log2,
+    int window) {
+  attention_decode_cluster_body<D, false, true>(qkv, ld, kcache, vtcache, out, nullptr, nullptr, n_head, n_kv, tcap,
+                                                scale_log2, window, cmap);
+}
+
 int attention_decode_cluster_ncta(int total_len) {
   const int blocks = (total_len + 31) / 32;
   return std::max(1, std::min(8, (blocks + kDecWarps - 1) / kDecWarps));
@@ -579,14 +590,17 @@ cudaError_t attention_decode_cluster_init() {
   cudaError_t e = cudaFuncSetAttribute(attention_decode_cluster_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (kDecWarps + 1) * (32 + 16 * 128) * (int)sizeof(float));
   if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(attention_decode_cluster_rows_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+  e = cudaFuncSetAttribute(attention_decode_cluster_rows_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (kDecWarps + 1) * (32 + 16 * 128) * (int)sizeof(float));
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(attention_decode_cluster_map_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                               (kDecWarps + 1) * (32 + 16 * 128) * (int)sizeof(float));
 }
 
 cudaError_t launch_attention_decode_cluster(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache,
                                             bf16* out, const GenState* state, int batch, int n_head, int n_kv, int d,
                                             int tcap, int ncta, int window, bool pdl, cudaStream_t st,
-                                            const RowState* rows) {
+                                            const RowState* rows, const svspec::ColMap* cmap) {
   const float scale_log2 = 1.4426950408889634f / sqrtf((float)d);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(ncta, n_kv, batch); cfg.blockDim = dim3(kDecWarps * 32);
@@ -597,7 +611,9 @@ cudaError_t launch_attention_decode_cluster(const bf16* qkv, int q_cols_total, c
   at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at; cfg.numAttrs = pdl ? 2 : 1;
-  cudaError_t e = rows ? cudaLaunchKernelEx(&cfg, attention_decode_cluster_rows_kernel<128>, qkv, q_cols_total, kcache,
+  cudaError_t e = cmap ? cudaLaunchKernelEx(&cfg, attention_decode_cluster_map_kernel<128>, qkv, q_cols_total, kcache,
+                                            vtcache, out, cmap, n_head, n_kv, tcap, scale_log2, window)
+                 : rows ? cudaLaunchKernelEx(&cfg, attention_decode_cluster_rows_kernel<128>, qkv, q_cols_total, kcache,
                                             vtcache, out, rows, n_head, n_kv, tcap, scale_log2, window)
                        : cudaLaunchKernelEx(&cfg, attention_decode_cluster_kernel<128>, qkv, q_cols_total, kcache,
                                             vtcache, out, state, n_head, n_kv, tcap, scale_log2, window);

@@ -25,7 +25,9 @@ namespace mega {
 
 // EPI_QKV_ROW: EPI_QKV of a continuous-batching session, each image row's K/V appended at its own position
 // (RowState::row_len); a separate instantiation, so the EPI_QKV kernels keep their code.
-enum { EPI_PLAIN = 0, EPI_QKV = 1, EPI_LMHEAD = 2, EPI_QKV_ROW = 3 };
+// EPI_QKV_MAP: EPI_QKV of a speculative verify step, column c's K/V appended at (cmap->row[c], cmap->pos[c]) while c is a
+// live column (svspec::ColMap); inert columns append nothing.
+enum { EPI_PLAIN = 0, EPI_QKV = 1, EPI_LMHEAD = 2, EPI_QKV_ROW = 3, EPI_QKV_MAP = 4 };
 
 struct Ctx {
   const Args* a;
@@ -38,6 +40,7 @@ struct Ctx {
   uint32_t ln_s = 0;            // shared address of [ln_w row | ln_b row] (K bf16 each), 0 = read them from global
   const float* bias_s = nullptr;   // [tile][16] biases of this CTA's output rows
   const int32_t* row_len = nullptr;   // EPI_QKV_ROW: per-row KV positions
+  const svspec::ColMap* cmap = nullptr;   // EPI_QKV_MAP: per-column cache row, position and liveness
 };
 
 // ---- consumer: one GEMV phase  Y[B,N] = epi( LN?(X)[B,K] . W[N,K]^T )
@@ -185,6 +188,14 @@ SV_DEVINL void gemv_phase(const Ctx& cx, Ring& r, const bf16* __restrict__ X, co
   int pos_now = 0;
   if constexpr (EPI == EPI_QKV) pos_now = __ldcg(&a.state->cur_len);         // read here, not behind the last MMA
   if constexpr (EPI == EPI_QKV_ROW) pos_now = __ldcg(cx.row_len + min((int)(threadIdx.x >> 4), 15));   // the epilogue row's
+  int row_now = 0;
+  bool live_now = true;
+  if constexpr (EPI == EPI_QKV_MAP) {                                           // the epilogue column's
+    const int c = min((int)(threadIdx.x >> 4), svspec::kMaxCols - 1);
+    pos_now = __ldcg(&cx.cmap->pos[c]);
+    row_now = __ldcg(&cx.cmap->row[c]);
+    live_now = c < __ldcg(&cx.cmap->n_live);
+  }
   for (int tl = 0; tl < p.ntile; ++tl) {
     const int tile = p.tile0 + tl;
     // the epilogue thread's residual value: requested now, used after the MMAs (an L2 round trip off the tail)
@@ -299,6 +310,19 @@ SV_DEVINL void gemv_phase(const Ctx& cx, Ring& r, const bf16* __restrict__ X, co
             } else {
               const int jj = j - a.n_kv * D, kvh = jj / D, dim = jj % D;
               L->vc[(((int64_t)mm * a.n_kv + kvh) * D + dim) * a.tcap + pos] = vb;
+            }
+          }
+        }
+        if constexpr (EPI == EPI_QKV_MAP) {
+          const int q_cols = a.n_head * D, j = col - q_cols;
+          const int pos = pos_now;
+          if (j >= 0 && pos < a.tcap && live_now) {
+            if (j < a.n_kv * D) {
+              const int kvh = j / D, dim = j % D;
+              L->kc[(((int64_t)row_now * a.n_kv + kvh) * a.tcap + pos) * D + dim] = vb;
+            } else {
+              const int jj = j - a.n_kv * D, kvh = jj / D, dim = jj % D;
+              L->vc[(((int64_t)row_now * a.n_kv + kvh) * D + dim) * a.tcap + pos] = vb;
             }
           }
         }
@@ -471,6 +495,14 @@ SV_DEVINL void gemv_phase_wide(const Ctx& cx, Ring& r, const bf16* __restrict__ 
   int pos_now = 0;
   if constexpr (EPI == EPI_QKV) pos_now = __ldcg(&a.state->cur_len);         // read here, not behind the last MMA
   if constexpr (EPI == EPI_QKV_ROW) pos_now = __ldcg(cx.row_len + min((int)(threadIdx.x >> 4), 15));   // the epilogue row's
+  int row_now = 0;
+  bool live_now = true;
+  if constexpr (EPI == EPI_QKV_MAP) {                                           // the epilogue column's
+    const int c = min((int)(threadIdx.x >> 4), svspec::kMaxCols - 1);
+    pos_now = __ldcg(&cx.cmap->pos[c]);
+    row_now = __ldcg(&cx.cmap->row[c]);
+    live_now = c < __ldcg(&cx.cmap->n_live);
+  }
   for (int tl = 0; tl < p.ntile; ++tl) {
     const int tile = p.tile0 + tl;
     // the epilogue thread's residual value: requested now, used after the MMAs (an L2 round trip off the tail)
@@ -585,6 +617,19 @@ SV_DEVINL void gemv_phase_wide(const Ctx& cx, Ring& r, const bf16* __restrict__ 
             }
           }
         }
+        if constexpr (EPI == EPI_QKV_MAP) {
+          const int q_cols = a.n_head * D, j = col - q_cols;
+          const int pos = pos_now;
+          if (j >= 0 && pos < a.tcap && live_now) {
+            if (j < a.n_kv * D) {
+              const int kvh = j / D, dim = j % D;
+              L->kc[(((int64_t)row_now * a.n_kv + kvh) * a.tcap + pos) * D + dim] = vb;
+            } else {
+              const int jj = j - a.n_kv * D, kvh = jj / D, dim = jj % D;
+              L->vc[(((int64_t)row_now * a.n_kv + kvh) * D + dim) * a.tcap + pos] = vb;
+            }
+          }
+        }
       }
       if constexpr (EPI == EPI_LMHEAD) {
         // greedy = argmax over the bf16 logits cast to float, lowest index wins ties (HF _sample): reduce the ROUNDED value
@@ -621,6 +666,7 @@ struct RingGemvArgs {
   int N, K, act;
   int nslots;        // ring depth of THIS launch
   const int32_t* row_len;   // EPI_QKV_ROW: RowState::row_len (KV append position and L2 prefetch range of each row)
+  const svspec::ColMap* cmap;   // EPI_QKV_MAP: the verify step's column map
 };
 
 // The c_attn GEMV's producer warp is idle once its two slabs are on their way: it pulls the K / V^T rows the NEXT kernel (the
@@ -699,6 +745,11 @@ SV_DEVINL void gemv_ring_body(const RingGemvArgs& ra) {
       l2_prefetch_kv(ra.L.kc, ra.L.vc, ra.a.state->cur_len, ra.a.B * ra.a.n_kv, ra.a.tcap, cta, ncta, lane);
     if constexpr (EPI == EPI_QKV_ROW)
       l2_prefetch_kv_rows(ra.L.kc, ra.L.vc, ra.row_len, ra.a.B, ra.a.n_kv, ra.a.tcap, cta, ncta, lane);
+    if constexpr (EPI == EPI_QKV_MAP) {     // the one cache row the columns share, up to the last live position
+      const int64_t r0 = (int64_t)ra.cmap->row[0] * ra.a.n_kv;
+      l2_prefetch_kv(ra.L.kc + r0 * ra.a.tcap * D, ra.L.vc + r0 * D * ra.a.tcap, ra.cmap->pos[0] + ra.cmap->n_live, ra.a.n_kv,
+                     ra.a.tcap, cta, ncta, lane);
+    }
     return;
   }
   Ctx cx;
@@ -706,6 +757,7 @@ SV_DEVINL void gemv_ring_body(const RingGemvArgs& ra) {
   cx.red = reinterpret_cast<float*>(smem + off_red);
   cx.stat = reinterpret_cast<float*>(smem + off_stat);
   if constexpr (EPI == EPI_QKV_ROW) cx.row_len = ra.row_len;
+  if constexpr (EPI == EPI_QKV_MAP) cx.cmap = ra.cmap;
   // immutable parameters (LayerNorm affine, biases of this CTA's rows) are staged into shared memory before the wait on the
   // previous kernel: their HBM misses (~1 us each, two per LayerNorm kernel, one per epilogue) overlap that kernel's tail
   {
@@ -779,7 +831,7 @@ cudaError_t gemv_ring_init() {   // set the shared-memory opt-in outside of any 
                            mega::ring_smem_bytes(mega::STAGES, 2));                                                   \
   if (e != cudaSuccess) return e;
   SV_RING_ATTR(true, mega::EPI_QKV) SV_RING_ATTR(true, mega::EPI_PLAIN) SV_RING_ATTR(true, mega::EPI_LMHEAD)
-  SV_RING_ATTR(false, mega::EPI_PLAIN) SV_RING_ATTR(true, mega::EPI_QKV_ROW)
+  SV_RING_ATTR(false, mega::EPI_PLAIN) SV_RING_ATTR(true, mega::EPI_QKV_ROW) SV_RING_ATTR(true, mega::EPI_QKV_MAP)
 #undef SV_RING_ATTR
   e = cudaFuncSetAttribute(mega::gemv_ring_kernel<true, mega::EPI_PLAIN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, mega::SMEM_BYTES);
   if (e != cudaSuccess) return e;
@@ -821,7 +873,9 @@ void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st) {
   ra.X = g.X; ra.W = g.W; ra.Wt = g.Wt; ra.bias = g.bias; ra.res = g.res; ra.ln_w = g.ln_w; ra.ln_b = g.ln_b; ra.Y = g.Y;
   ra.N = g.N; ra.K = g.K; ra.act = g.act;
   ra.row_len = g.rows ? g.rows->row_len : nullptr;
-  const int epi = (g.rows && g.epi == mega::EPI_QKV) ? (int)mega::EPI_QKV_ROW : g.epi;
+  ra.cmap = g.cmap;
+  const int epi = (g.rows && g.epi == mega::EPI_QKV) ? (int)mega::EPI_QKV_ROW
+                : (g.cmap && g.epi == mega::EPI_QKV) ? (int)mega::EPI_QKV_MAP : g.epi;
   const int nsm = gemv_ring_ncta();
   {   // ring depth: what this CTA will stream, capped so the next kernel's CTA can co-reside (227 KB per SM)
     static int cap = 0;
@@ -844,6 +898,7 @@ void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st) {
   }
   if (ring_row_groups(g.B) == 2) {           // 9-16 rows: two row groups share each weight fragment
     if (ln && epi == mega::EPI_QKV_ROW) launch_ring_t<true, mega::EPI_QKV_ROW, false, 2>(ra, nsm, g.pdl, st);
+    else if (ln && epi == mega::EPI_QKV_MAP) launch_ring_t<true, mega::EPI_QKV_MAP, false, 2>(ra, nsm, g.pdl, st);
     else if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV, false, 2>(ra, nsm, g.pdl, st);
     else if (ln && g.epi == mega::EPI_LMHEAD) launch_ring_t<true, mega::EPI_LMHEAD, false, 2>(ra, nsm, g.pdl, st);
     else if (ln) launch_ring_t<true, mega::EPI_PLAIN, false, 2>(ra, nsm, g.pdl, st);
@@ -851,6 +906,7 @@ void launch_gemv_ring(const RingGemvLaunch& g, cudaStream_t st) {
     return;
   }
   if (ln && epi == mega::EPI_QKV_ROW) launch_ring_t<true, mega::EPI_QKV_ROW>(ra, nsm, g.pdl, st);
+  else if (ln && epi == mega::EPI_QKV_MAP) launch_ring_t<true, mega::EPI_QKV_MAP>(ra, nsm, g.pdl, st);
   else if (ln && g.epi == mega::EPI_QKV) launch_ring_t<true, mega::EPI_QKV>(ra, nsm, g.pdl, st);
   else if (ln && g.epi == mega::EPI_LMHEAD) launch_ring_t<true, mega::EPI_LMHEAD>(ra, nsm, g.pdl, st);
   else if (ln) launch_ring_t<true, mega::EPI_PLAIN>(ra, nsm, g.pdl, st);

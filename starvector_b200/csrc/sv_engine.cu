@@ -20,6 +20,7 @@
 
 #include "../../include/starvector_b200.h"
 #include "sv_kernels.h"
+#include "sv_select.cuh"
 
 using namespace sv;
 
@@ -143,6 +144,13 @@ struct sv_engine {
   bf16* sess_logits = nullptr;               // [max_batch][vocab]: the prefill logits of admitted slots (token 0 is read there)
   std::vector<int> sess_live;                // host: slot holds a request whose finish was not reported yet
   std::vector<int> sess_len;                 // host: tokens of each slot at the last poll
+
+  // prompt-lookup speculative decoding (sv_generate_speculative): device state allocated by the first call, one verify-step
+  // graph per (columns, split count, sampling, PDL)
+  svspec::State* spec = nullptr;
+  RowState* spec_pos = nullptr;              // sv_spec_verify_step: the columns' embedding positions (row_len)
+  std::map<long long, GraphEntry> spec_graphs;
+  int32_t spec_stats[3] = {0, 0, 0};         // steps, drafted, accepted of the last call
 };
 
 namespace {
@@ -557,14 +565,16 @@ int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaS
 // 1 cluster attention) + lm_head, chained with programmatic dependent launch.  `ids` != nullptr embeds those tokens first
 // (teacher forcing / sampling); with nullptr, d_x was already written by select_fused.
 // Leaves bf16 logits in e->logits and per-tile argmax partials in e->amax_*.  rows != nullptr: a session step.
+// cmap != nullptr: a speculative verify step, B columns of one cache row placed by the column map (v1 only).
 int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st,
-                            const RowState* rows = nullptr) {
+                            const RowState* rows = nullptr, const svspec::ColMap* cmap = nullptr) {
   const sv_model_desc& d = e->d;
   const int H = d.hidden, D = d.head_dim;
   if (ids) launch_embed_tokens(ids, e->wte, e->wpe, e->state, e->d_x, B, H, d.vocab, d.n_positions, st, rows);
   bool first = true;
   RingGemvLaunch g{};
   g.B = B; g.ln_eps = d.ln_eps; g.n_head = d.n_head; g.n_kv = d.n_kv_head; g.tcap = e->tcap; g.state = e->state; g.rows = rows;
+  g.cmap = cmap;
   g.amax_val = e->amax_val; g.amax_idx = e->amax_idx;
   auto gemv = [&](const bf16* X, const bf16* W, const uint8_t* Wt, const bf16* bias, const bf16* res, bf16* Y, int N, int K, int act,
                   const bf16* lw, const bf16* lb, int epi, bf16* kc, bf16* vc, bool p) {
@@ -584,7 +594,7 @@ int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, b
       launch_rope_append(e->d_qkv, B, e->qkv_cols, d.n_head, d.n_kv_head, D, e->rope_cos, e->rope_sin, kc, vc, e->state,
                          e->tcap, d.n_positions, pdl, st, rows);
     launch_attention_decode_cluster(e->d_qkv, e->qkv_cols, kc, vc, e->d_attn, e->state, B, d.n_head, d.n_kv_head, D, e->tcap,
-                                    std::min(ncta, 8), e->window, pdl, st, rows);
+                                    std::min(ncta, 8), e->window, pdl, st, rows, cmap);
     gemv(e->d_attn, L.proj_w, tl ? e->t_proj[i] : nullptr, L.proj_b, e->d_x, e->d_x, H, H, SV_ACT_NONE, nullptr, nullptr, 0, nullptr, nullptr, pdl);
     gemv(e->d_x, L.fc_w, tl ? e->t_fc[i] : nullptr, L.fc_b, nullptr, e->d_h, d.n_inner, H, SV_ACT_GELU_TANH, L.ln2_w, L.ln2_b, 0, nullptr, nullptr, pdl);
     gemv(e->d_h, L.fc2_w, tl ? e->t_fc2[i] : nullptr, L.fc2_b, e->d_x, e->d_x, H, d.n_inner, SV_ACT_NONE, nullptr, nullptr, 0, nullptr, nullptr, pdl);
@@ -830,6 +840,7 @@ void sv_engine_destroy(sv_engine* e) {
   cudaDeviceSynchronize();
   for (auto& g : e->graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
   for (auto& g : e->beam_graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
+  for (auto& g : e->spec_graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
   for (void* p : e->allocs) cudaFree(p);
   if (e->host_flag) cudaFreeHost(e->host_flag);
   if (e->host_stream) cudaFreeHost(e->host_stream);
@@ -1041,9 +1052,11 @@ static GenParamsDev gen_params_dev(const sv_gen_params* p, int stop_row0_only, i
 }
 
 // The generate loop.  `cb` (optional) receives the new tokens of every row each time the host polls the device
-// (sv_generate_stream); with cb == NULL the code path is exactly sv_generate's.
+// (sv_generate_stream); with cb == NULL the code path is exactly sv_generate's.  `spec` != NULL: prompt-lookup
+// speculative decoding (sv_generate_speculative): every replay of the step graph verifies k + 1 columns of the one cache
+// row and emits 1 to k + 1 tokens.
 static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids, int32_t* out_len, void* stream,
-                         sv_token_callback cb, void* cb_user) {
+                         sv_token_callback cb, void* cb_user, const sv_spec_params* spec = nullptr) {
   if (!e) return fail(e, SV_ERR_INVALID, "null argument");
   SV_NO_SESSION(e, "sv_generate");
   if (!p || !out_ids) return fail(e, SV_ERR_INVALID, "null argument");
@@ -1056,8 +1069,21 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
   if (p->n_stop_ids < 0 || p->n_stop_ids > 8) return fail(e, SV_ERR_INVALID, "n_stop_ids outside [0,8]");
   if (p->do_sample && !(p->temperature > 0.f)) return fail(e, SV_ERR_INVALID, "temperature must be > 0");
   if (!(p->repetition_penalty > 0.f)) return fail(e, SV_ERR_INVALID, "repetition_penalty must be > 0");
+  const int ncols = spec ? spec->num_tokens + 1 : 0;
+  if (spec) {
+    if (e->v2) return fail(e, SV_ERR_UNSUPPORTED, "sv_generate_speculative: v2 engines decode through the per-op kernels; only v1 is built");
+    if (!e->fused_decode) return fail(e, SV_ERR_UNSUPPORTED, "sv_generate_speculative needs the fused graph decode path (SV_DECODE=legacy is set)");
+    if (B != 1) return fail(e, SV_ERR_UNSUPPORTED, "sv_generate_speculative decodes one image; batch is %d", B);
+    if (spec->num_tokens < 1 || ncols > e->d.max_batch || ncols > svspec::kMaxCols)
+      return fail(e, SV_ERR_INVALID, "prompt_lookup_num_tokens %d outside [1, %d] (max_batch - 1)", spec->num_tokens,
+                  std::min(e->d.max_batch, svspec::kMaxCols) - 1);
+    if (spec->max_matching_ngram_size < 1)
+      return fail(e, SV_ERR_INVALID, "max_matching_ngram_size must be >= 1, got %d", spec->max_matching_ngram_size);
+  }
   SV_CK(e, cudaSetDevice(e->device));
   LaunchScope scope(e);
+  if (spec && !e->spec && dev_alloc(e, &e->spec, 1) != cudaSuccess)
+    return fail(e, SV_ERR_CUDA, "allocation of the speculative decoding state failed: %s", cudaGetErrorString(cudaGetLastError()));
   cudaStream_t caller = (cudaStream_t)stream, st = e->gen_stream;
   SV_CK(e, cudaEventRecord(e->ev_in, caller));
   SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
@@ -1084,11 +1110,20 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
     }
   };
   select_step(/*advance_len=*/0, /*have_partials=*/false, /*pdl=*/false);
+  if (spec) {   // nothing to accept yet (n_live = 0): the first drafts, the column map and the columns' embeddings
+    svspec::State hs;
+    memset(&hs, 0, sizeof(hs));
+    hs.ncols = ncols; hs.k = spec->num_tokens; hs.max_ngram = spec->max_matching_ngram_size;
+    SV_CK(e, cudaMemcpyAsync(e->spec, &hs, sizeof(hs), cudaMemcpyHostToDevice, st));   // pageable: staged synchronously
+    launch_spec_accept(e->state, e->params, e->seen, e->next_ids, e->out_ids, e->d.vocab, e->wte, e->wpe, e->d_x,
+                       e->d.hidden, e->d.n_positions, e->spec, false, st);
+  }
 
   const int nsplit = fused ? attention_decode_cluster_ncta(e->prefix_len + max_new) : nsplit_for(e, e->prefix_len + max_new);
-  const long long key = (long long)B * 100000 + nsplit * 8 + (p->do_sample ? 1 : 0) + (fused ? 2 : 0) + (e->use_pdl ? 4 : 0);
-  GraphEntry& ge = e->graphs[key];
-  const bool flow = e->use_flow && fused_select;
+  const long long key = (long long)(spec ? ncols : B) * 100000 + nsplit * 8 + (p->do_sample ? 1 : 0) + (fused ? 2 : 0) +
+                        (e->use_pdl ? 4 : 0);
+  GraphEntry& ge = spec ? e->spec_graphs[key] : e->graphs[key];
+  const bool flow = e->use_flow && fused_select && !spec;
   if (!ge.exec && max_new > 1 && !flow) {
     for (int attempt = 0; attempt < 2 && !ge.exec; ++attempt) {
       const bool pdl = e->use_pdl && fused && attempt == 0;
@@ -1097,9 +1132,22 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
       cudaGraph_t graph = nullptr;
       SV_CK(e, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
       int r;
-      if (fused) r = run_decode_layers_fused(e, fused_select ? nullptr : e->next_ids, B, nsplit, pdl, st);
-      else r = run_decode_layers(e, e->next_ids, B, nsplit, st);
-      select_step(/*advance_len=*/1, /*have_partials=*/fused, pdl);
+      if (spec) {           // verify step: the columns' inputs were embedded by the previous accept
+        r = run_decode_layers_fused(e, nullptr, ncols, nsplit, pdl, st, nullptr, &e->spec->map);
+        if (fused_select) {
+          launch_select_fused_spec(e->logits, e->d.vocab, e->amax_val, e->amax_idx, ntiles, 8 * ring_row_groups(ncols),
+                                   e->state, e->params, e->seen, e->next_ids, e->out_ids, e->wte, e->wpe, e->d_x,
+                                   e->d.hidden, e->d.n_positions, e->spec, pdl, st);
+        } else {
+          launch_select_sample_spec(e->logits, e->d.vocab, ncols, e->state, e->params, e->seen, e->logits_f32, e->spec, st);
+          launch_spec_accept(e->state, e->params, e->seen, e->next_ids, e->out_ids, e->d.vocab, e->wte, e->wpe, e->d_x,
+                             e->d.hidden, e->d.n_positions, e->spec, false, st);
+        }
+      } else {
+        if (fused) r = run_decode_layers_fused(e, fused_select ? nullptr : e->next_ids, B, nsplit, pdl, st);
+        else r = run_decode_layers(e, e->next_ids, B, nsplit, st);
+        select_step(/*advance_len=*/1, /*have_partials=*/fused, pdl);
+      }
       cudaError_t ce = cudaStreamEndCapture(st, &graph);
       g_launch_counter = &e->launches;
       if (r != SV_OK) { if (graph) cudaGraphDestroy(graph); return r; }
@@ -1173,7 +1221,30 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
       }
     }
   }
-  for (int s = 1; s < max_new && !done && !flow; ++s) {
+  if (spec) {
+    // Each replay emits 1 to k + 1 tokens: replay as many times as the remaining budget needs at full acceptance (at most
+    // `poll`), then read {step, done}.  So the device never runs past max_new_tokens, and past the finish only after an
+    // EOS or a stop, as the plain loop does.
+    int known = 1;
+    while (!done && known < max_new) {
+      const int n_rep = std::max(1, std::min(poll, (max_new - known + ncols - 1) / ncols));
+      for (int i = 0; i < n_rep; ++i) {
+        SV_CK(e, cudaGraphLaunch(ge.exec, st));
+        e->launches += ge.kernels;
+        ++steps;
+      }
+      if (cb) {
+        const int r = poll_device(done);
+        if (r != SV_OK) return r;
+      } else {
+        SV_CK(e, cudaMemcpyAsync(e->host_flag, &e->state->step, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        SV_CK(e, cudaStreamSynchronize(st));
+        done = e->host_flag[1] != 0;
+      }
+      known = e->host_flag[0];
+    }
+  }
+  for (int s = 1; s < max_new && !done && !flow && !spec; ++s) {
     SV_CK(e, cudaGraphLaunch(ge.exec, st));
     e->launches += ge.kernels;
     ++steps;
@@ -1202,6 +1273,7 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
   SV_CK(e, cudaGetLastError());
   SV_CK(e, cudaEventElapsedTime(&e->last_decode_ms, e->ev_t0, e->ev_t1));
   e->last_decode_steps = steps;
+  if (spec) SV_CK(e, cudaMemcpy(e->spec_stats, &e->spec->steps, sizeof(e->spec_stats), cudaMemcpyDeviceToHost));
   e->host_cur_len = e->prefix_len + std::max(0, n_gen - 1);
   e->prefilled = false;   // the cache now holds a finished generation; a new prefill is required
   return SV_OK;
@@ -1215,6 +1287,83 @@ int sv_generate_stream(sv_engine* e, const sv_gen_params* p, int32_t* out_ids, i
                        void* user, void* stream) {
   if (!on_tokens) return fail(e, SV_ERR_INVALID, "sv_generate_stream needs a callback (use sv_generate otherwise)");
   return generate_impl(e, p, out_ids, out_len, stream, on_tokens, user);
+}
+
+int sv_generate_speculative(sv_engine* e, const sv_gen_params* p, const sv_spec_params* sp, int32_t* out_ids,
+                            int32_t* out_len, sv_token_callback on_tokens, void* user, void* stream) {
+  if (!e || !sp) return fail(e, SV_ERR_INVALID, "null argument");
+  if (e->session) return fail(e, SV_ERR_UNSUPPORTED, "sv_generate_speculative: a decode session is open (speculation inside sessions is not built)");
+  return generate_impl(e, p, out_ids, out_len, stream, on_tokens, user, sp);
+}
+
+int sv_last_spec_stats(const sv_engine* e, int32_t* steps, int32_t* drafted, int32_t* accepted) {
+  if (!e) return SV_ERR_INVALID;
+  if (steps) *steps = e->spec_stats[0];
+  if (drafted) *drafted = e->spec_stats[1];
+  if (accepted) *accepted = e->spec_stats[2];
+  return SV_OK;
+}
+
+int sv_spec_verify_step(sv_engine* e, const int32_t* ids_host, int32_t ncols, float* logits, void* stream) {
+  if (!e || !ids_host || !logits) return fail(e, SV_ERR_INVALID, "null argument");
+  SV_NO_SESSION(e, "sv_spec_verify_step");
+  if (e->v2 || !e->fused_decode) return fail(e, SV_ERR_UNSUPPORTED, "sv_spec_verify_step: v1 engines on the fused decode path only");
+  if (!e->prefilled || e->cur_batch != 1) return fail(e, SV_ERR_STATE, "sv_spec_verify_step needs a one-image prefill first");
+  if (ncols < 1 || ncols > std::min(e->d.max_batch, svspec::kMaxCols))
+    return fail(e, SV_ERR_INVALID, "ncols %d outside [1, %d]", ncols, std::min(e->d.max_batch, svspec::kMaxCols));
+  if (e->host_cur_len + ncols > e->d.max_len) return fail(e, SV_ERR_INVALID, "KV cache full (max_len %d)", e->d.max_len);
+  SV_CK(e, cudaSetDevice(e->device));
+  LaunchScope scope(e);
+  if (!e->spec && dev_alloc(e, &e->spec, 1) != cudaSuccess)
+    return fail(e, SV_ERR_CUDA, "allocation of the speculative decoding state failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if (!e->spec_pos && dev_alloc(e, &e->spec_pos, 1) != cudaSuccess)
+    return fail(e, SV_ERR_CUDA, "allocation of the column positions failed: %s", cudaGetErrorString(cudaGetLastError()));
+  cudaStream_t st = (cudaStream_t)stream;
+  const sv_model_desc& d = e->d;
+  svspec::State hs;
+  RowState rs;
+  memset(&hs, 0, sizeof(hs));
+  memset(&rs, 0, sizeof(rs));
+  hs.ncols = ncols;
+  svspec::set_map(hs.map, ncols, ncols, e->host_cur_len);
+  for (int c = 0; c < ncols; ++c) rs.row_len[c] = e->host_cur_len + c;      // the columns' embedding positions
+  SV_CK(e, cudaMemcpyAsync(e->spec, &hs, sizeof(hs), cudaMemcpyHostToDevice, st));   // pageable: staged synchronously
+  SV_CK(e, cudaMemcpyAsync(e->spec_pos, &rs, sizeof(rs), cudaMemcpyHostToDevice, st));
+  SV_CK(e, cudaMemcpyAsync(e->ids_tmp, ids_host, (size_t)ncols * 4, cudaMemcpyHostToDevice, st));
+  launch_embed_tokens(e->ids_tmp, e->wte, e->wpe, e->state, e->d_x, ncols, d.hidden, d.vocab, d.n_positions, st, e->spec_pos);
+  const int r = run_decode_layers_fused(e, nullptr, ncols, attention_decode_cluster_ncta(e->host_cur_len + ncols), false, st,
+                                        nullptr, &e->spec->map);
+  if (r != SV_OK) return r;
+  launch_logits_to_float(e->logits, logits, (int64_t)ncols * d.vocab, st);
+  SV_CK(e, cudaStreamSynchronize(st));
+  SV_CK(e, cudaGetLastError());
+  return SV_OK;
+}
+
+int sv_spec_draft_host(const int32_t* hist, int32_t n, int32_t k, int32_t max_ngram, int32_t eos_id, int32_t budget,
+                       int32_t* out) {
+  if ((!hist && n > 0) || !out || n < 0 || k < 0 || max_ngram < 1) return SV_ERR_INVALID;
+  return svspec::draft_host(hist, n, k, max_ngram, eos_id, budget, out);
+}
+
+int sv_spec_accept_host(const sv_gen_params* p, int32_t* state, int32_t* out_ids, int32_t out_stride, const int32_t* sel,
+                        const int32_t* cols, int32_t n_live) {
+  if (!p || !state || !out_ids || !sel || !cols || n_live < 0 || n_live > svspec::kMaxCols) return SV_ERR_INVALID;
+  if (p->n_stop_ids < 0 || p->n_stop_ids > 8 || out_stride < p->max_new_tokens) return SV_ERR_INVALID;
+  GenState gs;
+  memset(&gs, 0, sizeof(gs));
+  gs.cur_len = state[0]; gs.step = state[1]; gs.done = state[2]; gs.unfinished[0] = state[2] ? 0 : 1;
+  const GenParamsDev hp = gen_params_dev(p, p->stop_row0_only, out_stride);
+  int m = 0;
+  if (!gs.done) {
+    m = svspec::accept(sel, cols, n_live, [&](int t) {
+      int tk[1] = {t};
+      select_apply_tokens(tk, 1, /*vocab=*/0, &gs, &hp, nullptr, tk, out_ids, /*advance_len=*/1);
+      return gs.done != 0;
+    });
+  }
+  state[0] = gs.cur_len; state[1] = gs.step; state[2] = gs.done;
+  return m;
 }
 
 int sv_generate_im2svg_host(sv_engine* e, const void* pixels_host, int32_t batch, const int32_t* prompt_ids_host,
@@ -1707,7 +1856,7 @@ const char* sv_engine_describe(sv_engine* e) {
            !e->fused_decode ? "legacy-kernels" : e->use_flow ? (e->flow_realloc ? "dataflow-kernel-setmaxnreg" : "dataflow-kernel") : "ring-gemv-graph",
            e->ring_tiles ? "slab-tiled" : "row-major", (int)e->use_pdl, e->linear_impl, e->d.max_batch, decode_flow_status(),
            e->flow_requested && !e->use_flow && e->d.max_batch > 8 ? " SV_FLOW ignored: the dataflow kernel holds 8 rows, max_batch > 8 runs the graph path" : "",
-           e->use_flow ? " sessions: graph path (the dataflow kernel has no per-row positions)" : "");
+           e->use_flow ? " sessions and speculative decoding: graph path (the dataflow kernel has no per-row positions)" : "");
   e->describe = buf;
   return e->describe.c_str();
 }

@@ -6,6 +6,7 @@
 
 #include "sv_beam_core.h"
 #include "sv_common.cuh"
+#include "sv_spec_core.h"
 
 namespace sv {
 
@@ -155,7 +156,7 @@ cudaError_t attention_decode_cluster_init();
 cudaError_t launch_attention_decode_cluster(const bf16* qkv, int q_cols_total, const bf16* kcache, const bf16* vtcache,
                                             bf16* out, const GenState* state, int batch, int n_head, int n_kv, int d,
                                             int tcap, int ncta, int window, bool pdl, cudaStream_t st,
-                                            const RowState* rows = nullptr);
+                                            const RowState* rows = nullptr, const svspec::ColMap* cmap = nullptr);
 
 // ---- sv_decode_fused.cu : token selection fused with the next step's embedding, PDL-ready
 // rows != nullptr: the session variant (see launch_select_greedy); only the selecting rows' embeddings are written.
@@ -163,6 +164,21 @@ void launch_select_fused(const bf16* logits, int vocab, int batch, const float* 
                          int ntiles, int amax_stride, GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
                          int32_t* out_ids, int advance_len, const bf16* wte, const bf16* wpe, bf16* x, int h,
                          int n_positions, bool pdl, cudaStream_t st, RowState* rows = nullptr, uint32_t row_mask = 0);
+
+// ---- sv_decode_fused.cu : the verify step of sv_generate_speculative (one cache row, sp->ncols columns; sv_spec_core.h).
+// Greedy: per-column selection as launch_select_fused, then accept, next drafts, column map and the columns' embeddings.
+void launch_select_fused_spec(const bf16* logits, int vocab, const float* amax_val, const int* amax_idx, int ntiles,
+                              int amax_stride, GenState* state, const GenParamsDev* params, uint8_t* seen,
+                              int32_t* next_ids, int32_t* out_ids, const bf16* wte, const bf16* wpe, bf16* x, int h,
+                              int n_positions, svspec::State* sp, bool pdl, cudaStream_t st);
+// The same after launch_select_sample_spec (tokens in sp->sel); with sp->map.n_live = 0 it only drafts and embeds.
+void launch_spec_accept(GenState* state, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
+                        int vocab, const bf16* wte, const bf16* wpe, bf16* x, int h, int n_positions, svspec::State* sp,
+                        bool pdl, cudaStream_t st);
+// ---- sv_kernels_basic.cu : sampling of the live columns of a verify step (select_sample_kernel per column, Philox counter
+// (0, step + c), repetition-penalty set = row 0's seen plus drafts 1..c), tokens to sp->sel
+void launch_select_sample_spec(const bf16* logits, int vocab, int ncols, GenState* state, const GenParamsDev* params,
+                               uint8_t* seen, float* probs, svspec::State* sp, cudaStream_t st);
 
 // ---- sv_decode_mega.cu : per-phase weight-ring decode GEMV; layer descriptor shared with sv_decode_flow.cu
 struct MegaLayer {
@@ -184,6 +200,7 @@ struct RingGemvLaunch {
   int* amax_idx;
   bool pdl;
   const RowState* rows;           // != nullptr with epi 1: the session variant, KV appended at rows->row_len[row]
+  const svspec::ColMap* cmap;     // != nullptr with epi 1: a verify step, column c's KV appended at (row[c], pos[c]) if live
 };
 cudaError_t gemv_ring_init();
 bool gemv_ring_supported(int K, bool has_ln);

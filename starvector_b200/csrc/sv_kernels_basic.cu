@@ -505,28 +505,41 @@ SV_DEVINL float philox_uniform(unsigned long long seed, uint32_t c0, uint32_t c1
 }
 
 constexpr int kSampleThreads = 1024;
+
 // `probs` is an fp32 scratch row [B][vocab] (L2 resident): the kernel makes ~34 passes over it.
-template <bool ROWS>
+// SPEC (the verify step of sv_generate_speculative): block b is column b of cache row 0; only live columns select, with
+// row 0's seen set plus drafts 1..b and the counter of the token the column would be in a plain run (0, step + b); the
+// token goes to sp->sel[b] and the bookkeeping is left to spec_accept_kernel.
+template <bool ROWS, bool SPEC = false>
 SV_DEVINL void select_sample_body(const bf16* __restrict__ logits, int vocab, GenState* state,
                                   const GenParamsDev* __restrict__ p, uint8_t* seen, int32_t* next_ids, int32_t* out_ids,
-                                  float* __restrict__ probs, RowState* rows, uint32_t row_mask, int advance_len) {
+                                  float* __restrict__ probs, RowState* rows, uint32_t row_mask, int advance_len,
+                                  svspec::State* sp = nullptr) {
   const int b = blockIdx.x, tid = threadIdx.x;
   if constexpr (ROWS) {
     if (!session_row_selects(rows, row_mask, b)) return;
   } else {
     if (state->done) return;
   }
+  if constexpr (SPEC) {
+    if (b >= sp->map.n_live) return;
+  }
   __shared__ float smf[32];
   __shared__ float s_bcast;
   __shared__ int s_tok;
+  __shared__ int s_cols[SPEC ? svspec::kMaxCols : 1];
+  if constexpr (SPEC) {
+    if (tid < svspec::kMaxCols) s_cols[tid] = sp->tok[tid];
+    __syncthreads();
+  }
   const bf16* lr = logits + (int64_t)b * vocab;
-  const uint8_t* sr = seen + (int64_t)b * vocab;
+  const uint8_t* sr = seen + (int64_t)(SPEC ? 0 : b) * vocab;
   float* pr = probs + (int64_t)b * vocab;
   const float rp = p->rep_penalty, invT = 1.0f / p->temperature;
   float mx = -INFINITY;
   for (int i = tid; i < vocab; i += kSampleThreads) {
     float v = __bfloat162float(lr[i]);
-    if (rp != 1.0f && sr[i]) v = v < 0.f ? v * rp : v / rp;            // RepetitionPenaltyLogitsProcessor
+    if (rp != 1.0f && (sr[i] || (SPEC && svspec::drafted(s_cols, b, i)))) v = v < 0.f ? v * rp : v / rp;   // RepetitionPenaltyLogitsProcessor
     v *= invT;                                                         // TemperatureLogitsWarper
     pr[i] = v;
     mx = fmaxf(mx, v);
@@ -569,6 +582,7 @@ SV_DEVINL void select_sample_body(const bf16* __restrict__ logits, int vocab, Ge
   if (tid == 0) {
     // session rows: the counter of a one-row generate with the row's own seed (the slot index does not enter it)
     if constexpr (ROWS) s_bcast = philox_uniform(rows->row_seed[b], 0u, (uint32_t)rows->row_step[b]) * total;
+    else if constexpr (SPEC) s_bcast = philox_uniform(p->seed, 0u, (uint32_t)(state->step + b)) * total;
     else s_bcast = philox_uniform(p->seed, (uint32_t)b, (uint32_t)state->step) * total;
     s_tok = -1;
   }
@@ -595,8 +609,21 @@ SV_DEVINL void select_sample_body(const bf16* __restrict__ logits, int vocab, Ge
       if (tok < 0) tok = 0;
     }
     if constexpr (ROWS) session_append_token(b, tok, rows, p, seen, vocab, next_ids, out_ids, advance_len);
+    else if constexpr (SPEC) sp->sel[b] = tok;
     else append_token(b, tok, state, p, seen, vocab, next_ids, out_ids);
   }
+}
+__global__ void __launch_bounds__(kSampleThreads) select_sample_spec_kernel(const bf16* __restrict__ logits, int vocab,
+                                                                            GenState* state,
+                                                                            const GenParamsDev* __restrict__ p,
+                                                                            uint8_t* seen, float* __restrict__ probs,
+                                                                            svspec::State* sp) {
+  select_sample_body<false, true>(logits, vocab, state, p, seen, nullptr, nullptr, probs, nullptr, 0u, 0, sp);
+}
+void launch_select_sample_spec(const bf16* logits, int vocab, int ncols, GenState* state, const GenParamsDev* params,
+                               uint8_t* seen, float* probs, svspec::State* sp, cudaStream_t st) {
+  select_sample_spec_kernel<<<ncols, kSampleThreads, 0, st>>>(logits, vocab, state, params, seen, probs, sp);
+  count_launch();
 }
 __global__ void __launch_bounds__(kSampleThreads) select_sample_kernel(const bf16* __restrict__ logits, int vocab,
                                                                        GenState* state,

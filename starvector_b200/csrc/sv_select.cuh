@@ -9,8 +9,9 @@ namespace sv {
 struct AmaxPair { float v; int i; };
 SV_DEVINL AmaxPair amax_better(AmaxPair a, AmaxPair b) { return (b.v > a.v || (b.v == a.v && b.i < a.i)) ? b : a; }
 
-// toks[b] in: selected ids; out: ids after the EOS->pad rule (what gets fed to the next step).
-SV_DEVINL void select_apply_tokens(int* toks, int batch, int vocab, GenState* state, const GenParamsDev* p,
+// toks[b] in: selected ids; out: ids after the EOS->pad rule (what gets fed to the next step).  Also compiled for the host:
+// sv_spec_accept_host replays the speculative accept walk with it.
+__host__ __device__ __forceinline__ void select_apply_tokens(int* toks, int batch, int vocab, GenState* state, const GenParamsDev* p,
                                    uint8_t* seen, int32_t* next_ids, int32_t* out_ids, int advance_len) {
   const int step = state->step;
   for (int b = 0; b < batch; ++b) {

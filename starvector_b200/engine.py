@@ -33,6 +33,10 @@ class GenerationParams:
     stop_row0_only: bool = True
     seed: int = 0
     poll_interval: int = 16
+    # prompt-lookup speculative decoding (HF `prompt_lookup_num_tokens` / `max_matching_ngram_size`): > 0 drafts up to that
+    # many tokens per step from n-gram matches in the generated tokens (`sv_generate_speculative`); the tokens are the same
+    prompt_lookup_num_tokens: int = 0
+    max_matching_ngram_size: int = 2
 
     def to_c(self) -> _lib.GenParams:
         if len(self.stop_ids) > 8:
@@ -267,7 +271,15 @@ class Engine:
         out = torch.empty(B, max(n, 1), dtype=torch.int32, device=self.device)
         olen = torch.empty(B, dtype=torch.int32, device=self.device)
         cp = params.to_c()
-        if on_tokens is None:
+        spec = None
+        if params.prompt_lookup_num_tokens > 0:        # one image: `sv_generate_speculative`, the same tokens as below
+            spec = _lib.SpecParams(int(params.prompt_lookup_num_tokens), int(params.max_matching_ngram_size))
+        if spec is not None and on_tokens is None:
+            with self._lock:
+                self._ck(self._lib.sv_generate_speculative(self._h, C.byref(cp), C.byref(spec), C.c_void_p(out.data_ptr()),
+                                                           C.c_void_p(olen.data_ptr()), _lib.TOKEN_CALLBACK(), None,
+                                                           _stream_ptr(self.device)))
+        elif on_tokens is None:
             with self._lock:
                 self._ck(self._lib.sv_generate(self._h, C.byref(cp), C.c_void_p(out.data_ptr()), C.c_void_p(olen.data_ptr()),
                                                _stream_ptr(self.device)))
@@ -284,12 +296,32 @@ class Engine:
 
             cb = _lib.TOKEN_CALLBACK(trampoline)
             with self._lock:
-                self._ck(self._lib.sv_generate_stream(self._h, C.byref(cp), C.c_void_p(out.data_ptr()), C.c_void_p(olen.data_ptr()),
-                                                      cb, None, _stream_ptr(self.device)))
+                if spec is not None:
+                    self._ck(self._lib.sv_generate_speculative(self._h, C.byref(cp), C.byref(spec), C.c_void_p(out.data_ptr()),
+                                                               C.c_void_p(olen.data_ptr()), cb, None, _stream_ptr(self.device)))
+                else:
+                    self._ck(self._lib.sv_generate_stream(self._h, C.byref(cp), C.c_void_p(out.data_ptr()),
+                                                          C.c_void_p(olen.data_ptr()), cb, None, _stream_ptr(self.device)))
             if failure:
                 raise failure[0]
         n_gen = int(olen[0].item())
         return out[:, :n_gen]
+
+    def spec_verify_step(self, ids) -> torch.Tensor:
+        """Teacher-forced verify forward (`sv_spec_verify_step`) after a one-image prefill: the logits, fp32 `[len(ids),
+        vocab]`, of ids fed as the columns of one speculative verify step at the next positions (the cache does not advance)."""
+        ids = [int(t) for t in ids]
+        logits = torch.empty(len(ids), self.dims.vocab, dtype=torch.float32, device=self.device)
+        with self._lock:
+            self._ck(self._lib.sv_spec_verify_step(self._h, (C.c_int32 * len(ids))(*ids), len(ids),
+                                                   C.c_void_p(logits.data_ptr()), _stream_ptr(self.device)))
+        return logits
+
+    def last_spec_stats(self) -> Dict[str, int]:
+        """Counters of the last speculative `generate` (`sv_last_spec_stats`): verify steps, drafts proposed, drafts accepted."""
+        v = [C.c_int32() for _ in range(3)]
+        self._ck(self._lib.sv_last_spec_stats(self._h, *(C.byref(x) for x in v)))
+        return {"steps": v[0].value, "drafted": v[1].value, "accepted": v[2].value}
 
     def generate_im2svg_host(self, pixels_host: torch.Tensor, prompt_ids_host: torch.Tensor,
                              params: GenerationParams) -> Tuple[torch.Tensor, int]:

@@ -46,14 +46,23 @@ class _Transformer:
         o = self._o
         params = self._hf_params(kw, prefix_len=inputs_embeds.shape[1])
         nb = int(kw.get("num_beams", 1))
+        k = int(kw.get("prompt_lookup_num_tokens") or 0)
         if nb > 1:
+            if k > 0:                                                           # HF runs beam search and warns
+                warnings.warn("prompt_lookup_num_tokens is ignored with num_beams > 1: beam search runs")
             es = kw.get("early_stopping", False)                                # HF: False (default) | True | "never"
             return o._beam_generate(params, kw, nb, inputs_embeds=inputs_embeds, early_stopping=es if es == "never" else bool(es))
+        if k > 0:                                                               # prompt-lookup assisted generation
+            if inputs_embeds.shape[0] > 1:
+                raise ValueError("assisted generate is only supported for batch_size = 1")
+            params = dataclasses.replace(params, prompt_lookup_num_tokens=k,
+                                         max_matching_ngram_size=int(kw.get("max_matching_ngram_size") or 2))
         o.engine.prefill_embeds(inputs_embeds)
         return o.engine.generate(params).long()
 
     _HANDLED = {"do_sample", "top_p", "temperature", "num_beams", "max_length", "max_new_tokens", "min_length", "repetition_penalty",
-                "length_penalty", "use_cache", "stopping_criteria", "early_stopping", "pad_token_id", "eos_token_id", "seed"}
+                "length_penalty", "use_cache", "stopping_criteria", "early_stopping", "pad_token_id", "eos_token_id", "seed",
+                "prompt_lookup_num_tokens", "max_matching_ngram_size"}
 
     def _hf_params(self, kw: Dict[str, Any], prefix_len: int) -> GenerationParams:
         """HF `generate()` semantics for exactly the kwargs the reference passes (starvector_base.py:228-241, :292-295):
@@ -241,6 +250,17 @@ class StarVectorStarCoder:
             early_stopping=(not self.v2) if early_stopping is None else early_stopping,
             eos_token_id=params.eos_token_id, pad_token_id=params.pad_token_id, stop_ids=params.stop_ids, seed=params.seed)
 
+    def _spec_hint(self, params: GenerationParams, kw: Dict[str, Any], n_images: int) -> GenerationParams:
+        """`prompt_lookup_num_tokens` is a speed hint here (the reference ignores it): speculative decoding runs for one
+        image with one beam on a v1 engine on the fused decode path, with k clamped to max_batch - 1; otherwise the plain
+        path runs.  The tokens are the same either way."""
+        k = min(int(kw.get("prompt_lookup_num_tokens") or 0), self.engine.dims.max_batch - 1)
+        if (k < 1 or n_images != 1 or int(kw.get("_share_prefix", 1)) != 1 or self.v2
+                or "legacy" in self.engine.describe()):
+            return params
+        return dataclasses.replace(params, prompt_lookup_num_tokens=k,
+                                   max_matching_ngram_size=int(kw.get("max_matching_ngram_size") or 2))
+
     # -- the path ------------------------------------------------------------------------
     @torch.no_grad()
     def generate_im2svg_ids(self, batch: Dict[str, torch.Tensor], **kwargs) -> torch.Tensor:
@@ -255,6 +275,7 @@ class StarVectorStarCoder:
             out = self._beam_generate(params, kwargs, num_beams, image=image, prompt_ids=prompt_ids)
             return torch.cat([prompt_ids.to(out.device), out.long()], dim=1)
         mb = self.engine.dims.max_batch
+        params = self._spec_hint(params, kwargs, image.shape[0])
         streamer = kwargs.get("streamer")                                       # serve/model_worker.py:131,172
         if streamer is not None:
             if image.shape[0] > mb:
