@@ -315,11 +315,13 @@ SV_API int sv_op_attention_vit(const void* qkv, void* out, int32_t batch, int32_
  * over zeroed caches this call allocates. */
 SV_API int sv_op_attention_mqa(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t heads, void* stream);
 /* The scoring chunk attention: packed qkv [B*seq, (n_head + 2*n_kv)*D] (D=128) fills a cache with all seq positions;
- * the queries of positions [q0, seq) attend causally (keys > pos - window when window > 0) -> out [B*(seq-q0), n_head*D]. */
+ * the queries of positions [q0, seq) attend causally (keys > pos - window when window > 0) -> out [B*(seq-q0), n_head*D].
+ * sv_op_attention_score over zeroed caches this call allocates. */
 SV_API int sv_op_attention_chunk(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t q0, int32_t n_head,
                                  int32_t n_kv, int32_t window, void* stream);
 /* The fused lm_head log-likelihood: logprob fp32 [M] = log_softmax(float(bf16(x[M,K] . w[N,K]^T)))[m, targets[m]],
- * targets int32 [M] in [0, N) (device); any N, K % 64 == 0. */
+ * targets int32 [M] (device); any N >= 1, K % 64 == 0, x and w 16-byte aligned.  A target outside [0, N) gives NaN.
+ * Checked on the host (SV_ERR_INVALID before any launch); synchronous on `stream`. */
 SV_API int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets, float* logprob, int32_t M, int32_t N,
                             int32_t K, void* stream);
 
@@ -435,6 +437,19 @@ SV_API int sv_op_attention_prefill(const void* qkv, void* kcache, void* vtcache,
 /* y [M][N] = bf16(x[M,K] . w[N,K]^T) for any N: the resident last-position logits of a scoring call, with the tiling and
  * rounding of sv_op_lm_logprob.  Only the M * N outputs are written; K % 64 == 0. */
 SV_API int sv_op_lm_logits(const void* x, const void* w, void* y, int32_t M, int32_t N, int32_t K, void* stream);
+
+/* The teacher-forced scoring kernels one launch at a time (sv_score_tokens), same conventions as above.
+ * The chunk attention over caches the caller owns (D = 128; kcache [batch][n_kv][tcap][D], vtcache [batch][n_kv][D][tcap]):
+ * row [b][t] of packed qkv [batch * C][(n_head + 2 n_kv) * D] is position pos0 + t.  Its K/V columns are written to slots
+ * [pos0, pos0 + C) of image b, then query t attends to keys [0, pos0 + t] (keys > pos0 + t - window when window > 0) ->
+ * out [batch * C][n_head * D].  Slots < pos0 are the prefix an earlier call wrote; slots >= pos0 + C are neither written
+ * nor read into the result.  pos0 + C <= tcap, tcap % 32 == 0, n_head / n_kv <= 16. */
+SV_API int sv_op_attention_score(const void* qkv, void* kcache, void* vtcache, void* out, int32_t batch, int32_t C,
+                                 int32_t pos0, int32_t n_head, int32_t n_kv, int32_t tcap, int32_t window, void* stream);
+/* Position 0 of a scoring call: logprob fp32 [M] = log_softmax(float(logits[m]))[targets[m]] over resident bf16 logits
+ * [M][vocab] (16-byte aligned), with the tiles and merge of sv_op_lm_logprob.  A target outside [0, vocab) gives NaN. */
+SV_API int sv_op_logits_logprob(const void* logits, const int32_t* targets, float* logprob, int32_t M, int32_t vocab,
+                                void* stream);
 
 /* ---- image preprocessing (SURVEY.md §8f-2) ------------------------------------------------ */
 /* Replaces `ImageTrainProcessor.__call__` (reference starvector/data/util.py:40-66: RGBA pasted on white, pad to

@@ -154,6 +154,8 @@ SIGNATURES = {
     "sv_op_embed_prefix": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
     "sv_op_attention_prefill": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "sv_op_lm_logits": (C.c_int, [_P, _P, _P, _I, _I, _I, _P]),
+    "sv_op_attention_score": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "sv_op_logits_logprob": (C.c_int, [_P, _P, _P, _I, _I, _P]),
     "sv_preproc_create": (C.c_int, [C.POINTER(PreprocDesc), C.c_int, C.POINTER(_P)]),
     "sv_preproc_destroy": (None, [_P]),
     "sv_preproc_last_error": (C.c_char_p, [_P]),

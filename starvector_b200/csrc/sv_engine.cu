@@ -1876,6 +1876,7 @@ static int op_fail(const char* what, cudaError_t r) {
 }
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 
 int sv_op_layernorm(const void* x, const void* w, const void* b, void* y, int32_t rows, int32_t cols, float eps,
                     void* stream) {
@@ -1968,44 +1969,117 @@ int sv_op_attention_mqa(const void* qkv, void* out, int32_t batch, int32_t seq, 
   return rc;
 }
 
+// The scoring chunk's attention as run_score_chunk issues it: the K/V columns of qkv rows [b][0, C) go to cache slots
+// [pos0, pos0 + C) of image b (kv_write_kernel at pos0), then query t attends to keys [0, pos0 + t] of the cache
+// (attention_chunk_kernel).  Slots < pos0 hold the prefix an earlier call wrote; slots >= pos0 + C are neither written
+// nor used.
+int sv_op_attention_score(const void* qkv, void* kcache, void* vtcache, void* out, int32_t batch, int32_t C, int32_t pos0,
+                          int32_t n_head, int32_t n_kv, int32_t tcap, int32_t window, void* stream) {
+  const char* bad = nullptr;
+  if (!qkv || !kcache || !vtcache || !out) bad = "null pointer";
+  else if (batch < 1 || C < 1 || pos0 < 0) bad = "batch, C >= 1 and pos0 >= 0";
+  else if (n_head < 1 || n_kv < 1 || n_head % n_kv || n_head / n_kv > 16) bad = "n_head % n_kv != 0 or group > 16";
+  else if (tcap < 32 || tcap % 32) bad = "tcap % 32 != 0";
+  else if ((int64_t)pos0 + C > tcap) bad = "pos0 + C > tcap";
+  else if (window < 0) bad = "window < 0";
+  else if (!aligned16(qkv) || !aligned16(kcache) || !aligned16(vtcache) || !aligned16(out))
+    bad = "qkv, the caches and out must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad attention_score arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = 128, cols = (n_head + 2 * n_kv) * D;
+  launch_kv_scatter((const bf16*)qkv, (bf16*)kcache, (bf16*)vtcache, batch, C, n_head * D, n_kv, D, tcap, pos0, st);
+  cudaError_t r = launch_attention_chunk((const bf16*)qkv, cols, C, (const bf16*)kcache, (const bf16*)vtcache, (bf16*)out,
+                                         batch, C, pos0, n_head, n_kv, D, tcap, window, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  return r == cudaSuccess ? SV_OK : op_fail("attention_score", r);
+}
+
+// All `seq` positions of qkv go to zeroed caches this call allocates, then sv_op_attention_score runs the queries of
+// [q0, seq) (copied to rows of their own) against them.
 int sv_op_attention_chunk(const void* qkv, void* out, int32_t batch, int32_t seq, int32_t q0, int32_t n_head, int32_t n_kv,
                           int32_t window, void* stream) {
   if (!qkv || !out || batch < 1 || seq < 1 || q0 < 0 || q0 >= seq || n_kv < 1 || n_head % n_kv || n_head / n_kv > 16 ||
       window < 0)
     return fail(nullptr, SV_ERR_INVALID, "bad attention arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  const int D = 128, tcap = (seq + 31) / 32 * 32, cols = (n_head + 2 * n_kv) * D;
-  const size_t n = (size_t)batch * n_kv * tcap * D;
+  const int D = 128, tcap = (seq + 31) / 32 * 32, cols = (n_head + 2 * n_kv) * D, C = seq - q0;
+  const size_t n = (size_t)batch * n_kv * tcap * D, row = (size_t)cols * 2;
   bf16* kc = nullptr;
-  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&kc), 2 * n * 2);
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&kc), 2 * n * 2 + (size_t)batch * C * row);
   if (r != cudaSuccess) return op_fail("attention_chunk alloc", r);
   bf16* vc = kc + n;
-  cudaMemsetAsync(kc, 0, 2 * n * 2, st);
-  launch_kv_scatter((const bf16*)qkv, kc, vc, batch, seq, n_head * D, n_kv, D, tcap, 0, st);
-  r = launch_attention_chunk((const bf16*)qkv + (size_t)q0 * cols, cols, seq, kc, vc, (bf16*)out, batch, seq - q0, q0, n_head,
-                             n_kv, D, tcap, window, st);
-  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  bf16* chunk = vc + n;
+  r = cudaMemsetAsync(kc, 0, 2 * n * 2, st);
+  if (r == cudaSuccess) r = cudaMemcpy2DAsync(chunk, C * row, (const bf16*)qkv + (size_t)q0 * cols, seq * row, C * row, batch,
+                                              cudaMemcpyDeviceToDevice, st);
+  int rc = SV_OK;
+  if (r == cudaSuccess) {
+    launch_kv_scatter((const bf16*)qkv, kc, vc, batch, seq, n_head * D, n_kv, D, tcap, 0, st);
+    rc = sv_op_attention_score(chunk, kc, vc, out, batch, C, q0, n_head, n_kv, tcap, window, stream);
+  } else {
+    rc = op_fail("attention_chunk", r);
+  }
   cudaFree(kc);
-  return r == cudaSuccess ? SV_OK : op_fail("attention_chunk", r);
+  return rc;
+}
+
+// Scratch for the (max, sum) partials of M rows and their target logits.  The target logits start as NaN, so a target
+// that no column matches (outside [0, N)) gives NaN instead of whatever the memory held.
+static cudaError_t logprob_scratch(int M, int N, cudaStream_t st, float2** part, float** tl) {
+  const size_t np = (size_t)M * lm_logprob_ntiles(N);
+  void* buf = nullptr;
+  cudaError_t r = cudaMalloc(&buf, np * sizeof(float2) + (size_t)M * sizeof(float));
+  if (r != cudaSuccess) return r;
+  *part = reinterpret_cast<float2*>(buf);
+  *tl = reinterpret_cast<float*>(*part + np);
+  r = cudaMemsetAsync(*tl, 0xff, (size_t)M * sizeof(float), st);      // 0xffffffff: a quiet NaN
+  if (r != cudaSuccess) cudaFree(buf);
+  return r;
 }
 
 int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets, float* logprob, int32_t M, int32_t N, int32_t K,
                      void* stream) {
-  if (!x || !w || !targets || !logprob || M < 1 || N < 1 || K < 64 || K % 64) return fail(nullptr, SV_ERR_INVALID, "bad lm_logprob arguments");
+  const char* bad = nullptr;
+  if (!x || !w || !targets || !logprob) bad = "null pointer";
+  else if (M < 1 || N < 1 || K < 64 || K % 64) bad = "M, N >= 1 and K % 64 == 0";
+  else if (!aligned16(x) || !aligned16(w) || !aligned4(targets) || !aligned4(logprob))
+    bad = "x and w must be 16-byte aligned, targets and logprob 4-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad lm_logprob arguments: %s", bad);
   cudaStream_t st = (cudaStream_t)stream;
-  const int nt = lm_logprob_ntiles(N);
-  void* buf = nullptr;
-  cudaError_t r = cudaMalloc(&buf, (size_t)M * nt * sizeof(float2) + (size_t)M * sizeof(float));
+  float2* part = nullptr;
+  float* tl = nullptr;
+  cudaError_t r = logprob_scratch(M, N, st, &part, &tl);
   if (r != cudaSuccess) return op_fail("lm_logprob alloc", r);
-  float2* part = reinterpret_cast<float2*>(buf);
-  float* tl = reinterpret_cast<float*>(part + (size_t)M * nt);
   r = launch_lm_logprob_partials((const bf16*)x, (const bf16*)w, targets, part, tl, M, N, K, st);
   if (r == cudaSuccess) {
-    launch_logprob_merge(part, nt, tl, M, M, 0, M, logprob, st);
-    r = cudaStreamSynchronize(st);
+    launch_logprob_merge(part, lm_logprob_ntiles(N), tl, M, M, 0, M, logprob, st);
+    r = cudaGetLastError();
+    if (r == cudaSuccess) r = cudaStreamSynchronize(st);
   }
-  cudaFree(buf);
+  cudaFree(part);
   return r == cudaSuccess ? SV_OK : op_fail("lm_logprob", r);
+}
+
+// Position 0 of a scoring call: the log-likelihood of targets[m] under resident bf16 logits [M][vocab]
+// (logits_logprob_partials_kernel, then the merge).
+int sv_op_logits_logprob(const void* logits, const int32_t* targets, float* logprob, int32_t M, int32_t vocab, void* stream) {
+  const char* bad = nullptr;
+  if (!logits || !targets || !logprob) bad = "null pointer";
+  else if (M < 1 || vocab < 1) bad = "M and vocab must be >= 1";
+  else if (!aligned16(logits) || !aligned4(targets) || !aligned4(logprob))
+    bad = "logits must be 16-byte aligned, targets and logprob 4-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad logits_logprob arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  float2* part = nullptr;
+  float* tl = nullptr;
+  cudaError_t r = logprob_scratch(M, vocab, st, &part, &tl);
+  if (r != cudaSuccess) return op_fail("logits_logprob alloc", r);
+  launch_logits_logprob_partials((const bf16*)logits, vocab, M, targets, part, tl, st);
+  launch_logprob_merge(part, lm_logprob_ntiles(vocab), tl, M, M, 0, M, logprob, st);
+  r = cudaGetLastError();
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(part);
+  return r == cudaSuccess ? SV_OK : op_fail("logits_logprob", r);
 }
 
 // ---- the decode-step kernels one at a time, over caches the caller owns -------------------------------------------

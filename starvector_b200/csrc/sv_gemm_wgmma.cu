@@ -206,7 +206,9 @@ __global__ void __launch_bounds__(kThreads, 2) linear_wgmma_kernel(const __grid_
     for (int i = 0; i < BN / 2; ++i) se[(i >> 1) & 1] += expf(acc[i] - mx[(i >> 1) & 1]);
     se[0] = quad_sum(se[0]);
     se[1] = quad_sum(se[1]);
-    const int tg0 = r0 < M ? targets[r0] : -1, tg1 = r0 + 8 < M ? targets[r0 + 8] : -1;
+    int tg0 = r0 < M ? targets[r0] : -1, tg1 = r0 + 8 < M ? targets[r0 + 8] : -1;
+    tg0 = tg0 < N ? tg0 : -1;                                       // a column past N (-inf) is no target
+    tg1 = tg1 < N ? tg1 : -1;
     float tv0 = 0.f, tv1 = 0.f;
     bool hit0 = false, hit1 = false;
 #pragma unroll

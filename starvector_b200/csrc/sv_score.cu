@@ -30,7 +30,7 @@ __global__ void __launch_bounds__(128) logits_logprob_partials_kernel(const bf16
   const int tile = blockIdx.x, row = blockIdx.y, col = tile * 128 + threadIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float v = col < vocab ? __bfloat162float(logits[(int64_t)row * vocab + col]) : -INFINITY;
-  if (col == targets[row]) tgt_logit[row] = v;
+  if (col < vocab && col == targets[row]) tgt_logit[row] = v;      // the padded tail of the last tile is no target
   float m = warp_max(v);
   if (lane == 0) red[warp] = m;
   __syncthreads();

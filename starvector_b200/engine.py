@@ -548,6 +548,30 @@ def op_lm_logits(x: torch.Tensor, w: torch.Tensor, y: Optional[torch.Tensor] = N
     return y
 
 
+def op_attention_score(qkv: torch.Tensor, kcache: torch.Tensor, vtcache: torch.Tensor, chunk: int, pos0: int, n_head: int,
+                       n_kv: int, window: int = 0) -> torch.Tensor:
+    """The scoring chunk attention over caller-owned caches `kcache [>= B, n_kv, tcap, 128]`, `vtcache [>= B, n_kv, 128,
+    tcap]`: row `[b][t]` of packed qkv `[B * chunk, (n_head + 2 n_kv) * 128]` is position `pos0 + t`; its K/V go to slot
+    `pos0 + t` of image b, then it attends causally to slots `[0, pos0 + t]` -> `[B * chunk, n_head * 128]`."""
+    lib = _lib.load()
+    B, tcap = qkv.shape[0] // chunk, kcache.shape[2]
+    out = torch.empty(B * chunk, n_head * 128, dtype=torch.bfloat16, device=qkv.device)
+    _lib.check(lib, lib.sv_op_attention_score(_p(qkv), _p(kcache), _p(vtcache), _p(out), B, chunk, pos0, n_head, n_kv, tcap,
+                                              window, _stream_ptr(qkv.device)))
+    return out
+
+
+def op_logits_logprob(logits: torch.Tensor, targets: torch.Tensor) -> torch.Tensor:
+    """`log_softmax(float(logits))[m, targets[m]]` over bf16 `logits [M, vocab]`, fp32 `[M]` (NaN where a target lies
+    outside [0, vocab)): position 0 of a scoring call."""
+    lib = _lib.load()
+    M, V = logits.shape
+    tg = targets.to(device=logits.device, dtype=torch.int32).contiguous()
+    out = torch.empty(M, dtype=torch.float32, device=logits.device)
+    _lib.check(lib, lib.sv_op_logits_logprob(_p(logits), _p(tg), _p(out), M, V, _stream_ptr(logits.device)))
+    return out
+
+
 def _i32s(v) -> C.Array:
     v = [int(a) for a in v]
     return (C.c_int32 * max(1, len(v)))(*v)

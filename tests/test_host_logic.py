@@ -202,6 +202,71 @@ def test_prefill_ops_reject_on_the_host(case):
     assert b"bad" in lib.sv_last_error(None)
 
 
+SCORE_OPS = ("sv_op_attention_score", "sv_op_logits_logprob", "sv_op_lm_logprob", "sv_op_attention_chunk")
+
+
+def test_score_op_symbols():
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    for name in SCORE_OPS:
+        assert name in _header_symbols() and name in _lib.SIGNATURES and name in exported, name
+
+
+def _score_op_calls():
+    p, u, n = C.c_void_p(_A), C.c_void_p(_U), None
+    u2 = C.c_void_p(_A + 2)                   # not even 4-byte aligned
+    #              qkv kc vc out  B  C    pos0 nh nkv tcap  window
+    ok = (p, p, p, p, 1, 256, 259, 16, 1, 544, 0, n)
+
+    def score(i, v):
+        a = list(ok)
+        a[i] = v
+        return ("sv_op_attention_score", tuple(a))
+    return {
+        "attention_score null qkv": score(0, n),
+        "attention_score null vtcache": score(2, n),
+        "attention_score null out": score(3, n),
+        "attention_score batch 0": score(4, 0),
+        "attention_score C 0": score(5, 0),
+        "attention_score pos0 < 0": score(6, -1),
+        "attention_score pos0 + C > tcap": score(6, 289),
+        "attention_score group": ("sv_op_attention_score", (p, p, p, p, 1, 256, 259, 6, 4, 544, 0, n)),
+        "attention_score group > 16": score(7, 17),
+        "attention_score n_kv 0": score(8, 0),
+        "attention_score tcap % 32": score(9, 528),
+        "attention_score window < 0": score(10, -1),
+        "attention_score misaligned qkv": score(0, u),
+        "attention_score misaligned kcache": score(1, u),
+        "attention_chunk q0 >= seq": ("sv_op_attention_chunk", (p, p, 1, 40, 40, 16, 1, 0, n)),
+        "attention_chunk group": ("sv_op_attention_chunk", (p, p, 1, 40, 8, 6, 4, 0, n)),
+        "lm_logprob null targets": ("sv_op_lm_logprob", (p, p, n, p, 4, 49156, 2048, n)),
+        "lm_logprob null out": ("sv_op_lm_logprob", (p, p, p, n, 4, 49156, 2048, n)),
+        "lm_logprob M 0": ("sv_op_lm_logprob", (p, p, p, p, 0, 49156, 2048, n)),
+        "lm_logprob N 0": ("sv_op_lm_logprob", (p, p, p, p, 4, 0, 2048, n)),
+        "lm_logprob K % 64": ("sv_op_lm_logprob", (p, p, p, p, 4, 49156, 2000, n)),
+        "lm_logprob misaligned x": ("sv_op_lm_logprob", (u, p, p, p, 4, 49156, 2048, n)),
+        "lm_logprob misaligned w": ("sv_op_lm_logprob", (p, u, p, p, 4, 49156, 2048, n)),
+        "lm_logprob misaligned targets": ("sv_op_lm_logprob", (p, p, u2, p, 4, 49156, 2048, n)),
+        "logits_logprob null logits": ("sv_op_logits_logprob", (n, p, p, 4, 49156, n)),
+        "logits_logprob null targets": ("sv_op_logits_logprob", (p, n, p, 4, 49156, n)),
+        "logits_logprob null out": ("sv_op_logits_logprob", (p, p, n, 4, 49156, n)),
+        "logits_logprob M 0": ("sv_op_logits_logprob", (p, p, p, 0, 49156, n)),
+        "logits_logprob vocab 0": ("sv_op_logits_logprob", (p, p, p, 4, 0, n)),
+        "logits_logprob misaligned logits": ("sv_op_logits_logprob", (u, p, p, 4, 49156, n)),
+        "logits_logprob misaligned out": ("sv_op_logits_logprob", (p, p, u2, 4, 49156, n)),
+    }
+
+
+@pytest.mark.parametrize("case", sorted(_score_op_calls()))
+def test_score_ops_reject_on_the_host(case):
+    """The scoring entry points check every argument before any CUDA call: SV_ERR_INVALID here, on a machine without a
+    GPU too."""
+    name, args = _score_op_calls()[case]
+    lib = _lib.load()
+    assert getattr(lib, name)(*args) == _lib.SV_ERR_INVALID
+    assert b"bad" in lib.sv_last_error(None)
+
+
 def test_select_op_symbols_and_descriptor_layout():
     assert _lib.ABI_VERSION == 7
     exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],

@@ -101,16 +101,17 @@ def _close_attn(got, ref, dim, ulps=1.0, c=0.02):
     return (err / tol).max().item()
 
 
-def ref_causal_attention(qkv, B, T, n_head, n_kv, window=0, chunk=512):
+def ref_causal_attention(qkv, B, T, n_head, n_kv, window=0, chunk=512, q0=0):
     """fp64 causal attention of packed qkv rows [B*T, (n_head + 2 n_kv) * 128] (query head h reads KV head h // group;
-    keys > t - window when window > 0) -> [B*T, n_head * 128], over chunks of queries."""
+    keys > t - window when window > 0) -> [B*(T - q0), n_head * 128] for the queries of positions [q0, T), over chunks of
+    queries."""
     D, grp = 128, n_head // n_kv
     x = qkv.double().view(B, T, n_head + 2 * n_kv, D)
     q = x[:, :, :n_head].reshape(B, T, n_kv, grp, D)
     k, v = x[:, :, n_head:n_head + n_kv], x[:, :, n_head + n_kv:]
-    out = torch.empty(B, T, n_kv, grp, D, dtype=torch.float64, device=qkv.device)
+    out = torch.empty(B, T - q0, n_kv, grp, D, dtype=torch.float64, device=qkv.device)
     ks = torch.arange(T, device=qkv.device)
-    for t0 in range(0, T, chunk):
+    for t0 in range(q0, T, chunk):
         t1 = min(T, t0 + chunk)
         s = torch.einsum("btkgd,bskd->bkgts", q[:, t0:t1], k) / math.sqrt(D)
         tq = torch.arange(t0, t1, device=qkv.device)[:, None]
@@ -118,8 +119,8 @@ def ref_causal_attention(qkv, B, T, n_head, n_kv, window=0, chunk=512):
         if window > 0:
             mask &= ks[None, :] > tq - window
         p = torch.softmax(s.masked_fill(~mask, float("-inf")), dim=-1)
-        out[:, t0:t1] = torch.einsum("bkgts,bskd->btkgd", p, v)
-    return out.reshape(B * T, n_head * D)
+        out[:, t0 - q0:t1 - q0] = torch.einsum("bkgts,bskd->btkgd", p, v)
+    return out.reshape(B * (T - q0), n_head * D)
 
 
 def plant_strong_keys(x, B, L, groups, dim, positions, seed):
