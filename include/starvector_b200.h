@@ -331,7 +331,9 @@ SV_API int sv_op_lm_logprob(const void* x, const void* w, const int32_t* targets
 enum { SV_ATTN_DECODE_SPLIT = 0 /* split + merge, nsplit in [1, 128] */, SV_ATTN_DECODE_CLUSTER = 1 /* nsplit = CTAs in [1, 8] */ };
 /* Decode attention: row b's query (qkv row b) attends to keys [0, lens_host[b]) of its cache (the last, lens - 1, is the
  * new token; keys > lens - 1 - window when window > 0) -> out [batch][n_head * D].  per_row = 0: the plain kernels
- * (equal lengths); 1: the session kernels.  1 <= lens <= tcap, tcap % 32 == 0, batch <= 16, n_head / n_kv <= 16. */
+ * (equal lengths); 1: the session kernels.  1 <= lens <= tcap, tcap % 32 == 0, batch <= 16, n_head / n_kv <= 16.
+ * per_row = 2: the column map of a speculative verify step (SV_ATTN_DECODE_CLUSTER only, window 0): column c (qkv row c)
+ * attends to keys [0, lens_host[c]] of cache row 0, i.e. lens_host[c] is the column's position, in [0, tcap - 1]. */
 SV_API int sv_op_attention_decode(int32_t impl, int32_t per_row, const void* qkv, const void* kcache, const void* vtcache,
                                   void* out, const int32_t* lens_host, int32_t batch, int32_t n_head, int32_t n_kv,
                                   int32_t tcap, int32_t nsplit, int32_t window, void* stream);
@@ -346,7 +348,10 @@ typedef struct sv_op_ring {
   float ln_eps;
   void *kcache, *vtcache;              /* epi 1 */
   int32_t n_head, n_kv, tcap, per_row;
-  const int32_t* pos_host;             /* epi 1: the append position (per_row = 0: [0] for every row; 1: one per row) */
+  const int32_t* pos_host;             /* epi 1: the append position (per_row = 0: [0] for every row; 1: one per row;
+                                          2: the column map of a speculative verify step, [B + 1]: pos_host[c] = column c's
+                                          position in cache row 0, in [0, tcap - 1], then n_live = pos_host[B]: columns
+                                          [0, n_live) append their K/V, the others write nothing; pos_host[0] + n_live <= tcap) */
   float* amax_val;                     /* epi 2: [sv_op_ring_ntiles(N)][sv_op_ring_row_stride(B)] */
   int32_t* amax_idx;
 } sv_op_ring;
@@ -398,6 +403,38 @@ typedef struct sv_op_select_args {
   int32_t h, n_positions;       /* h % 8 == 0 */
 } sv_op_select_args;
 SV_API int sv_op_select(const sv_op_select_args* args, void* stream);
+/* The selection kernels of a speculative verify step (sv_generate_speculative, one image row) one launch at a time, same
+ * conventions as sv_op_select: the state travels as host structs read on entry and written back. */
+enum {
+  SV_SPEC_GREEDY = 0,  /* select_fused_spec_kernel: per-column greedy selection, the accept walk, next drafts and embeddings */
+  SV_SPEC_SAMPLE = 1,  /* select_sample_spec_kernel (writes sel), then spec_accept_kernel, as the sampled verify graph runs them */
+  SV_SPEC_ACCEPT = 2   /* spec_accept_kernel alone on the given sel (n_live = 0: the first drafts of a generation) */
+};
+/* The device state of one speculative generation (svspec::State, sv_spec_core.h), field for field. */
+typedef struct sv_spec_state {
+  int32_t n_live, row[16], pos[16];  /* the column map: column c < n_live decodes (row[c], pos[c]); the others are inert */
+  int32_t tok[16], sel[16];          /* column inputs (tok[0] the last token, tok[c] draft c) and selected tokens */
+  int32_t ncols, k, max_ngram;       /* columns (k + 1), drafts per step, the largest n-gram matched */
+  int32_t steps, drafted, accepted;  /* counters */
+} sv_spec_state;
+typedef struct sv_op_spec_args {
+  int32_t impl;                 /* SV_SPEC_* */
+  const void* logits;           /* bf16 [ncols][vocab] (GREEDY, SAMPLE) */
+  int32_t vocab;                /* >= 1 */
+  sv_gen_params params;         /* max_new_tokens <= out_stride is the cap; do_sample and poll_interval are ignored */
+  void* seen;                   /* uint8 [vocab]: ids generated so far (repetition penalty), updated */
+  int32_t* out_ids;             /* [out_stride]: the generated ids (the draft history), updated */
+  int32_t* next_ids;            /* [1] */
+  int32_t out_stride;
+  int32_t* gen_host;            /* [4]: step, cur_len, done, unfinished[0] */
+  sv_spec_state* spec_host;
+  const float* amax_val;        /* GREEDY only: lm_head argmax partials [sv_op_ring_ntiles(vocab)][sv_op_ring_row_stride(ncols)], */
+  const int32_t* amax_idx;      /*   or NULL: the logits rows are scanned (always so when repetition_penalty != 1) */
+  const void *wte, *wpe;        /* bf16 [vocab][h], [n_positions][h]; wpe may be NULL */
+  void* x;                      /* bf16 [ncols][h]: the next step's column inputs */
+  int32_t h, n_positions;       /* h % 8 == 0 */
+} sv_op_spec_args;
+SV_API int sv_op_spec_select(const sv_op_spec_args* args, void* stream);
 /* One beam_candidates_kernel launch over R = batch * num_beams rows: logits bf16 [R][vocab]; cur_len = tokens every
  * running beam holds (0: no repetition penalty yet), running_scores_host float [R], run_seq int32 [R][seq_stride] (device,
  * the beams' generated ids) -> cand_key / cand_val float and cand_tok int32 [R][2 * num_beams] (device).  p is checked as

@@ -83,6 +83,22 @@ class OpSelect(C.Structure):   # sv_op_select_args
                 ("x", C.c_void_p), ("h", C.c_int32), ("n_positions", C.c_int32)]
 
 
+SV_SPEC_GREEDY, SV_SPEC_SAMPLE, SV_SPEC_ACCEPT = 0, 1, 2
+
+
+class SpecState(C.Structure):   # sv_spec_state (svspec::State)
+    _fields_ = [("n_live", C.c_int32), ("row", C.c_int32 * 16), ("pos", C.c_int32 * 16), ("tok", C.c_int32 * 16),
+                ("sel", C.c_int32 * 16)] + [(n, C.c_int32) for n in ("ncols", "k", "max_ngram", "steps", "drafted", "accepted")]
+
+
+class OpSpec(C.Structure):   # sv_op_spec_args
+    _fields_ = [("impl", C.c_int32), ("logits", C.c_void_p), ("vocab", C.c_int32), ("params", GenParams),
+                ("seen", C.c_void_p), ("out_ids", C.c_void_p), ("next_ids", C.c_void_p), ("out_stride", C.c_int32),
+                ("gen_host", C.POINTER(C.c_int32)), ("spec_host", C.POINTER(SpecState)),
+                ("amax_val", C.c_void_p), ("amax_idx", C.c_void_p), ("wte", C.c_void_p), ("wpe", C.c_void_p),
+                ("x", C.c_void_p), ("h", C.c_int32), ("n_positions", C.c_int32)]
+
+
 class SpecParams(C.Structure):   # sv_spec_params
     _fields_ = [("num_tokens", C.c_int32), ("max_matching_ngram_size", C.c_int32)]
 
@@ -147,6 +163,7 @@ SIGNATURES = {
     "sv_op_rope_table": (C.c_int, [_P, _P, _I, _I, _F, _P]),
     "sv_op_rope": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, C.POINTER(_I), _I, _P, _P, _I, _P]),
     "sv_op_select": (C.c_int, [C.POINTER(OpSelect), _P]),
+    "sv_op_spec_select": (C.c_int, [C.POINTER(OpSpec), _P]),
     "sv_op_beam_candidates": (C.c_int, [_P, _I, C.POINTER(BeamParams), _I, _I, C.POINTER(C.c_float), _P, _I, _P, _P, _P, _P]),
     "sv_op_im2col": (C.c_int, [_P, _P, _I, _I, _I, _I, _P]),
     "sv_op_vit_assemble": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),

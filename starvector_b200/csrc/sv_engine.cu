@@ -2094,7 +2094,8 @@ int sv_op_attention_decode(int32_t impl, int32_t per_row, const void* qkv, const
   const char* bad = nullptr;
   if (!qkv || !kcache || !vtcache || !out || !lens_host) bad = "null pointer";
   else if (impl != SV_ATTN_DECODE_SPLIT && impl != SV_ATTN_DECODE_CLUSTER) bad = "unknown impl";
-  else if (per_row != 0 && per_row != 1) bad = "per_row is 0 or 1";
+  else if (per_row < 0 || per_row > 2) bad = "per_row is 0, 1 or 2";
+  else if (per_row == 2 && (impl != SV_ATTN_DECODE_CLUSTER || window != 0)) bad = "the column map (per_row = 2) is cluster-only with window 0";
   else if (batch < 1 || batch > kSessionRows) bad = "batch not in [1, 16]";
   else if (n_head < 1 || n_kv < 1 || n_head % n_kv || n_head / n_kv > 16) bad = "n_head % n_kv != 0 or group > 16";
   else if (tcap < 32 || tcap % 32) bad = "tcap % 32 != 0";
@@ -2102,7 +2103,8 @@ int sv_op_attention_decode(int32_t impl, int32_t per_row, const void* qkv, const
   else if (window < 0) bad = "window < 0";
   else if (!aligned16(qkv) || !aligned16(kcache) || !aligned16(vtcache)) bad = "qkv and the caches must be 16-byte aligned";
   for (int b = 0; !bad && b < batch; ++b) {
-    if (lens_host[b] < 1 || lens_host[b] > tcap) bad = "a length is not in [1, tcap]";
+    if (per_row == 2) { if (lens_host[b] < 0 || lens_host[b] >= tcap) bad = "a column position is not in [0, tcap - 1]"; }
+    else if (lens_host[b] < 1 || lens_host[b] > tcap) bad = "a length is not in [1, tcap]";
     else if (!per_row && lens_host[b] != lens_host[0]) bad = "per_row = 0 needs equal lengths";
   }
   if (bad) return fail(nullptr, SV_ERR_INVALID, "bad attention_decode arguments: %s", bad);
@@ -2111,26 +2113,33 @@ int sv_op_attention_decode(int32_t impl, int32_t per_row, const void* qkv, const
   const size_t part_floats = impl == SV_ATTN_DECODE_SPLIT ? (size_t)batch * n_kv * nsplit * (32 + 16 * D) : 0;
   GenState gs{};
   RowState rs{};
+  svspec::ColMap cm{};
   gs.cur_len = lens_host[0] - 1;
   for (int b = 0; b < batch; ++b) rs.row_len[b] = lens_host[b] - 1;    // the new token's key sits at lens - 1
+  cm.n_live = batch;                                                   // every column reads cache row 0 (row[c] = 0)
+  for (int b = 0; b < batch; ++b) cm.pos[b] = lens_host[b];
+  static_assert(sizeof(svspec::ColMap) <= kOpState, "the column map fits the scratch header");
   void* buf = nullptr;
   cudaError_t r = cudaMalloc(&buf, kOpState + part_floats * sizeof(float));
   if (r != cudaSuccess) return op_fail("attention_decode alloc", r);
   GenState* d_gs = reinterpret_cast<GenState*>(buf);
   RowState* d_rs = reinterpret_cast<RowState*>(buf);
+  svspec::ColMap* d_cm = reinterpret_cast<svspec::ColMap*>(buf);
   float* partial = reinterpret_cast<float*>(static_cast<char*>(buf) + kOpState);
-  if (per_row) r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
+  if (per_row == 2) r = cudaMemcpyAsync(d_cm, &cm, sizeof(cm), cudaMemcpyHostToDevice, st);
+  else if (per_row) r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
   else r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
   if (r == cudaSuccess) {
     if (impl == SV_ATTN_DECODE_SPLIT) {
       launch_attention_decode((const bf16*)qkv, cols, (const bf16*)kcache, (const bf16*)vtcache, (bf16*)out, partial, d_gs,
-                              batch, n_head, n_kv, D, tcap, nsplit, window, st, per_row ? d_rs : nullptr);
+                              batch, n_head, n_kv, D, tcap, nsplit, window, st, per_row == 1 ? d_rs : nullptr);
       r = cudaGetLastError();
     } else {
       r = attention_decode_cluster_init();
       if (r == cudaSuccess)
         r = launch_attention_decode_cluster((const bf16*)qkv, cols, (const bf16*)kcache, (const bf16*)vtcache, (bf16*)out, d_gs,
-                                            batch, n_head, n_kv, D, tcap, nsplit, window, false, st, per_row ? d_rs : nullptr);
+                                            batch, n_head, n_kv, D, tcap, nsplit, window, false, st, per_row == 1 ? d_rs : nullptr,
+                                            per_row == 2 ? d_cm : nullptr);
     }
   }
   if (r == cudaSuccess) r = cudaStreamSynchronize(st);
@@ -2162,9 +2171,14 @@ int sv_op_gemv_ring(const sv_op_ring* args, void* stream) {
     if (!o.kcache || !o.vtcache || !o.pos_host) bad = "QKV needs kcache, vtcache and pos_host";
     else if (o.n_head < 1 || o.n_kv < 1 || o.n_head % o.n_kv || o.N != (o.n_head + 2 * o.n_kv) * 128) bad = "N != (n_head + 2 n_kv) * 128";
     else if (o.tcap < 32 || o.tcap % 32) bad = "tcap % 32 != 0";
-    else if (o.per_row != 0 && o.per_row != 1) bad = "per_row is 0 or 1";
+    else if (o.per_row < 0 || o.per_row > 2) bad = "per_row is 0, 1 or 2";
+    else if (o.per_row == 2 && (o.B > svspec::kMaxCols || o.pos_host[o.B] < 0 || o.pos_host[o.B] > o.B))
+      bad = "the column map needs 0 <= n_live = pos_host[B] <= B";
     for (int b = 0; !bad && b < (o.per_row ? o.B : 1); ++b)
       if (o.pos_host[b] < 0 || o.pos_host[b] > o.tcap) bad = "a position is not in [0, tcap]";
+    // the map kernel prefetches row 0's keys [0, pos[0] + n_live): svspec::set_map's form keeps that inside the row
+    for (int b = 0; !bad && o.per_row == 2 && b < o.B; ++b)
+      if (o.pos_host[b] >= o.tcap || o.pos_host[0] + o.pos_host[o.B] > o.tcap) bad = "a column position is not in [0, tcap - 1] or pos[0] + n_live > tcap";
   }
   if (bad) return fail(nullptr, SV_ERR_INVALID, "bad gemv_ring arguments: %s", bad);
   cudaStream_t st = (cudaStream_t)stream;
@@ -2175,14 +2189,20 @@ int sv_op_gemv_ring(const sv_op_ring* args, void* stream) {
   if (r != cudaSuccess) return op_fail("gemv_ring alloc", r);
   GenState gs{};
   RowState rs{};
+  svspec::ColMap cm{};
+  const bool map = o.epi == 1 && o.per_row == 2;
   if (o.epi == 1) {
     gs.cur_len = o.pos_host[0];
-    for (int b = 0; o.per_row && b < o.B; ++b) rs.row_len[b] = o.pos_host[b];
+    for (int b = 0; o.per_row == 1 && b < o.B; ++b) rs.row_len[b] = o.pos_host[b];
+    if (map) cm.n_live = o.pos_host[o.B];                              // svspec::set_map's form: every column in row 0
+    for (int b = 0; map && b < o.B; ++b) cm.pos[b] = o.pos_host[b];
   }
   GenState* d_gs = reinterpret_cast<GenState*>(buf);
   RowState* d_rs = reinterpret_cast<RowState*>(buf);
+  svspec::ColMap* d_cm = reinterpret_cast<svspec::ColMap*>(buf);
   uint8_t* wt = static_cast<uint8_t*>(buf) + kOpState;
-  if (o.per_row) r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
+  if (map) r = cudaMemcpyAsync(d_cm, &cm, sizeof(cm), cudaMemcpyHostToDevice, st);
+  else if (o.per_row) r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
   else r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
   if (r == cudaSuccess) r = gemv_ring_init();
   if (r == cudaSuccess) {
@@ -2193,7 +2213,7 @@ int sv_op_gemv_ring(const sv_op_ring* args, void* stream) {
     g.B = o.B; g.N = o.N; g.K = o.K; g.act = o.act; g.epi = o.epi; g.ln_eps = o.ln_eps;
     g.n_head = o.n_head; g.n_kv = o.n_kv; g.tcap = o.tcap; g.state = d_gs;
     g.kcache = (bf16*)o.kcache; g.vtcache = (bf16*)o.vtcache; g.amax_val = o.amax_val; g.amax_idx = o.amax_idx;
-    g.pdl = false; g.rows = (o.epi == 1 && o.per_row) ? d_rs : nullptr;
+    g.pdl = false; g.rows = (o.epi == 1 && o.per_row == 1) ? d_rs : nullptr; g.cmap = map ? d_cm : nullptr;
     launch_gemv_ring(g, st);
     r = cudaGetLastError();
   }
@@ -2352,6 +2372,86 @@ int sv_op_select(const sv_op_select_args* args, void* stream) {
     o.counters_host[0] = gs.step; o.counters_host[1] = gs.cur_len; o.counters_host[2] = gs.done;
     for (int b = 0; b < o.B; ++b) o.unfinished_host[b] = gs.unfinished[b];
   }
+  return SV_OK;
+}
+
+// The selection kernels of a speculative verify step, launched as generate_impl launches them.
+static_assert(sizeof(sv_spec_state) == sizeof(svspec::State) && offsetof(sv_spec_state, tok) == offsetof(svspec::State, tok) &&
+              offsetof(sv_spec_state, ncols) == offsetof(svspec::State, ncols) &&
+              offsetof(sv_spec_state, accepted) == offsetof(svspec::State, accepted),
+              "sv_spec_state mirrors svspec::State");
+int sv_op_spec_select(const sv_op_spec_args* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad spec_select arguments: null descriptor");
+  const sv_op_spec_args& o = *args;
+  const sv_gen_params& p = o.params;
+  const char* bad = nullptr;
+  if (o.impl != SV_SPEC_GREEDY && o.impl != SV_SPEC_SAMPLE && o.impl != SV_SPEC_ACCEPT) bad = "unknown impl";
+  else if (!o.seen || !o.out_ids || !o.next_ids || !o.gen_host || !o.spec_host) bad = "seen, out_ids, next_ids, gen_host and spec_host are required";
+  else if (o.impl != SV_SPEC_ACCEPT && !o.logits) bad = "GREEDY and SAMPLE need logits";
+  else if (o.vocab < 1) bad = "vocab < 1";
+  else if (o.impl == SV_SPEC_SAMPLE && !(p.temperature > 0.f)) bad = "temperature must be > 0";
+  else if (o.impl == SV_SPEC_SAMPLE && !(p.top_p > 0.f && p.top_p <= 1.f)) bad = "top_p not in (0, 1]";
+  else if (!(p.repetition_penalty > 0.f)) bad = "repetition_penalty must be > 0";
+  else if (p.n_stop_ids < 0 || p.n_stop_ids > 8) bad = "n_stop_ids outside [0, 8]";
+  else if (p.max_new_tokens < 1 || p.max_new_tokens > o.out_stride) bad = "max_new_tokens not in [1, out_stride]";
+  else if (o.gen_host[0] < 1 || o.gen_host[0] >= o.out_stride) bad = "step (the history's length) not in [1, out_stride)";
+  else if (o.gen_host[1] < 0 || o.gen_host[1] >= o.n_positions) bad = "cur_len not in [0, n_positions - 1]";
+  else if (!o.wte || !o.x) bad = "wte and x are required";
+  else if (o.h < 8 || o.h % 8) bad = "h % 8 != 0";
+  else if (o.n_positions < 1) bad = "n_positions < 1";
+  else if (!aligned16(o.wte) || !aligned16(o.wpe) || !aligned16(o.x)) bad = "wte, wpe and x must be 16-byte aligned";
+  else if ((o.amax_val != nullptr) != (o.amax_idx != nullptr)) bad = "amax_val and amax_idx go together";
+  else if (o.amax_val && o.impl != SV_SPEC_GREEDY) bad = "the argmax partials are GREEDY's";
+  if (!bad) {
+    const sv_spec_state& q = *o.spec_host;
+    if (q.ncols < 1 || q.ncols > svspec::kMaxCols) bad = "ncols not in [1, 16]";
+    else if (q.n_live < 0 || q.n_live > q.ncols) bad = "n_live not in [0, ncols]";
+    else if (q.k != q.ncols - 1) bad = "k != ncols - 1";
+    else if (q.max_ngram < 1) bad = "max_ngram < 1";
+    for (int c = 0; !bad && c < q.ncols; ++c)
+      if (q.row[c] != 0 || q.pos[c] < 0 || q.pos[c] >= o.n_positions) bad = "a column is not in row 0 at a position in [0, n_positions - 1]";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad spec_select arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const GenParamsDev hp = gen_params_dev(&p, p.stop_row0_only, o.out_stride);
+  GenState gs{};
+  gs.step = o.gen_host[0]; gs.cur_len = o.gen_host[1]; gs.done = o.gen_host[2]; gs.unfinished[0] = o.gen_host[3];
+  svspec::State sp;
+  memcpy(&sp, o.spec_host, sizeof(sp));
+  const int ncols = sp.ncols;
+  const size_t probs_bytes = o.impl == SV_SPEC_SAMPLE ? (size_t)ncols * o.vocab * sizeof(float) : 0;
+  char* buf = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&buf), 3 * kOpState + probs_bytes);
+  if (r != cudaSuccess) return op_fail("spec_select alloc", r);
+  GenState* d_gs = reinterpret_cast<GenState*>(buf);
+  svspec::State* d_sp = reinterpret_cast<svspec::State*>(buf + kOpState);
+  GenParamsDev* d_p = reinterpret_cast<GenParamsDev*>(buf + 2 * kOpState);
+  float* probs = reinterpret_cast<float*>(buf + 3 * kOpState);
+  static_assert(sizeof(svspec::State) <= kOpState, "the speculative state fits a scratch slot");
+  r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_sp, &sp, sizeof(sp), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_p, &hp, sizeof(hp), cudaMemcpyHostToDevice, st);
+  const bf16* lg = (const bf16*)o.logits;
+  uint8_t* seen = (uint8_t*)o.seen;
+  if (r == cudaSuccess) {
+    if (o.impl == SV_SPEC_GREEDY) {
+      launch_select_fused_spec(lg, o.vocab, o.amax_val, o.amax_idx, gemv_ring_ntiles(o.vocab), 8 * ring_row_groups(ncols), d_gs,
+                               d_p, seen, o.next_ids, o.out_ids, (const bf16*)o.wte, (const bf16*)o.wpe, (bf16*)o.x, o.h,
+                               o.n_positions, d_sp, false, st);
+    } else {
+      if (o.impl == SV_SPEC_SAMPLE) launch_select_sample_spec(lg, o.vocab, ncols, d_gs, d_p, seen, probs, d_sp, st);
+      launch_spec_accept(d_gs, d_p, seen, o.next_ids, o.out_ids, o.vocab, (const bf16*)o.wte, (const bf16*)o.wpe, (bf16*)o.x,
+                         o.h, o.n_positions, d_sp, false, st);
+    }
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&gs, d_gs, sizeof(gs), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&sp, d_sp, sizeof(sp), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  if (r != cudaSuccess) return op_fail("spec_select", r);
+  o.gen_host[0] = gs.step; o.gen_host[1] = gs.cur_len; o.gen_host[2] = gs.done; o.gen_host[3] = gs.unfinished[0];
+  memcpy(o.spec_host, &sp, sizeof(sp));
   return SV_OK;
 }
 

@@ -578,11 +578,12 @@ def _i32s(v) -> C.Array:
 
 
 def op_attention_decode(qkv: torch.Tensor, kcache: torch.Tensor, vtcache: torch.Tensor, lens, n_head: int, n_kv: int,
-                        nsplit: int, window: int = 0, impl: int = _lib.SV_ATTN_DECODE_SPLIT, per_row: bool = False) -> torch.Tensor:
+                        nsplit: int, window: int = 0, impl: int = _lib.SV_ATTN_DECODE_SPLIT, per_row: int = 0) -> torch.Tensor:
     """One decode-attention launch over caller-filled caches `kcache [B, n_kv, tcap, 128]`, `vtcache [B, n_kv, 128, tcap]`:
-    row b's query (qkv row b) attends to keys `[0, lens[b])` -> `[B, n_head * 128]`."""
+    row b's query (qkv row b) attends to keys `[0, lens[b])` -> `[B, n_head * 128]`.  `per_row=2` (cluster only): the column
+    map of a verify step, qkv row c attends to keys `[0, lens[c]]` of cache row 0, `B` = qkv's rows."""
     lib = _lib.load()
-    B, tcap = kcache.shape[0], kcache.shape[2]
+    B, tcap = (qkv.shape[0] if int(per_row) == 2 else kcache.shape[0]), kcache.shape[2]
     out = torch.empty(B, n_head * 128, dtype=torch.bfloat16, device=qkv.device)
     _lib.check(lib, lib.sv_op_attention_decode(impl, int(per_row), _p(qkv), _p(kcache), _p(vtcache), _p(out), _i32s(lens), B,
                                                n_head, n_kv, tcap, nsplit, window, _stream_ptr(qkv.device)))
@@ -592,9 +593,11 @@ def op_attention_decode(qkv: torch.Tensor, kcache: torch.Tensor, vtcache: torch.
 def op_gemv_ring(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
                  ln: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, act: int = 0, epi: int = 0, tiled: bool = False,
                  ln_eps: float = 1e-5, y: Optional[torch.Tensor] = None, kcache: Optional[torch.Tensor] = None,
-                 vtcache: Optional[torch.Tensor] = None, n_head: int = 0, n_kv: int = 0, pos=None, per_row: bool = False):
+                 vtcache: Optional[torch.Tensor] = None, n_head: int = 0, n_kv: int = 0, pos=None, per_row: int = 0,
+                 n_live: int = 0):
     """One weight-ring GEMV launch (the decode step's): `y [B, N]`; with `epi=2` also the argmax partials
-    `(amax_val, amax_idx)`, `[ntiles, row_stride]`.  `y` may be `residual` (in place)."""
+    `(amax_val, amax_idx)`, `[ntiles, row_stride]`.  `y` may be `residual` (in place).  `epi=1, per_row=2`: the column map of
+    a verify step, column c's K/V appended in cache row 0 at `pos[c]` for `c < n_live` (passed as `pos_host[B]`)."""
     lib = _lib.load()
     B, K = x.shape
     N = w.shape[0]
@@ -611,7 +614,7 @@ def op_gemv_ring(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] 
     if kcache is not None:
         a.kcache, a.vtcache, a.tcap = kcache.data_ptr(), vtcache.data_ptr(), kcache.shape[2]
     if pos is not None:
-        posv = _i32s(pos)
+        posv = _i32s(list(pos) + ([n_live] if int(per_row) == 2 else []))
         a.pos_host = C.cast(posv, C.POINTER(C.c_int32))
     amax = None
     if epi == 2:
@@ -688,6 +691,30 @@ def op_select(impl: int, logits: torch.Tensor, params: GenerationParams, seen: t
     else:
         state["step"], state["cur_len"], state["done"] = (int(v) for v in counters)
         state["unfinished"] = list(unfinished)[:B]
+    return state
+
+
+def op_spec_select(impl: int, params: GenerationParams, seen: torch.Tensor, out_ids: torch.Tensor, next_ids: torch.Tensor,
+                   state: dict, spec: "_lib.SpecState", wte: torch.Tensor, wpe: Optional[torch.Tensor], x: torch.Tensor,
+                   n_positions: int, logits: Optional[torch.Tensor] = None,
+                   amax: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> dict:
+    """One speculative verify step's selection (see sv_op_spec_select) on one image row: bf16 `logits [ncols, vocab]`
+    (GREEDY, SAMPLE); `seen` uint8 `[vocab]`, `out_ids` int32 `[out_stride]` (the history), `next_ids` int32 `[1]` and
+    `x [ncols, h]` are updated in place, as are `spec` (a `_lib.SpecState`) and `state`: `step, cur_len, done, unfinished`."""
+    lib = _lib.load()
+    vocab = wte.shape[0]
+    gen = _i32s([state["step"], state["cur_len"], state["done"], state["unfinished"]])
+    a = _lib.OpSpec(impl=impl, vocab=vocab, params=params.to_c(), seen=seen.data_ptr(), out_ids=out_ids.data_ptr(),
+                    next_ids=next_ids.data_ptr(), out_stride=out_ids.shape[-1], gen_host=C.cast(gen, C.POINTER(C.c_int32)),
+                    spec_host=C.pointer(spec), wte=wte.data_ptr(), x=x.data_ptr(), h=wte.shape[1], n_positions=n_positions)
+    if logits is not None:
+        a.logits = logits.data_ptr()
+    if wpe is not None:
+        a.wpe = wpe.data_ptr()
+    if amax is not None:
+        a.amax_val, a.amax_idx = amax[0].data_ptr(), amax[1].data_ptr()
+    _lib.check(lib, lib.sv_op_spec_select(C.byref(a), _stream_ptr(seen.device)))
+    state["step"], state["cur_len"], state["done"], state["unfinished"] = (int(v) for v in gen)
     return state
 
 

@@ -226,6 +226,103 @@ def test_decode_attention_batches(B, impl):
     _calib(f"attention_decode impl={impl} B={B}", c.worst)
 
 
+class MapAttnCase:
+    """The column map of a speculative verify step: ncols query columns over ONE cache row holding L0 prefix keys plus the
+    live columns' own keys; column c attends to keys [0, pos[c]].  The slot of each column and the slot right after it
+    (pos[c] + 1, the next column's key) hold a probe aimed at one head of that column (score ~11 against N(0, 1) for the
+    other keys), so a column that reads one key too many or too few is far outside the tolerance.  Cache rows 1..15, which
+    no column may read, hold other keys."""
+
+    ROWS = 16
+
+    def __init__(self, nh, nkv, ncols, n_live, L0, tcap, seed):
+        self.nh, self.nkv, self.ncols, self.tcap = nh, nkv, ncols, tcap
+        self.pos = _map_positions(ncols, n_live, L0)
+        g = torch.Generator(device=DEV).manual_seed(seed)
+        grp = nh // nkv
+        f64 = dict(device=DEV, dtype=torch.float64)
+        q = torch.randn(ncols, nkv, grp, D, generator=g, **f64)
+        u = q / q.norm(dim=-1, keepdim=True)                            # column c, head h's direction
+        K = torch.randn(self.ROWS, nkv, tcap, D, generator=g, **f64)
+        V = torch.randn(self.ROWS, nkv, tcap, D, generator=g, **f64)
+        aimed = {}                                                      # (kv head, slot) -> the directions aimed at it
+        for c, p in enumerate(self.pos):
+            for kvh in range(nkv):
+                for slot in (p, p + 1):
+                    if slot < tcap:
+                        aimed.setdefault((kvh, slot), []).append(u[c, kvh, (c + kvh) % grp])
+        for (kvh, slot), dirs in aimed.items():
+            K[0, kvh, slot] = sum(dirs) * PROBE_SCORE
+            V[0, kvh, slot] = 4.0 * torch.randn(D, generator=g, **f64)
+        self.q = (u * math.sqrt(D)).reshape(ncols, nh, D).to(torch.bfloat16)
+        self.qkv = torch.randn(ncols, (nh + 2 * nkv) * D, generator=g, device=DEV).to(torch.bfloat16)
+        self.qkv[:, :nh * D] = self.q.reshape(ncols, nh * D)
+        Kb, Vb = K.to(torch.bfloat16), V.to(torch.bfloat16)
+        self.kc, self.vc = Kb.contiguous(), Vb.transpose(2, 3).contiguous()
+        qd, Kd, Vd = self.q.double(), Kb.double(), Vb.double()
+        self.ref = torch.empty(ncols, nh, D, **f64)
+        for c, p in enumerate(self.pos):
+            for kvh in range(nkv):
+                hs = slice(kvh * grp, (kvh + 1) * grp)
+                w = torch.softmax(qd[c, hs] @ Kd[0, kvh, :p + 1].T / math.sqrt(D), dim=-1)
+                self.ref[c, hs] = w @ Vd[0, kvh, :p + 1]
+        self.rms = self.ref.pow(2).mean(-1, keepdim=True).sqrt()
+
+    def run(self, ncta, kc=None, vc=None):
+        return E.op_attention_decode(self.qkv, self.kc if kc is None else kc, self.vc if vc is None else vc, self.pos, self.nh,
+                                     self.nkv, ncta, 0, CLUSTER, 2)
+
+    def poisoned(self, after):
+        """Caches whose row-0 slots > after and whose other rows hold other finite values."""
+        kc, vc = self.kc.clone(), self.vc.clone()
+        kc[0, :, after + 1:] = 2.0
+        vc[0, :, :, after + 1:] = 300.0
+        kc[1:] = -3.0 * kc[1:]
+        vc[1:] = 500.0
+        return kc, vc
+
+
+def _map_l0s(ncta, tcap):
+    """31/32/33, the first and last key of each CTA's 32-key block range at ~1100 keys with this cluster size, tcap - 16."""
+    edges = {31, 32, 33, tcap - 16}
+    for a, z in _ranges(1100, 0, ncta)[:3]:
+        edges.update({a, z, z + 1})
+    return sorted(edges)
+
+
+@pytest.mark.parametrize("ncta", [1, 2, 3, 4, 5, 6, 7, 8])
+def test_decode_attention_column_map(ncta):
+    """attention_decode_cluster_map_kernel against fp64, and bitwise against the plain cluster kernel at each column's
+    length with the same cluster size (the verify step's bit-identity with plain decoding).  Columns at L0 + c, inert ones
+    at the last live position; 8-CTA clusters over short rows (the engine sizes the cluster from prefix + max_new)."""
+    tcap = 2080
+    worst = 0.0
+    cases = [(16, 1, 16, 16), (4, 2, 9, 5)]
+    for i, L0 in enumerate(_map_l0s(ncta, tcap)):
+        nh, nkv, ncols, n_live = cases[i % len(cases)]
+        if i % 3 == 2:
+            n_live = 1
+        c = MapAttnCase(nh, nkv, ncols, n_live, L0, tcap, seed=ncta * 1000 + L0)
+        out = c.run(ncta)
+        assert bool(torch.isfinite(out.float()).all())
+        o = out.view(ncols, nh, D).double()
+        tol = ATTN_ULPS * _ulp(c.ref) + ATTN_C * c.rms
+        ratio = ((o - c.ref).abs() / tol).max().item()
+        worst = max(worst, ratio)
+        assert ratio <= 1.0, (L0, ncols, n_live, ratio, ((o - c.ref).abs() > tol).nonzero()[:5].tolist())
+        assert torch.equal(out, c.run(ncta)), "repeated launches differ"
+        for col, p in enumerate(c.pos):
+            one = E.op_attention_decode(c.qkv[col:col + 1], c.kc[:1], c.vc[:1], [p + 1], nh, nkv, ncta, 0, CLUSTER, 0)
+            assert torch.equal(one[0], out[col]), (L0, col, p)
+        for p in sorted(set(c.pos)):
+            kc, vc = c.poisoned(p)
+            alt = c.run(ncta, kc, vc)
+            for col, pc in enumerate(c.pos):
+                if pc <= p:
+                    assert torch.equal(alt[col], out[col]), f"column {col} (pos {pc}) reads a slot > {p} or another row"
+    _calib(f"attention_decode column map ncta={ncta}", worst)
+
+
 # ---- RoPE ----------------------------------------------------------------------------------------------------------------
 def _hf_rope_table(theta, max_pos, d=128):
     """cos / sin [max_pos, d / 2] as transformers' Starcoder2RotaryEmbedding returns them in bf16, with the oracle's config."""
@@ -490,19 +587,54 @@ def test_gemv_ring_constant_row_gives_ln_bias():
     assert torch.equal(y, plain)
 
 
-@pytest.mark.parametrize("per_row", [0, 1], ids=["plain", "rows"])
-@pytest.mark.parametrize("B", [3, 13])
+def _map_positions(ncols, n_live, cur):
+    """svspec::set_map: live column c at cur + c, inert columns at the last live position (cur - 1 when n_live = 0)."""
+    return [cur + c if c < n_live else cur + n_live - 1 for c in range(ncols)]
+
+
+@pytest.mark.parametrize("per_row", [0, 1, 2], ids=["plain", "rows", "map"])
+@pytest.mark.parametrize("B", [1, 2, 3, 8, 9, 13, 16])
 @pytest.mark.parametrize("nh,nkv", [(16, 1), (4, 2)])
 def test_gemv_ring_qkv_appends_kv(nh, nkv, B, per_row):
-    """The QKV epilogue changes the caches only at (row, kv head, pos), with y's K / V columns; pos == tcap writes nothing."""
+    """The QKV epilogue changes the caches only at (row, kv head, pos), with y's K / V columns; pos == tcap writes nothing.
+    The column map of a verify step (per_row = 2, B columns of cache row 0): live columns append at their positions, which
+    straddle a 32-slot edge or end at tcap - 1; inert columns write nothing, not even at the last live position they point
+    to (cur - 1 with no live column, a slot holding data); y is bitwise the plain QKV launch's; the other cache rows keep
+    every byte.  Row-major and slab-tiled weights."""
     K, tcap = 2048, 128
     N = (nh + 2 * nkv) * D
     g = torch.Generator(device=DEV).manual_seed(B * 10 + per_row)
     w, b = _weights(N, K, g)
     ln = _ln_params(K, g)
     x = _ln_rows(B, K, g)
+    ref, scale, _ = _ring_ref(x, w, b, None, ln)
+    if per_row == 2:
+        bf = dict(dtype=torch.bfloat16, device=DEV)
+        for n_live in sorted({0, 1, B - 1, B}):
+            for cur in (96 - n_live // 2, tcap - n_live) if n_live else (96, tcap):
+                pos = _map_positions(B, n_live, cur)
+                for tiled in (False, True):
+                    kc = torch.randn(3, nkv, tcap, D, generator=g, device=DEV).to(torch.bfloat16)
+                    vc = torch.randn(3, nkv, D, tcap, generator=g, device=DEV).to(torch.bfloat16)
+                    k0, v0 = kc.clone(), vc.clone()
+                    y = E.op_gemv_ring(x, w, b, None, ln, epi=1, kcache=kc, vtcache=vc, n_head=nh, n_kv=nkv, pos=pos,
+                                       per_row=2, n_live=n_live, tiled=tiled)
+                    # the plain launch on the same inputs (B cache rows, as it reads them; pos = tcap: it writes nothing)
+                    plain = E.op_gemv_ring(x, w, b, None, ln, epi=1, kcache=torch.zeros(B, nkv, tcap, D, **bf),
+                                           vtcache=torch.zeros(B, nkv, D, tcap, **bf), n_head=nh, n_kv=nkv, pos=[tcap],
+                                           tiled=tiled)
+                    assert torch.equal(y, plain), (n_live, cur, tiled)
+                    kexp, vexp = k0.clone(), v0.clone()
+                    ky = y[:, nh * D:(nh + nkv) * D].view(B, nkv, D)
+                    vy = y[:, (nh + nkv) * D:].view(B, nkv, D)
+                    for c in range(n_live):
+                        kexp[0, :, pos[c]] = ky[c]
+                        vexp[0, :, :, pos[c]] = vy[c]
+                    assert torch.equal(kc, kexp) and torch.equal(vc, vexp), (n_live, cur, tiled)
+        _ring_check(y, ref, scale, f"qkv {nh}/{nkv} B={B} per_row=map")
+        return
     pos_sets = [[(7 * r + 3) % tcap for r in range(B)], [tcap] * B] if per_row else [[77] * B, [tcap] * B]
-    if per_row:
+    if per_row and B > 1:
         pos_sets[0][1] = tcap                       # one row past the cache: nothing written for it
     for pos in pos_sets:
         kc = torch.randn(B, nkv, tcap, D, generator=g, device=DEV).to(torch.bfloat16)
@@ -510,7 +642,6 @@ def test_gemv_ring_qkv_appends_kv(nh, nkv, B, per_row):
         k0, v0 = kc.clone(), vc.clone()
         y = E.op_gemv_ring(x, w, b, None, ln, epi=1, kcache=kc, vtcache=vc, n_head=nh, n_kv=nkv, pos=pos,
                            per_row=bool(per_row))
-        ref, scale, _ = _ring_ref(x, w, b, None, ln)
         _ring_check(y, ref, scale, f"qkv {nh}/{nkv} B={B} per_row={per_row}")
         kexp, vexp = k0.clone(), v0.clone()
         ky = y[:, nh * D:(nh + nkv) * D].view(B, nkv, D)

@@ -79,7 +79,9 @@ def _bad_decode_attention(**kw):
 @pytest.mark.parametrize("kw", [dict(n_head=6, n_kv=4), dict(n_head=17, n_kv=1), dict(tcap=48), dict(lens=[0]),
                                 dict(lens=[65]), dict(lens=[5, 6]), dict(lens=[1] * 17, per_row=1), dict(nsplit=0),
                                 dict(nsplit=129), dict(impl=1, nsplit=9), dict(impl=2), dict(window=-1), dict(ptr=0x10008),
-                                dict(ptr=0)], ids=str)
+                                dict(ptr=0), dict(per_row=3), dict(per_row=2), dict(per_row=2, impl=1, window=4),
+                                dict(per_row=2, impl=1, lens=[64]), dict(per_row=2, impl=1, lens=[3, -1]),
+                                dict(per_row=2, impl=1, lens=[0] * 17)], ids=str)
 def test_decode_attention_op_rejects_on_the_host(kw):
     """Checked before any CUDA call: these return SV_ERR_INVALID on a machine without a GPU too."""
     assert _bad_decode_attention(**kw) == _lib.SV_ERR_INVALID
@@ -91,12 +93,18 @@ def test_decode_attention_op_rejects_on_the_host(kw):
                                 dict(ln=True, K=4608, B=9), dict(ln=True, K=640, B=9), dict(ln=True, K=4608, epi=1),
                                 dict(ln=True, epi=2, amax=False), dict(ln=True, epi=1, N=2304, tcap=40),
                                 dict(ln=True, epi=1, N=2300), dict(ln=True, epi=1, N=2304, pos=[65]),
-                                dict(ln=True, epi=1, N=2304, pos=[3, -1], per_row=1, B=2), dict(act=4), dict(epi=3)], ids=str)
+                                dict(ln=True, epi=1, N=2304, pos=[3, -1], per_row=1, B=2), dict(act=4), dict(epi=3),
+                                dict(ln=True, epi=1, N=2304, per_row=3), dict(ln=True, epi=1, N=2304, per_row=2, n_live=-1),
+                                dict(ln=True, epi=1, N=2304, pos=[3, 4], per_row=2, B=2, n_live=3),
+                                dict(ln=True, epi=1, N=2304, pos=[3, 65], per_row=2, B=2, n_live=1),
+                                dict(ln=True, epi=1, N=2304, pos=[64], per_row=2, n_live=0),
+                                dict(ln=True, epi=1, N=2304, pos=[63, 63], per_row=2, B=2, n_live=2)], ids=str)
 def test_gemv_ring_op_rejects_on_the_host(kw):
     """Among them the LayerNorm GEMV over K > 2048 with more than 8 rows, which has no ring kernel (the launcher would abort)."""
-    a = dict(B=1, N=2304, K=2048, ln=False, epi=0, act=0, tcap=64, pos=[3], per_row=0, amax=True)
+    a = dict(B=1, N=2304, K=2048, ln=False, epi=0, act=0, tcap=64, pos=[3], per_row=0, amax=True, n_live=1)
     a.update(kw)
-    pos = (C.c_int32 * len(a["pos"]))(*a["pos"])
+    posl = a["pos"] + ([a["n_live"]] if a["per_row"] == 2 else [])      # the column map's n_live follows the positions
+    pos = (C.c_int32 * len(posl))(*posl)
     o = _lib.OpRing(x=a.get("x", 0x10000), w=a.get("w", 0x20000), y=0x30000, B=a["B"], N=a["N"], K=a["K"], act=a["act"],
                     epi=a["epi"], n_head=16, n_kv=1, tcap=a["tcap"], per_row=a["per_row"], kcache=0x40000, vtcache=0x50000,
                     pos_host=C.cast(pos, C.POINTER(C.c_int32)))
@@ -321,6 +329,67 @@ def _bad_select(**kw):
 def test_select_op_rejects_on_the_host(kw):
     assert _bad_select(**kw) == _lib.SV_ERR_INVALID
     assert b"bad select arguments" in _lib.load().sv_last_error(None)
+
+
+def test_spec_select_op_symbol_and_descriptor_layout():
+    assert _lib.ABI_VERSION == 7
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    assert "sv_op_spec_select" in _header_symbols() and "sv_op_spec_select" in _lib.SIGNATURES and "sv_op_spec_select" in exported
+    # sv_spec_state = svspec::State: n_live, row[16], pos[16], tok[16], sel[16], ncols, k, max_ngram, steps, drafted, accepted
+    s = _lib.SpecState
+    assert C.sizeof(s) == 71 * 4
+    assert (s.row.offset, s.pos.offset, s.tok.offset, s.sel.offset, s.ncols.offset, s.max_ngram.offset, s.accepted.offset) == (
+        4, 68, 132, 196, 260, 268, 280)
+    # sv_op_spec_args: int32 (+4), pointer, int32 (+4), sv_gen_params (88), 3 pointers, int32 (+4), 8 pointers, 2 int32
+    o = _lib.OpSpec
+    assert C.sizeof(o) == 208
+    assert (o.logits.offset, o.vocab.offset, o.params.offset, o.seen.offset, o.out_stride.offset, o.gen_host.offset,
+            o.spec_host.offset, o.amax_val.offset, o.wte.offset, o.x.offset, o.h.offset, o.n_positions.offset) == (
+        8, 16, 24, 112, 136, 144, 152, 160, 176, 192, 200, 204)
+
+
+def _bad_spec(**kw):
+    a = dict(impl=0, vocab=500, out_stride=64, max_new=32, step=5, cur_len=40, done=0, logits=0x10000, seen=0x20000,
+             out_ids=0x30000, next_ids=0x40000, temperature=1.0, top_p=1.0, rp=1.0, stop=0, h=64, n_positions=128,
+             wte=0x50000, wpe=0x60000, x=0x70000, amax=None, gen=True, spec=True, ncols=4, n_live=2, k=None, max_ngram=2,
+             pos=None, row=None)
+    a.update(kw)
+    st = _lib.SpecState(n_live=a["n_live"], ncols=a["ncols"], k=a["ncols"] - 1 if a["k"] is None else a["k"],
+                        max_ngram=a["max_ngram"])
+    for c in range(16):
+        st.pos[c] = a["cur_len"] + min(c, 1) if a["pos"] is None else a["pos"]
+        st.row[c] = 0 if a["row"] is None else a["row"]
+    gen = (C.c_int32 * 4)(a["step"], a["cur_len"], a["done"], 1)
+    o = _lib.OpSpec(impl=a["impl"], logits=a["logits"], vocab=a["vocab"], seen=a["seen"], out_ids=a["out_ids"],
+                    next_ids=a["next_ids"], out_stride=a["out_stride"], wte=a["wte"], wpe=a["wpe"], x=a["x"], h=a["h"],
+                    n_positions=a["n_positions"])
+    if a["gen"]:
+        o.gen_host = C.cast(gen, C.POINTER(C.c_int32))
+    if a["spec"]:
+        o.spec_host = C.pointer(st)
+    p = o.params
+    p.max_new_tokens, p.temperature, p.top_p, p.repetition_penalty = a["max_new"], a["temperature"], a["top_p"], a["rp"]
+    p.eos_token_id, p.n_stop_ids = 0, a["stop"]
+    if a["amax"] is not None:
+        o.amax_val, o.amax_idx = a["amax"]
+    return _lib.load().sv_op_spec_select(C.byref(o), None)
+
+
+@pytest.mark.parametrize("kw", [dict(impl=3), dict(impl=-1), dict(seen=0), dict(out_ids=0), dict(next_ids=0), dict(gen=False),
+                                dict(spec=False), dict(logits=0), dict(impl=1, logits=0), dict(vocab=0),
+                                dict(impl=1, temperature=0.0), dict(impl=1, temperature=float("nan")), dict(impl=1, top_p=0.0),
+                                dict(impl=1, top_p=1.5), dict(rp=0.0), dict(stop=9), dict(stop=-1), dict(max_new=0),
+                                dict(max_new=65), dict(step=0), dict(step=64), dict(cur_len=-1), dict(cur_len=128, pos=3),
+                                dict(wte=0), dict(x=0), dict(h=60), dict(h=0), dict(n_positions=0), dict(wpe=0x60008),
+                                dict(x=0x70004), dict(amax=(0x80000, 0)), dict(amax=(0, 0x90000)),
+                                dict(impl=1, amax=(0x80000, 0x90000)), dict(impl=2, amax=(0x80000, 0x90000)), dict(ncols=0),
+                                dict(ncols=17, k=16), dict(n_live=-1), dict(n_live=5), dict(k=2), dict(ncols=1, k=1),
+                                dict(max_ngram=0), dict(pos=-1), dict(pos=128), dict(row=1)], ids=str)
+def test_spec_select_op_rejects_on_the_host(kw):
+    """Checked before any CUDA call: these return SV_ERR_INVALID on a machine without a GPU too."""
+    assert _bad_spec(**kw) == _lib.SV_ERR_INVALID
+    assert b"bad spec_select arguments" in _lib.load().sv_last_error(None)
 
 
 @pytest.mark.parametrize("kw", [dict(num_beams=1), dict(num_beams=9), dict(batch=9), dict(max_new_tokens=0), dict(n_stop_ids=9),

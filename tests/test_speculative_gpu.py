@@ -10,6 +10,8 @@ from starvector_b200.engine import Engine, GenerationParams
 from starvector_b200.modeling import StarVectorForCausalLM
 from starvector_b200.weights import synthetic_images, synthetic_state_dict
 
+from test_speculative_logic import draft
+
 pytestmark = pytest.mark.gpu
 PROMPT = [44, 78]
 
@@ -38,10 +40,29 @@ def _run(eng, img, n_new, on_tokens=None, **kw):
     return out
 
 
+def simulate_schedule(toks, k, g, eos, max_new):
+    """The verify steps a speculative run of these (plain) tokens takes: each step drafts from the history with the host
+    rule (sv_spec_draft_host), then emits one token plus the drafts that match the tokens, cut at the finish (the end of
+    `toks`).  -> the counters sv_last_spec_stats reports."""
+    n, m = len(toks), 1
+    steps = drafted = accepted = 0
+    while m < n:
+        d = draft(toks[:m], k, g, -1 if eos is None else eos, max_new - m - 1)
+        a = 0
+        while a < len(d) and m + a + 1 < n and toks[m + a] == d[a]:
+            a += 1
+        steps, drafted, accepted, m = steps + 1, drafted + len(d), accepted + a, m + 1 + a
+    return dict(steps=steps, drafted=drafted, accepted=accepted)
+
+
 def _pair(eng, img, n_new, k, **kw):
     plain = _run(eng, img, n_new, **kw)
     spec = _run(eng, img, n_new, prompt_lookup_num_tokens=k, **kw)
-    return plain, spec, eng.last_spec_stats()
+    st = eng.last_spec_stats()
+    if plain.shape[0] == 1:     # the device drafts are the host rule's: the schedule of the plain tokens
+        want = simulate_schedule(plain[0].tolist(), k, kw.get("max_matching_ngram_size", 2), kw.get("eos_token_id"), n_new)
+        assert {key: st[key] for key in want} == want, (st, want)
+    return plain, spec, st
 
 
 def _late_first(seq, width):
@@ -247,5 +268,24 @@ def test_1b_speculative_equals_plain(sd_1b, max_batch, k):
         eng.prefill(torch.tensor([PROMPT]))
         for c, t in enumerate(ids):
             assert torch.equal(cols[c], eng.decode_step(torch.tensor([t]))[0].cpu()), c
+    finally:
+        eng.close()
+
+
+def test_1b_long_history_eight_cta_clusters():
+    """1B widths with 2 layers, 4096 cache slots and a prefix + max_new > 2048: 8-CTA cluster attention, drafts searched
+    over histories past both 1024-token strides, k = 15 on a 16-row engine; greedy with a repetition penalty and nucleus
+    sampling.  Speculative = plain, and the counters = the host schedule of the plain tokens."""
+    d = dims_1b(max_batch=16, max_len=4096)
+    d.n_layer = 2
+    eng = _engine(d, synthetic_state_dict(d, seed=0, init="randomized"))
+    try:
+        img = synthetic_images(d, 1, seed=2)
+        n_new = 2300
+        assert 2048 < d.query_length + len(PROMPT) + n_new <= d.max_len
+        for kw in (dict(repetition_penalty=1.3), dict(do_sample=True, temperature=0.9, top_p=0.9, seed=7)):
+            plain, spec, st = _pair(eng, img, n_new, 15, **kw)
+            assert torch.equal(plain, spec), kw
+            print(f"1b long history {kw}: {plain.shape[1]} tokens, stats {st}")
     finally:
         eng.close()
