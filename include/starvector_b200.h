@@ -443,6 +443,73 @@ SV_API int sv_op_beam_candidates(const void* logits, int32_t vocab, const sv_bea
                                  const float* running_scores_host, const int32_t* run_seq, int32_t seq_stride,
                                  float* cand_key, float* cand_val, int32_t* cand_tok, void* stream);
 
+/* The beam-search bookkeeping and KV-cache movement kernels one launch at a time (what follows beam_candidates_kernel in
+ * sv_beam_search, and the cache copies of sv_reorder_cache, sv_expand_batch and sv_session_admit).  Same conventions as
+ * sv_op_select: the caller owns the device tensors, host-side state travels as host structs read on entry and written
+ * back, every argument is checked on the host (SV_ERR_INVALID before any launch), synchronous on `stream`. */
+/* The device state of one beam search (svbeam::State, sv_beam_core.h), field for field; the same bytes as the state blob
+ * of sv_beam_state_init_host / sv_beam_step_host.  Rows r = b * num_beams + j. */
+typedef struct sv_beam_state {
+  int32_t cur_len, done, parity, pad_;   /* generated tokens per running beam, search over, live half of the sequence arrays */
+  float running_scores[16], beam_scores[16];
+  int32_t is_finished[16], fin_len[16];
+  int32_t unsatisfied[16];               /* per image */
+  int32_t div[16][16];                   /* first cache position at which rows r and q (same image) differ */
+} sv_beam_state;
+/* What one step decided (svbeam::Plan): new running row r = old row run_parent[r] + run_tok[r]; finished slot r = old
+ * finished row fin_old[r] (>= 0) or old running row fin_parent[r] + fin_tok[r]; KV row r <- row copy_src[r] (-1: none)
+ * over cache positions [copy_lo[r], copy_hi]; cont: the search goes on; old_len: cur_len before the step. */
+typedef struct sv_beam_plan {
+  int32_t run_parent[16], run_tok[16], fin_old[16], fin_parent[16], fin_tok[16], copy_src[16], copy_lo[16];
+  int32_t copy_hi, cont, old_len;
+} sv_beam_plan;
+typedef struct sv_op_beam_step_args {
+  const sv_beam_params* params;  /* checked as sv_beam_params_check_rows(params, batch, 16) */
+  int32_t batch, vocab, seq_stride;
+  int32_t advance;               /* 0: the first step (candidates of the prefill logits), 1: a decode step; cache_hi =
+                                    cur_len - 1 + advance, and cur_len += advance when the search goes on */
+  sv_beam_state* state_host;     /* in/out; 0 <= cur_len < seq_stride, parity 0 or 1, fin_len in [0, seq_stride] */
+  const float *cand_key, *cand_val;   /* device [R][2 * num_beams], R = batch * num_beams: each row's candidates best-first, */
+  const int32_t* cand_tok;            /*   as beam_candidates_kernel writes them */
+  int32_t *run_seq, *fin_seq;    /* device [2][R][seq_stride]: the double-buffered sequences, updated */
+  int32_t* gen_host;             /* [2]: cur_len (the position of the token fed next, >= 0), done; in/out */
+  const void *wte, *wpe;         /* bf16 [vocab][h], [n_positions][h]; wpe may be NULL (RoPE models) */
+  void* x;                       /* bf16 [R][h]: the next tokens' embeddings at position min(cur_len, n_positions - 1) */
+  int32_t h, n_positions;        /* h % 8 == 0 */
+  int32_t* next_ids;             /* device [R] */
+  sv_beam_plan* plan_host;       /* in/out: the device plan starts as this and is read back (rows >= R are not defined
+                                    after a step that ran) */
+} sv_op_beam_step_args;
+SV_API int sv_op_beam_step(const sv_op_beam_step_args* args, void* stream);
+/* Both phases of the KV suffix copies (parent rows -> a staging cache this call allocates -> child rows) over caches
+ * kcache [n_layer][>= rows][n_kv][tcap][D] and vtcache [n_layer][>= rows][n_kv][D][tcap] (D = 128), layer_stride elements
+ * apart, following *plan_host for rows [0, rows).  copy_src in [-1, rows), copy_hi < tcap, copy_lo >= 0, tcap % 32 == 0,
+ * caches 16-byte aligned. */
+SV_API int sv_op_beam_kv_copy(void* kcache, void* vtcache, int64_t layer_stride, int32_t n_layer, int32_t rows,
+                              int32_t n_kv, int32_t tcap, const sv_beam_plan* plan_host, void* stream);
+/* One layer's cache-row gather (sv_reorder_cache, sv_expand_batch, the n-completions copy of sv_session_admit): row r of
+ * kdst / vdst takes K positions [0, len) and V^T positions [0, round_up(len, 8)) of source row idx[r] (idx: device int32
+ * [rows] with entries in the source's rows, or NULL: r).  Layouts as sv_op_attention_decode; 1 <= len <= tcap,
+ * tcap % 32 == 0, rows <= 16. */
+SV_API int sv_op_kv_gather(const void* ksrc, const void* vsrc, void* kdst, void* vdst, const int32_t* idx, int32_t rows,
+                           int32_t n_kv, int32_t tcap, int32_t len, void* stream);
+/* Admission of k session slots in one launch: slot slot_host[j] gets seen[slot] cleared, out_ids[slot] filled with pad_id
+ * and its RowState fields row_len = len_host[j], row_step = 0, row_active = 1, row_max_new = max_new_host[j], row_seed =
+ * seed_host[j].  The RowState travels as the host arrays [S] (and event [1]), read on entry and written back. */
+typedef struct sv_op_admit_args {
+  int32_t k, S;                  /* 1 <= k <= S <= 16 */
+  const int32_t *slot_host, *len_host, *max_new_host;   /* [k]: distinct slots in [0, S), len >= 0 */
+  const uint64_t* seed_host;     /* [k] */
+  void* seen;                    /* uint8 [S][vocab] (device) */
+  int32_t vocab;
+  int32_t* out_ids;              /* [S][out_stride] (device) */
+  int32_t out_stride, pad_id;
+  int32_t *row_len_host, *row_step_host, *row_active_host, *row_max_new_host;   /* [S] each */
+  uint64_t* row_seed_host;       /* [S] */
+  int32_t* event_host;           /* [1] */
+} sv_op_admit_args;
+SV_API int sv_op_session_admit(const sv_op_admit_args* args, void* stream);
+
 /* The image-encoder, adapter and prefill kernels one launch at a time (the half of a request before the first decode
  * step).  The caller owns the device tensors; every argument is checked on the host: SV_ERR_INVALID before any launch.
  * Synchronous on `stream`.  sv_op_layernorm, sv_op_linear and sv_op_attention_vit above are the rest of that half. */

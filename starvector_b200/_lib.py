@@ -99,6 +99,34 @@ class OpSpec(C.Structure):   # sv_op_spec_args
                 ("x", C.c_void_p), ("h", C.c_int32), ("n_positions", C.c_int32)]
 
 
+class BeamState(C.Structure):   # sv_beam_state (svbeam::State): also the state blob of sv_beam_state_init_host / _step_host
+    _fields_ = [(n, C.c_int32) for n in ("cur_len", "done", "parity", "pad_")] + [
+        ("running_scores", C.c_float * 16), ("beam_scores", C.c_float * 16), ("is_finished", C.c_int32 * 16),
+        ("fin_len", C.c_int32 * 16), ("unsatisfied", C.c_int32 * 16), ("div", (C.c_int32 * 16) * 16)]
+
+
+class BeamPlan(C.Structure):   # sv_beam_plan (svbeam::Plan)
+    _fields_ = [(n, C.c_int32 * 16) for n in ("run_parent", "run_tok", "fin_old", "fin_parent", "fin_tok", "copy_src",
+                                              "copy_lo")] + [(n, C.c_int32) for n in ("copy_hi", "cont", "old_len")]
+
+
+class OpBeamStep(C.Structure):   # sv_op_beam_step_args
+    _fields_ = [("params", C.POINTER(BeamParams))] + [(n, C.c_int32) for n in ("batch", "vocab", "seq_stride", "advance")] + [
+        ("state_host", C.POINTER(BeamState)), ("cand_key", C.c_void_p), ("cand_val", C.c_void_p), ("cand_tok", C.c_void_p),
+        ("run_seq", C.c_void_p), ("fin_seq", C.c_void_p), ("gen_host", C.POINTER(C.c_int32)), ("wte", C.c_void_p),
+        ("wpe", C.c_void_p), ("x", C.c_void_p), ("h", C.c_int32), ("n_positions", C.c_int32), ("next_ids", C.c_void_p),
+        ("plan_host", C.POINTER(BeamPlan))]
+
+
+class OpAdmit(C.Structure):   # sv_op_admit_args
+    _fields_ = [("k", C.c_int32), ("S", C.c_int32), ("slot_host", C.POINTER(C.c_int32)), ("len_host", C.POINTER(C.c_int32)),
+                ("max_new_host", C.POINTER(C.c_int32)), ("seed_host", C.POINTER(C.c_uint64)), ("seen", C.c_void_p),
+                ("vocab", C.c_int32), ("out_ids", C.c_void_p), ("out_stride", C.c_int32), ("pad_id", C.c_int32),
+                ("row_len_host", C.POINTER(C.c_int32)), ("row_step_host", C.POINTER(C.c_int32)),
+                ("row_active_host", C.POINTER(C.c_int32)), ("row_max_new_host", C.POINTER(C.c_int32)),
+                ("row_seed_host", C.POINTER(C.c_uint64)), ("event_host", C.POINTER(C.c_int32))]
+
+
 class SpecParams(C.Structure):   # sv_spec_params
     _fields_ = [("num_tokens", C.c_int32), ("max_matching_ngram_size", C.c_int32)]
 
@@ -165,6 +193,10 @@ SIGNATURES = {
     "sv_op_select": (C.c_int, [C.POINTER(OpSelect), _P]),
     "sv_op_spec_select": (C.c_int, [C.POINTER(OpSpec), _P]),
     "sv_op_beam_candidates": (C.c_int, [_P, _I, C.POINTER(BeamParams), _I, _I, C.POINTER(C.c_float), _P, _I, _P, _P, _P, _P]),
+    "sv_op_beam_step": (C.c_int, [C.POINTER(OpBeamStep), _P]),
+    "sv_op_beam_kv_copy": (C.c_int, [_P, _P, C.c_int64, _I, _I, _I, _I, C.POINTER(BeamPlan), _P]),
+    "sv_op_kv_gather": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "sv_op_session_admit": (C.c_int, [C.POINTER(OpAdmit), _P]),
     "sv_op_im2col": (C.c_int, [_P, _P, _I, _I, _I, _I, _P]),
     "sv_op_vit_assemble": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
     "sv_op_adapter_norm": (C.c_int, [_I, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _P]),

@@ -2495,6 +2495,189 @@ int sv_op_beam_candidates(const void* logits, int32_t vocab, const sv_beam_param
   return r == cudaSuccess ? SV_OK : op_fail("beam_candidates", r);
 }
 
+// The bookkeeping and KV-movement kernels of the beam loop, launched as sv_beam_search / sv_reorder_cache / sv_session_admit
+// launch them.
+static_assert(sizeof(sv_beam_state) == sizeof(svbeam::State) &&
+              offsetof(sv_beam_state, running_scores) == offsetof(svbeam::State, running_scores) &&
+              offsetof(sv_beam_state, beam_scores) == offsetof(svbeam::State, beam_scores) &&
+              offsetof(sv_beam_state, is_finished) == offsetof(svbeam::State, is_finished) &&
+              offsetof(sv_beam_state, fin_len) == offsetof(svbeam::State, fin_len) &&
+              offsetof(sv_beam_state, unsatisfied) == offsetof(svbeam::State, unsatisfied) &&
+              offsetof(sv_beam_state, div) == offsetof(svbeam::State, div),
+              "sv_beam_state mirrors svbeam::State");
+static_assert(sizeof(sv_beam_plan) == sizeof(svbeam::Plan) && offsetof(sv_beam_plan, run_tok) == offsetof(svbeam::Plan, run_tok) &&
+              offsetof(sv_beam_plan, fin_old) == offsetof(svbeam::Plan, fin_old) &&
+              offsetof(sv_beam_plan, fin_parent) == offsetof(svbeam::Plan, fin_parent) &&
+              offsetof(sv_beam_plan, fin_tok) == offsetof(svbeam::Plan, fin_tok) &&
+              offsetof(sv_beam_plan, copy_src) == offsetof(svbeam::Plan, copy_src) &&
+              offsetof(sv_beam_plan, copy_lo) == offsetof(svbeam::Plan, copy_lo) &&
+              offsetof(sv_beam_plan, copy_hi) == offsetof(svbeam::Plan, copy_hi) &&
+              offsetof(sv_beam_plan, cont) == offsetof(svbeam::Plan, cont) &&
+              offsetof(sv_beam_plan, old_len) == offsetof(svbeam::Plan, old_len),
+              "sv_beam_plan mirrors svbeam::Plan");
+
+int sv_op_beam_step(const sv_op_beam_step_args* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad beam_step arguments: null descriptor");
+  const sv_op_beam_step_args& o = *args;
+  const char* bad = nullptr;
+  if (!o.params || !o.state_host || !o.cand_key || !o.cand_val || !o.cand_tok || !o.run_seq || !o.fin_seq || !o.gen_host ||
+      !o.wte || !o.x || !o.next_ids || !o.plan_host)
+    bad = "null pointer (only wpe may be NULL)";
+  else if (sv_beam_params_check_rows(o.params, o.batch, svbeam::kMaxRows) != SV_OK)
+    bad = "beam parameters (num_beams in [2, 8], batch * num_beams <= 16, max_new_tokens >= 1, n_stop_ids in [0, 8], "
+          "early_stopping in {0, 1, 2}, temperature > 0, repetition_penalty > 0)";
+  else if (o.vocab < 1 || o.seq_stride < 1) bad = "vocab and seq_stride must be >= 1";
+  else if (o.advance != 0 && o.advance != 1) bad = "advance is 0 or 1";
+  else if (o.h < 8 || o.h % 8) bad = "h % 8 != 0";
+  else if (o.n_positions < 1) bad = "n_positions < 1";
+  else if (!aligned16(o.wte) || !aligned16(o.wpe) || !aligned16(o.x)) bad = "wte, wpe and x must be 16-byte aligned";
+  else if (o.gen_host[0] < 0) bad = "cur_len < 0";
+  else {
+    const sv_beam_state& s = *o.state_host;
+    // the sequence moves write positions [0, cur_len] of every row; the row-0 stop check reads the n_stop - 1 before it
+    if (s.cur_len < 0 || s.cur_len >= o.seq_stride) bad = "state cur_len not in [0, seq_stride)";
+    else if (s.parity != 0 && s.parity != 1) bad = "state parity is 0 or 1";
+    for (int r = 0; !bad && r < o.batch * o.params->num_beams; ++r)
+      if (s.fin_len[r] < 0 || s.fin_len[r] > o.seq_stride) bad = "a state fin_len is not in [0, seq_stride]";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad beam_step arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const svbeam::Params hp = beam_params_dev(o.params, o.batch, o.vocab, o.seq_stride);
+  GenState gs{};
+  gs.cur_len = o.gen_host[0];
+  gs.done = o.gen_host[1];
+  char* buf = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&buf), 4 * kOpState + sizeof(svbeam::State));
+  if (r != cudaSuccess) return op_fail("beam_step alloc", r);
+  static_assert(sizeof(svbeam::Params) <= kOpState && sizeof(svbeam::Plan) <= kOpState, "params and plan fit a scratch slot");
+  svbeam::Params* d_p = reinterpret_cast<svbeam::Params*>(buf);
+  GenState* d_gs = reinterpret_cast<GenState*>(buf + kOpState);
+  svbeam::Plan* d_plan = reinterpret_cast<svbeam::Plan*>(buf + 2 * kOpState);
+  svbeam::State* d_s = reinterpret_cast<svbeam::State*>(buf + 4 * kOpState);
+  r = cudaMemcpyAsync(d_p, &hp, sizeof(hp), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_plan, o.plan_host, sizeof(svbeam::Plan), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_s, o.state_host, sizeof(svbeam::State), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) {
+    launch_beam_step(d_p, d_s, d_plan, o.cand_key, o.cand_val, o.cand_tok, o.run_seq, o.fin_seq, d_gs, o.advance,
+                     (const bf16*)o.wte, (const bf16*)o.wpe, (bf16*)o.x, o.h, o.n_positions, o.next_ids, st);
+    r = cudaGetLastError();
+  }
+  svbeam::State hs;
+  svbeam::Plan hplan;
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&gs, d_gs, sizeof(gs), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&hs, d_s, sizeof(hs), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&hplan, d_plan, sizeof(hplan), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  if (r != cudaSuccess) return op_fail("beam_step", r);
+  memcpy(o.state_host, &hs, sizeof(hs));
+  memcpy(o.plan_host, &hplan, sizeof(hplan));
+  o.gen_host[0] = gs.cur_len;
+  o.gen_host[1] = gs.done;
+  return SV_OK;
+}
+
+int sv_op_beam_kv_copy(void* kcache, void* vtcache, int64_t layer_stride, int32_t n_layer, int32_t rows, int32_t n_kv,
+                       int32_t tcap, const sv_beam_plan* plan_host, void* stream) {
+  const int D = 128;
+  const char* bad = nullptr;
+  if (!kcache || !vtcache || !plan_host) bad = "null pointer";
+  else if (n_layer < 1 || rows < 1 || rows > svbeam::kMaxRows || n_kv < 1) bad = "n_layer, n_kv >= 1 and rows in [1, 16]";
+  else if (tcap < 32 || tcap % 32) bad = "tcap % 32 != 0";
+  else if (layer_stride < (int64_t)rows * n_kv * tcap * D || layer_stride % 8) bad = "layer_stride < rows * n_kv * tcap * 128 or % 8 != 0";
+  else if (!aligned16(kcache) || !aligned16(vtcache)) bad = "the caches must be 16-byte aligned";
+  else if (plan_host->copy_hi >= tcap) bad = "copy_hi >= tcap";
+  for (int r = 0; !bad && r < rows; ++r) {
+    if (plan_host->copy_src[r] < -1 || plan_host->copy_src[r] >= rows) bad = "a copy_src is not in [-1, rows)";
+    else if (plan_host->copy_src[r] >= 0 && plan_host->copy_lo[r] <= plan_host->copy_hi && plan_host->copy_lo[r] < 0)
+      bad = "a copy_lo < 0";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad beam_kv_copy arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t stage = layer_stride * n_layer;          // the staging cache has the caches' layout (as sv_beam_search's)
+  char* buf = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&buf), kOpState + 2 * stage * sizeof(bf16));
+  if (r != cudaSuccess) return op_fail("beam_kv_copy alloc", r);
+  svbeam::Plan* d_plan = reinterpret_cast<svbeam::Plan*>(buf);
+  bf16* kstage = reinterpret_cast<bf16*>(buf + kOpState);
+  bf16* vstage = kstage + stage;
+  r = cudaMemcpyAsync(d_plan, plan_host, sizeof(svbeam::Plan), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) {
+    launch_beam_kv_copy((bf16*)kcache, (bf16*)vtcache, kstage, vstage, layer_stride, n_layer, rows, n_kv, tcap, D, d_plan, st);
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  return r == cudaSuccess ? SV_OK : op_fail("beam_kv_copy", r);
+}
+
+int sv_op_kv_gather(const void* ksrc, const void* vsrc, void* kdst, void* vdst, const int32_t* idx, int32_t rows, int32_t n_kv,
+                    int32_t tcap, int32_t len, void* stream) {
+  const char* bad = nullptr;
+  if (!ksrc || !vsrc || !kdst || !vdst) bad = "null pointer";
+  else if (rows < 1 || rows > kSessionRows || n_kv < 1) bad = "rows in [1, 16] and n_kv >= 1";
+  else if (tcap < 32 || tcap % 32) bad = "tcap % 32 != 0";
+  else if (len < 1 || len > tcap) bad = "len not in [1, tcap]";
+  else if (!aligned16(ksrc) || !aligned16(vsrc) || !aligned16(kdst) || !aligned16(vdst)) bad = "the caches must be 16-byte aligned";
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad kv_gather arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  launch_kv_gather((const bf16*)ksrc, (const bf16*)vsrc, (bf16*)kdst, (bf16*)vdst, idx, rows, n_kv, tcap, 128, len, st);
+  cudaError_t r = cudaGetLastError();
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  return r == cudaSuccess ? SV_OK : op_fail("kv_gather", r);
+}
+
+int sv_op_session_admit(const sv_op_admit_args* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad session_admit arguments: null descriptor");
+  const sv_op_admit_args& o = *args;
+  const char* bad = nullptr;
+  if (!o.slot_host || !o.len_host || !o.max_new_host || !o.seed_host || !o.seen || !o.out_ids || !o.row_len_host ||
+      !o.row_step_host || !o.row_active_host || !o.row_max_new_host || !o.row_seed_host || !o.event_host)
+    bad = "null pointer";
+  else if (o.S < 1 || o.S > kSessionRows || o.k < 1 || o.k > o.S) bad = "1 <= k <= S <= 16";
+  else if (o.vocab < 1 || o.out_stride < 1) bad = "vocab and out_stride must be >= 1";
+  uint32_t used = 0;
+  for (int j = 0; !bad && j < o.k; ++j) {
+    const int s = o.slot_host[j];
+    if (s < 0 || s >= o.S || (used >> s & 1u)) bad = "a slot is outside [0, S) or listed twice";
+    else if (o.len_host[j] < 0) bad = "a len is < 0";
+    else used |= 1u << s;
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad session_admit arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  RowState rs{};
+  for (int b = 0; b < o.S; ++b) {
+    rs.row_len[b] = o.row_len_host[b]; rs.row_step[b] = o.row_step_host[b]; rs.row_active[b] = o.row_active_host[b];
+    rs.row_max_new[b] = o.row_max_new_host[b]; rs.row_seed[b] = o.row_seed_host[b];
+  }
+  rs.event = o.event_host[0];
+  SessionAdmit adm;
+  memset(&adm, 0, sizeof(adm));
+  adm.n = o.k;
+  for (int j = 0; j < o.k; ++j) {
+    adm.slot[j] = o.slot_host[j]; adm.len[j] = o.len_host[j]; adm.max_new[j] = o.max_new_host[j]; adm.seed[j] = o.seed_host[j];
+  }
+  RowState* d_rs = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&d_rs), kOpState);
+  if (r != cudaSuccess) return op_fail("session_admit alloc", r);
+  r = cudaMemcpyAsync(d_rs, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) {
+    launch_session_admit(d_rs, adm, (uint8_t*)o.seen, o.vocab, o.out_ids, o.out_stride, o.pad_id, st);
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&rs, d_rs, sizeof(rs), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(d_rs);
+  if (r != cudaSuccess) return op_fail("session_admit", r);
+  for (int b = 0; b < o.S; ++b) {
+    o.row_len_host[b] = rs.row_len[b]; o.row_step_host[b] = rs.row_step[b]; o.row_active_host[b] = rs.row_active[b];
+    o.row_max_new_host[b] = rs.row_max_new[b]; o.row_seed_host[b] = rs.row_seed[b];
+  }
+  o.event_host[0] = rs.event;
+  return SV_OK;
+}
+
 // ---- the image-encoder, adapter and prefill kernels one at a time --------------------------------------------------
 static int op_sync(const char* what, cudaStream_t st) {
   cudaError_t r = cudaGetLastError();

@@ -732,3 +732,65 @@ def op_beam_candidates(logits: torch.Tensor, bp: "_lib.BeamParams", batch: int, 
     _lib.check(lib, lib.sv_op_beam_candidates(_p(logits), vocab, C.byref(bp), batch, cur_len, rs, _p(run_seq), run_seq.shape[1],
                                               _p(key), _p(val), _p(tok), _stream_ptr(logits.device)))
     return key, val, tok
+
+
+def op_beam_step(bp: "_lib.BeamParams", batch: int, vocab: int, state: "_lib.BeamState", cand, run_seq: torch.Tensor,
+                 fin_seq: torch.Tensor, gen: list, advance: int, wte: torch.Tensor, wpe: Optional[torch.Tensor], x: torch.Tensor,
+                 n_positions: int, next_ids: torch.Tensor, plan: "_lib.BeamPlan") -> None:
+    """One beam-step launch (see sv_op_beam_step): `cand = (cand_key, cand_val, cand_tok)` `[R, 2 * num_beams]`; `run_seq`,
+    `fin_seq` int32 `[2, R, seq_stride]`, `x [R, h]` and `next_ids` int32 `[R]` are updated in place, as are `state` (a
+    `_lib.BeamState`), `plan` (a `_lib.BeamPlan`) and `gen = [cur_len, done]`."""
+    lib = _lib.load()
+    g = _i32s(gen)
+    a = _lib.OpBeamStep(params=C.pointer(bp), batch=batch, vocab=vocab, seq_stride=run_seq.shape[-1], advance=advance,
+                        state_host=C.pointer(state), cand_key=cand[0].data_ptr(), cand_val=cand[1].data_ptr(),
+                        cand_tok=cand[2].data_ptr(), run_seq=run_seq.data_ptr(), fin_seq=fin_seq.data_ptr(),
+                        gen_host=C.cast(g, C.POINTER(C.c_int32)), wte=wte.data_ptr(), x=x.data_ptr(), h=wte.shape[1],
+                        n_positions=n_positions, next_ids=next_ids.data_ptr(), plan_host=C.pointer(plan))
+    if wpe is not None:
+        a.wpe = wpe.data_ptr()
+    _lib.check(lib, lib.sv_op_beam_step(C.byref(a), _stream_ptr(x.device)))
+    gen[:] = [int(g[0]), int(g[1])]
+
+
+def op_beam_kv_copy(kcache: torch.Tensor, vtcache: torch.Tensor, rows: int, plan: "_lib.BeamPlan") -> None:
+    """The KV suffix copies of a beam step (see sv_op_beam_kv_copy) in place over `kcache [n_layer, rows_cap, n_kv, tcap, 128]`
+    and `vtcache [n_layer, rows_cap, n_kv, 128, tcap]` for rows `[0, rows)`."""
+    lib = _lib.load()
+    n_layer, _, n_kv, tcap = kcache.shape[:4]
+    _lib.check(lib, lib.sv_op_beam_kv_copy(_p(kcache), _p(vtcache), kcache[0].numel(), n_layer, rows, n_kv, tcap, C.byref(plan),
+                                           _stream_ptr(kcache.device)))
+
+
+def op_kv_gather(ksrc: torch.Tensor, vsrc: torch.Tensor, kdst: torch.Tensor, vdst: torch.Tensor, idx: Optional[torch.Tensor],
+                 rows: int, length: int) -> None:
+    """One layer's cache-row gather (see sv_op_kv_gather): row r of `kdst [>= rows, n_kv, tcap, 128]` / `vdst [>= rows, n_kv,
+    128, tcap]` takes the first `length` positions of source row `idx[r]` (int32 on the device, or None: r)."""
+    lib = _lib.load()
+    n_kv, tcap = ksrc.shape[1], ksrc.shape[2]
+    _lib.check(lib, lib.sv_op_kv_gather(_p(ksrc), _p(vsrc), _p(kdst), _p(vdst), _p(idx), rows, n_kv, tcap, length,
+                                        _stream_ptr(ksrc.device)))
+
+
+def op_session_admit(slots, lens, max_new, seeds, seen: torch.Tensor, out_ids: torch.Tensor, pad_id: int, state: dict) -> dict:
+    """One session-admission launch (see sv_op_session_admit) over `seen` uint8 `[S, vocab]` and `out_ids` int32
+    `[S, out_stride]` (updated in place); `state` holds the RowState and is updated too: `row_len, row_step, row_active,
+    row_max_new, row_seed` (`[S]` each) and `event`."""
+    lib = _lib.load()
+    S, vocab = seen.shape
+    i32p, u64 = C.POINTER(C.c_int32), lambda v: (C.c_uint64 * max(1, len(v)))(*[int(s) & (2 ** 64 - 1) for s in v])
+    keys = ("row_len", "row_step", "row_active", "row_max_new")
+    arrs = {k: _i32s(state[k]) for k in keys}
+    row_seed, event, seed = u64(state["row_seed"]), _i32s([state["event"]]), u64(seeds)
+    sl, ln, mn = _i32s(slots), _i32s(lens), _i32s(max_new)
+    a = _lib.OpAdmit(k=len(slots), S=S, slot_host=C.cast(sl, i32p), len_host=C.cast(ln, i32p), max_new_host=C.cast(mn, i32p),
+                     seed_host=C.cast(seed, C.POINTER(C.c_uint64)), seen=seen.data_ptr(), vocab=vocab, out_ids=out_ids.data_ptr(),
+                     out_stride=out_ids.shape[1], pad_id=pad_id, row_seed_host=C.cast(row_seed, C.POINTER(C.c_uint64)),
+                     event_host=C.cast(event, i32p))
+    for k in keys:
+        setattr(a, k + "_host", C.cast(arrs[k], i32p))
+    _lib.check(lib, lib.sv_op_session_admit(C.byref(a), _stream_ptr(seen.device)))
+    for k in keys:
+        state[k] = list(arrs[k])[:S]
+    state["row_seed"], state["event"] = list(row_seed)[:S], int(event[0])
+    return state

@@ -128,6 +128,62 @@ def test_1b_batch8_greedy_vs_oracle(sd_1b):
                      lambda ids: o.teacher_forced_logits(img[B8_ROWS].float(), PROMPT, ids))
 
 
+class _CountingEngine:
+    """The host-stepped beam loop over the engine, counting the steps whose cache permutation is not the identity."""
+
+    def __init__(self, eng):
+        self._eng, self.dims, self.steps, self.reordered = eng, eng.dims, 0, 0
+
+    def encode_images(self, image):
+        return self._eng.encode_images(image)
+
+    def prefill(self, prompt_ids, return_logits=False):
+        return self._eng.prefill(prompt_ids, return_logits=return_logits)
+
+    def reorder_cache(self, idx):
+        self.steps += 1
+        self.reordered += int(not torch.equal(idx.cpu().long(), torch.arange(idx.numel())))
+        return self._eng.reorder_cache(idx)
+
+    def decode_step(self, tokens):
+        return self._eng.decode_step(tokens)
+
+
+def test_1b_device_beam_search_equals_host_loop(sd_1b):
+    """sv_beam_search at the 1B shape (24 layers, 49156-token vocabulary, the whole search in the replayed graph) against the
+    host-stepped loop over the same engine: the reference configuration (2 images, num_beams=2, early_stopping=True) and 4
+    images x 4 beams (16 cache rows).  An untied random lm_head makes the beams reorder at most steps."""
+    from starvector_b200.beam_search import beam_search
+    from test_beam_gpu import PROMPT as BEAM_PROMPT, _same_or_equivalent
+
+    d, sd = dims_1b(max_batch=16, max_len=512), dict(sd_1b[1])
+    g = torch.Generator().manual_seed(3)
+    head = (torch.randn(d.vocab, d.hidden, generator=g) * 0.2).to(torch.bfloat16)
+    sd["model.svg_transformer.transformer.lm_head.weight"] = head
+    e = _engine(d, sd)
+    pad = 49152
+    try:
+        for B, nb in ((2, 2), (4, 4)):
+            img = synthetic_images(d, B, seed=4 + B)
+            ids = torch.tensor([BEAM_PROMPT] * B)
+            kw = dict(num_beams=nb, max_new_tokens=32, early_stopping=True, eos_token_id=0, pad_token_id=pad)
+            host = _CountingEngine(e)
+            ref = beam_search(host, img, ids, impl="host", **kw).cpu()
+            assert host.reordered * 2 > host.steps, (B, nb, host.reordered, host.steps)
+            got = beam_search(e, img, ids, impl="device", **kw).cpu()
+            assert got.shape == ref.shape, (B, nb, got.shape, ref.shape)
+            if not torch.equal(got, ref):
+                o = _oracle_fp32(d, sd_1b[1])
+                tied = o.llm.lm_head.weight
+                o.llm.lm_head.weight = torch.nn.Parameter(head.float())
+                try:
+                    _same_or_equivalent(o, img.float(), got, ref, pad, 1.0, 1.0)
+                finally:
+                    o.llm.lm_head.weight = tied
+    finally:
+        e.close()
+
+
 @pytest.mark.parametrize("mode", ["flow", "graph"])
 def test_1b_long_context_logits(sd_1b, mode):
     """The benchmarked shape: 4096 new tokens at B = 1 reach context 4355.  Teacher-force 4100 fixed tokens and compare the

@@ -412,6 +412,144 @@ def test_beam_candidates_op_rejects_on_the_host(kw):
     assert b"bad beam_candidates arguments" in lib.sv_last_error(None)
 
 
+BEAM_OPS = ("sv_op_beam_step", "sv_op_beam_kv_copy", "sv_op_kv_gather", "sv_op_session_admit")
+
+
+def test_beam_op_symbols_and_struct_layouts():
+    assert _lib.ABI_VERSION == 7
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    for name in BEAM_OPS:
+        assert name in _header_symbols() and name in _lib.SIGNATURES and name in exported, name
+    # sv_beam_state = svbeam::State: 4 int32, running_scores[16], beam_scores[16], is_finished[16], fin_len[16],
+    # unsatisfied[16], div[16][16]
+    s = _lib.BeamState
+    assert C.sizeof(s) == 340 * 4 == _lib.load().sv_beam_state_bytes()
+    assert (s.running_scores.offset, s.beam_scores.offset, s.is_finished.offset, s.fin_len.offset, s.unsatisfied.offset,
+            s.div.offset) == (16, 80, 144, 208, 272, 336)
+    # sv_beam_plan = svbeam::Plan: 7 x int32[16], copy_hi, cont, old_len
+    p = _lib.BeamPlan
+    assert C.sizeof(p) == 115 * 4
+    assert (p.run_tok.offset, p.fin_old.offset, p.fin_parent.offset, p.fin_tok.offset, p.copy_src.offset, p.copy_lo.offset,
+            p.copy_hi.offset, p.cont.offset, p.old_len.offset) == (64, 128, 192, 256, 320, 384, 448, 452, 456)
+    # sv_op_beam_step_args: pointer, 4 int32, 10 pointers, 2 int32, 2 pointers
+    o = _lib.OpBeamStep
+    assert C.sizeof(o) == 128
+    assert (o.batch.offset, o.advance.offset, o.state_host.offset, o.cand_tok.offset, o.fin_seq.offset, o.gen_host.offset,
+            o.wpe.offset, o.x.offset, o.h.offset, o.n_positions.offset, o.next_ids.offset, o.plan_host.offset) == (
+        8, 20, 24, 48, 64, 72, 88, 96, 104, 108, 112, 120)
+    # sv_op_admit_args: 2 int32, 5 pointers, int32 (+4), pointer, 2 int32, 6 pointers
+    a = _lib.OpAdmit
+    assert C.sizeof(a) == 120
+    assert (a.slot_host.offset, a.seed_host.offset, a.seen.offset, a.vocab.offset, a.out_ids.offset, a.out_stride.offset,
+            a.pad_id.offset, a.row_len_host.offset, a.row_seed_host.offset, a.event_host.offset) == (
+        8, 32, 40, 48, 56, 64, 68, 72, 104, 112)
+
+
+def test_beam_state_struct_is_the_host_replay_blob():
+    """sv_beam_state_init_host writes svbeam::State: read through the ctypes mirror, every field sits where it should."""
+    lib = _lib.load()
+    bp = _lib.BeamParams(num_beams=4, max_new_tokens=8, temperature=1.0, repetition_penalty=1.0, length_penalty=1.0)
+    s = _lib.BeamState()
+    C.memset(C.byref(s), 0x55, C.sizeof(s))
+    assert lib.sv_beam_state_init_host(C.byref(bp), 4, 261, C.byref(s)) == 0
+    assert (s.cur_len, s.done, s.parity, s.pad_) == (0, 0, 0, 0)
+    assert list(s.running_scores) == [0.0 if r % 4 == 0 else -1e9 for r in range(16)]
+    assert list(s.beam_scores) == [-1e9] * 16
+    assert list(s.is_finished) == [0] * 16 and list(s.fin_len) == [0] * 16 and list(s.unsatisfied) == [1] * 16
+    assert all(list(row) == [261] * 16 for row in s.div)
+
+
+def _bad_beam_step(**kw):
+    a = dict(num_beams=2, batch=2, vocab=500, seq_stride=64, advance=1, cur_len=5, parity=0, fin_len=0, gen_cur=300, h=64,
+             n_positions=512, wpe=0x60000, x=0x70000, null=None, descriptor=True)
+    a.update(kw)
+    bp = _lib.BeamParams(num_beams=a["num_beams"], max_new_tokens=64, early_stopping=1, temperature=1.0, repetition_penalty=1.0,
+                         length_penalty=1.0)
+    st = _lib.BeamState(cur_len=a["cur_len"], parity=a["parity"])
+    st.fin_len[1] = a["fin_len"]
+    plan = _lib.BeamPlan()
+    gen = (C.c_int32 * 2)(a["gen_cur"], 0)
+    o = _lib.OpBeamStep(params=C.pointer(bp), batch=a["batch"], vocab=a["vocab"], seq_stride=a["seq_stride"],
+                        advance=a["advance"], state_host=C.pointer(st), cand_key=0x10000, cand_val=0x11000, cand_tok=0x12000,
+                        run_seq=0x20000, fin_seq=0x30000, gen_host=C.cast(gen, C.POINTER(C.c_int32)), wte=0x50000,
+                        wpe=a["wpe"], x=a["x"], h=a["h"], n_positions=a["n_positions"], next_ids=0x40000,
+                        plan_host=C.pointer(plan))
+    if a["null"]:
+        setattr(o, a["null"], None)
+    return _lib.load().sv_op_beam_step(C.byref(o) if a["descriptor"] else None, None)
+
+
+@pytest.mark.parametrize("kw", [dict(descriptor=False), dict(null="params"), dict(null="state_host"), dict(null="cand_key"),
+                                dict(null="cand_val"), dict(null="cand_tok"), dict(null="run_seq"), dict(null="fin_seq"),
+                                dict(null="gen_host"), dict(null="wte"), dict(null="x"), dict(null="next_ids"),
+                                dict(null="plan_host"), dict(num_beams=1), dict(num_beams=9), dict(batch=9), dict(batch=0),
+                                dict(vocab=0), dict(seq_stride=0), dict(advance=2), dict(advance=-1), dict(h=60), dict(h=0),
+                                dict(n_positions=0), dict(wpe=0x60008), dict(x=0x70004), dict(gen_cur=-1),
+                                dict(cur_len=64), dict(cur_len=-1), dict(parity=2), dict(fin_len=65), dict(fin_len=-1)],
+                         ids=str)
+def test_beam_step_op_rejects_on_the_host(kw):
+    """Checked before any CUDA call: these return SV_ERR_INVALID on a machine without a GPU too."""
+    assert _bad_beam_step(**kw) == _lib.SV_ERR_INVALID
+    assert b"bad beam_step arguments" in _lib.load().sv_last_error(None)
+
+
+def _bad_kv_copy(**kw):
+    a = dict(k=0x10000, v=0x20000, n_layer=2, rows=4, n_kv=2, tcap=64, stride=None, plan=True, copy_hi=40, src=1, lo=30)
+    a.update(kw)
+    stride = a["rows"] * a["n_kv"] * a["tcap"] * 128 if a["stride"] is None else a["stride"]
+    plan = _lib.BeamPlan(copy_hi=a["copy_hi"], cont=1)
+    for r in range(16):
+        plan.copy_src[r], plan.copy_lo[r] = -1, 0
+    plan.copy_src[0], plan.copy_lo[0] = a["src"], a["lo"]
+    return _lib.load().sv_op_beam_kv_copy(C.c_void_p(a["k"]), C.c_void_p(a["v"]), stride, a["n_layer"], a["rows"], a["n_kv"],
+                                          a["tcap"], C.byref(plan) if a["plan"] else None, None)
+
+
+@pytest.mark.parametrize("kw", [dict(k=0), dict(v=0), dict(plan=False), dict(n_layer=0), dict(rows=0), dict(rows=17),
+                                dict(n_kv=0), dict(tcap=48), dict(tcap=0), dict(stride=4 * 2 * 64 * 128 - 8), dict(stride=65540),
+                                dict(k=0x10008), dict(v=0x20002), dict(copy_hi=64), dict(src=4), dict(src=-2),
+                                dict(lo=-1)], ids=str)
+def test_beam_kv_copy_op_rejects_on_the_host(kw):
+    assert _bad_kv_copy(**kw) == _lib.SV_ERR_INVALID
+    assert b"bad beam_kv_copy arguments" in _lib.load().sv_last_error(None)
+
+
+@pytest.mark.parametrize("kw", [dict(ks=0), dict(vs=0), dict(kd=0), dict(vd=0), dict(rows=0), dict(rows=17), dict(n_kv=0),
+                                dict(tcap=48), dict(len=0), dict(len=65), dict(ks=0x10008), dict(vd=0x40004)], ids=str)
+def test_kv_gather_op_rejects_on_the_host(kw):
+    a = dict(ks=0x10000, vs=0x20000, kd=0x30000, vd=0x40000, rows=4, n_kv=2, tcap=64, len=64)
+    a.update(kw)
+    lib = _lib.load()
+    assert lib.sv_op_kv_gather(*(C.c_void_p(a[n]) for n in ("ks", "vs", "kd", "vd")), None, a["rows"], a["n_kv"], a["tcap"],
+                               a["len"], None) == _lib.SV_ERR_INVALID
+    assert b"bad kv_gather arguments" in lib.sv_last_error(None)
+
+
+@pytest.mark.parametrize("kw", [dict(descriptor=False), dict(null="slot_host"), dict(null="len_host"), dict(null="max_new_host"),
+                                dict(null="seed_host"), dict(null="seen"), dict(null="out_ids"), dict(null="row_len_host"),
+                                dict(null="row_seed_host"), dict(null="event_host"), dict(S=0), dict(S=17), dict(k=0),
+                                dict(k=5), dict(vocab=0), dict(out_stride=0), dict(slots=[1, 1]), dict(slots=[0, 4]),
+                                dict(slots=[-1, 0]), dict(lens=[3, -1])], ids=str)
+def test_session_admit_op_rejects_on_the_host(kw):
+    a = dict(k=2, S=4, slots=[2, 0], lens=[7, 7], vocab=500, out_stride=64, null=None, descriptor=True)
+    a.update(kw)
+    i32p = C.POINTER(C.c_int32)
+    arr = lambda v, t=C.c_int32: (t * max(16, len(v)))(*v)
+    keep = [arr(a["slots"]), arr(a["lens"]), arr([8] * 16), arr([1] * 16, C.c_uint64), arr([0] * 16), arr([0] * 16, C.c_uint64)]
+    o = _lib.OpAdmit(k=a["k"], S=a["S"], slot_host=C.cast(keep[0], i32p), len_host=C.cast(keep[1], i32p),
+                     max_new_host=C.cast(keep[2], i32p), seed_host=C.cast(keep[3], C.POINTER(C.c_uint64)), seen=0x10000,
+                     vocab=a["vocab"], out_ids=0x20000, out_stride=a["out_stride"], pad_id=0,
+                     row_seed_host=C.cast(keep[5], C.POINTER(C.c_uint64)), event_host=C.cast(keep[4], i32p))
+    for n in ("row_len_host", "row_step_host", "row_active_host", "row_max_new_host"):
+        setattr(o, n, C.cast(keep[4], i32p))
+    if a["null"]:
+        setattr(o, a["null"], None)
+    lib = _lib.load()
+    assert lib.sv_op_session_admit(C.byref(o) if a["descriptor"] else None, None) == _lib.SV_ERR_INVALID
+    assert b"bad session_admit arguments" in lib.sv_last_error(None)
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")
 def test_engine_fails_loudly_without_gpu():
     from starvector_b200.engine import Engine
