@@ -367,6 +367,50 @@ SV_API int sv_op_rope_table(void* cos_t, void* sin_t, int32_t max_pos, int32_t d
 SV_API int sv_op_rope(void* qkv, const void* cos_t, const void* sin_t, int32_t rows, int32_t seq, int32_t n_head,
                       int32_t n_kv, int32_t max_pos, int32_t pos0, const int32_t* pos_host, int32_t per_row, void* kcache,
                       void* vtcache, int32_t tcap, void* stream);
+/* The decode step as the engine chains it (the same host code as sv_decode_step), over weights, caches and activation
+ * buffers the caller owns: layers [0, n_layer) then, optionally, the lm_head.  Same conventions as the ops above (every
+ * argument checked on the host, SV_ERR_INVALID before any launch; synchronous on `stream`).
+ * SV_CHAIN_FUSED: per layer the c_attn ring GEMV (LayerNorm fused; v1 appends K/V in its epilogue, RoPE models run the
+ * RoPE + append kernel after it), the cluster attention, and the c_proj / c_fc / c_fc2 ring GEMVs; the tail is the lm_head
+ * ring with its argmax partials.  SV_CHAIN_PER_OP: LayerNorm, rowgroup GEMVs, RoPE, KV append and split attention; the
+ * tail is ln_f + the rowgroup lm_head.
+ * Activation slots: x[2l] is layer l's input (the embedding of ids, or the caller's when ids is NULL), x[2l + 1] the
+ * residual stream after its attention, x[2l + 2] its output; ln[2l], ln[2l + 1] its two LayerNorm outputs and ln[2 n_layer]
+ * ln_f's (PER_OP only); qkv[l], attn[l], h[l].  Slot k of buffer p is p + k * p_stride elements: stride 0 reuses one
+ * buffer for every layer (the engine's aliasing, the residual stream updated in place); a nonzero stride is at least one
+ * slot ([B][width]) and keeps every layer's intermediates. */
+enum { SV_CHAIN_FUSED = 0, SV_CHAIN_PER_OP = 1 };
+typedef struct sv_op_chain_layer {
+  const void *ln1_w, *ln1_b, *attn_w, *attn_b, *proj_w, *proj_b, *ln2_w, *ln2_b, *fc_w, *fc_b, *fc2_w, *fc2_b;
+} sv_op_chain_layer;
+typedef struct sv_op_chain {
+  int32_t mode;                        /* SV_CHAIN_* */
+  int32_t n_layer, B;                  /* layers run (from layer 0) >= 1; rows in [1, 16] */
+  int32_t per_row;                     /* 0: every row at pos_host[0] (GenState); 1: row b at pos_host[b] (RowState, sessions) */
+  int32_t hidden, n_inner, n_head, n_kv, vocab, n_positions, tcap, window;   /* hidden = n_head * 128 */
+  float ln_eps;
+  int32_t rope;                        /* 1: StarCoder2 (RoPE on q and k; rope_cos / rope_sin [n_positions][64]) */
+  const sv_op_chain_layer* layers;     /* host array [n_layer] */
+  const void *wte, *wpe;               /* wpe may be NULL (no learned positions) */
+  const void *lnf_w, *lnf_b, *lm_head, *rope_cos, *rope_sin;
+  void *kcache, *vtcache;              /* [layer][B][n_kv][tcap][128] / [layer][B][n_kv][128][tcap], layer_stride apart */
+  int64_t layer_stride;
+  const int32_t* ids;                  /* device int32 [B] or NULL */
+  const int32_t* pos_host;             /* [B]: the position each row's token takes, in [0, tcap - 1] (the appended slot) */
+  void *x, *ln, *qkv, *attn, *h;
+  int64_t x_stride, ln_stride, qkv_stride, attn_stride, h_stride;
+  int32_t lm_head_tail;                /* 1: the tail; logits [B][vocab], FUSED also amax_val / amax_idx */
+  void* logits;                        /*   [sv_op_ring_ntiles(vocab)][sv_op_ring_row_stride(B)] */
+  float* amax_val;
+  int32_t* amax_idx;
+  int32_t pdl;                         /* FUSED: programmatic dependent launch between the chain's kernels */
+  int32_t graph;                       /* 1: capture the chain in a CUDA graph once and launch the graph */
+  int32_t tiled;                       /* FUSED: stream slab-tiled copies of the weights (built by the call) */
+  int32_t parts;                       /* CTAs per cluster (FUSED, <= 8) / splits (PER_OP, <= 128); 0: the engine's rule */
+  int32_t parts_used;                  /* out: the cluster size / split count the attention ran with */
+  int32_t pdl_used;                    /* out: 1 if the chain ran with PDL edges (graph: the PDL capture was accepted) */
+} sv_op_chain;
+SV_API int sv_op_decode_chain(sv_op_chain* args, void* stream);
 
 /* The token-selection kernels one launch at a time: what follows the logits of a decode step.  The caller owns the device
  * tensors; the generation state travels as HOST arrays that are read on entry and written back on return.  The same

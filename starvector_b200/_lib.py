@@ -67,6 +67,26 @@ class OpRing(C.Structure):   # sv_op_ring
         ("pos_host", C.POINTER(C.c_int32)), ("amax_val", C.c_void_p), ("amax_idx", C.c_void_p)]
 
 
+SV_CHAIN_FUSED, SV_CHAIN_PER_OP = 0, 1
+CHAIN_LAYER_FIELDS = ("ln1_w", "ln1_b", "attn_w", "attn_b", "proj_w", "proj_b", "ln2_w", "ln2_b", "fc_w", "fc_b", "fc2_w", "fc2_b")
+
+
+class OpChainLayer(C.Structure):   # sv_op_chain_layer
+    _fields_ = [(n, C.c_void_p) for n in CHAIN_LAYER_FIELDS]
+
+
+class OpChain(C.Structure):   # sv_op_chain
+    _fields_ = [(n, C.c_int32) for n in ("mode", "n_layer", "B", "per_row", "hidden", "n_inner", "n_head", "n_kv", "vocab",
+                                         "n_positions", "tcap", "window")] + [
+        ("ln_eps", C.c_float), ("rope", C.c_int32), ("layers", C.POINTER(OpChainLayer))] + [
+        (n, C.c_void_p) for n in ("wte", "wpe", "lnf_w", "lnf_b", "lm_head", "rope_cos", "rope_sin", "kcache", "vtcache")] + [
+        ("layer_stride", C.c_int64), ("ids", C.c_void_p), ("pos_host", C.POINTER(C.c_int32))] + [
+        (n, C.c_void_p) for n in ("x", "ln", "qkv", "attn", "h")] + [
+        (n, C.c_int64) for n in ("x_stride", "ln_stride", "qkv_stride", "attn_stride", "h_stride")] + [
+        ("lm_head_tail", C.c_int32), ("logits", C.c_void_p), ("amax_val", C.c_void_p), ("amax_idx", C.c_void_p)] + [
+        (n, C.c_int32) for n in ("pdl", "graph", "tiled", "parts", "parts_used", "pdl_used")]
+
+
 SV_SELECT_GREEDY, SV_SELECT_SAMPLE, SV_SELECT_FUSED = 0, 1, 2
 SV_ADAPTER_NORM_SLAB, SV_ADAPTER_NORM_TOKENS = 0, 1
 
@@ -190,6 +210,7 @@ SIGNATURES = {
     "sv_op_ring_row_stride": (C.c_int32, [_I]),
     "sv_op_rope_table": (C.c_int, [_P, _P, _I, _I, _F, _P]),
     "sv_op_rope": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, C.POINTER(_I), _I, _P, _P, _I, _P]),
+    "sv_op_decode_chain": (C.c_int, [C.POINTER(OpChain), _P]),
     "sv_op_select": (C.c_int, [C.POINTER(OpSelect), _P]),
     "sv_op_spec_select": (C.c_int, [C.POINTER(OpSpec), _P]),
     "sv_op_beam_candidates": (C.c_int, [_P, _I, C.POINTER(BeamParams), _I, _I, C.POINTER(C.c_float), _P, _I, _P, _P, _P, _P]),

@@ -534,73 +534,139 @@ int run_score_chunk(sv_engine* e, const int32_t* ids, int n, int c0, int C, int 
 }
 
 // ---- one decode step: token ids (device) at position state->cur_len -> logits ----------------
-// rows != nullptr: a session step, row b at its own position rows->row_len[b]
-int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaStream_t st, const RowState* rows = nullptr) {
+// The decode chain of one step as plain data.  The engine fills it from its own state with every activation stride 0
+// (one buffer reused by every layer, the residual stream updated in place); sv_op_decode_chain fills it from the caller's
+// tensors, where a nonzero stride (elements) keeps every layer's intermediates.  Slots: x[2l] is layer l's input,
+// x[2l + 1] the residual stream after its attention, x[2l + 2] its output; ln[2l], ln[2l + 1] its LayerNorm outputs and
+// ln[2 n_layer] ln_f's (per-op chain only); qkv[l], attn[l], h[l].
+struct DecodeChain {
+  int n_layer = 0;
+  const DecLayer* layers = nullptr;
+  uint8_t* const *t_attn = nullptr, *const *t_proj = nullptr, *const *t_fc = nullptr, *const *t_fc2 = nullptr;   // slab-tiled
+  const uint8_t* t_lm_head = nullptr;                                                        //   copies, or nullptr
+  bf16 *kcache = nullptr, *vtcache = nullptr;   // [layer][row][n_kv][tcap][D] / [layer][row][n_kv][D][tcap]
+  int64_t layer_stride = 0;
+  GenState* state = nullptr;
+  const RowState* rows = nullptr;               // != nullptr: a session step, row b at rows->row_len[b]
+  const svspec::ColMap* cmap = nullptr;         // != nullptr: a speculative verify step (fused chain, v1 only)
+  int H = 0, I = 0, n_head = 0, n_kv = 0, D = 0, qkv_cols = 0, vocab = 0, n_positions = 0, tcap = 0, window = 0;
+  float ln_eps = 0.f;
+  bool rope = false;                            // StarCoder2: RoPE on q and k before the append
+  const bf16 *rope_cos = nullptr, *rope_sin = nullptr, *wte = nullptr, *wpe = nullptr, *lnf_w = nullptr, *lnf_b = nullptr,
+             *lm_head = nullptr;
+  bf16 *x = nullptr, *ln = nullptr, *qkv = nullptr, *attn = nullptr, *h = nullptr;
+  int64_t sx = 0, sln = 0, sqkv = 0, sattn = 0, sh = 0;
+  float* attn_partial = nullptr;                // split partials of the per-op attention
+  bool lm_tail = true;                          // ln_f + lm_head after the layers
+  bf16* logits = nullptr;
+  float* amax_val = nullptr;                    // fused chain: the lm_head's argmax partials
+  int* amax_idx = nullptr;
+};
+
+DecodeChain engine_chain(sv_engine* e, const RowState* rows = nullptr, const svspec::ColMap* cmap = nullptr) {
   const sv_model_desc& d = e->d;
-  const int H = d.hidden, D = d.head_dim;
-  launch_embed_tokens(ids, e->wte, e->wpe, e->state, e->d_x, B, H, d.vocab, d.n_positions, st, rows);
-  for (int i = 0; i < d.n_layer; ++i) {
-    const DecLayer& L = e->dec[i];
-    bf16* kc = e->kcache + e->cache_layer_stride * i;
-    bf16* vc = e->vtcache + e->cache_layer_stride * i;
-    launch_layernorm(e->d_x, L.ln1_w, L.ln1_b, e->d_ln, B, H, d.ln_eps, H, st);
-    launch_linear_rowgroup(e->d_ln, L.attn_w, L.attn_b, nullptr, e->d_qkv, B, e->qkv_cols, H, SV_ACT_NONE, st);
-    if (e->v2)
-      launch_rope(e->d_qkv, B, 1, e->qkv_cols, d.n_head + d.n_kv_head, D, e->rope_cos, e->rope_sin, e->state, d.n_positions, 0, st,
-                  rows);
-    launch_kv_append(e->d_qkv, kc, vc, e->state, B, d.n_head * D, d.n_kv_head, D, e->tcap, st, rows);
-    launch_attention_decode(e->d_qkv, e->qkv_cols, kc, vc, e->d_attn, e->attn_partial, e->state, B, d.n_head,
-                            d.n_kv_head, D, e->tcap, nsplit, e->window, st, rows);
-    launch_linear_rowgroup(e->d_attn, L.proj_w, L.proj_b, e->d_x, e->d_x, B, H, H, SV_ACT_NONE, st);
-    launch_layernorm(e->d_x, L.ln2_w, L.ln2_b, e->d_ln, B, H, d.ln_eps, H, st);
-    launch_linear_rowgroup(e->d_ln, L.fc_w, L.fc_b, nullptr, e->d_h, B, d.n_inner, H, SV_ACT_GELU_TANH, st);
-    launch_linear_rowgroup(e->d_h, L.fc2_w, L.fc2_b, e->d_x, e->d_x, B, H, d.n_inner, SV_ACT_NONE, st);
+  DecodeChain c;
+  c.n_layer = d.n_layer; c.layers = e->dec.data();
+  if (e->ring_tiles) { c.t_attn = e->t_attn.data(); c.t_proj = e->t_proj.data(); c.t_fc = e->t_fc.data(); c.t_fc2 = e->t_fc2.data(); }
+  c.t_lm_head = (e->ring_tiles && e->t_lm_src == e->lm_head) ? e->t_lm_head : nullptr;
+  c.kcache = e->kcache; c.vtcache = e->vtcache; c.layer_stride = e->cache_layer_stride;
+  c.state = e->state; c.rows = rows; c.cmap = cmap;
+  c.H = d.hidden; c.I = d.n_inner; c.n_head = d.n_head; c.n_kv = d.n_kv_head; c.D = d.head_dim; c.qkv_cols = e->qkv_cols;
+  c.vocab = d.vocab; c.n_positions = d.n_positions; c.tcap = e->tcap; c.window = e->window; c.ln_eps = d.ln_eps; c.rope = e->v2;
+  c.rope_cos = e->rope_cos; c.rope_sin = e->rope_sin; c.wte = e->wte; c.wpe = e->wpe; c.lnf_w = e->lnf_w; c.lnf_b = e->lnf_b;
+  c.lm_head = e->lm_head;
+  c.x = e->d_x; c.ln = e->d_ln; c.qkv = e->d_qkv; c.attn = e->d_attn; c.h = e->d_h;
+  c.attn_partial = e->attn_partial; c.logits = e->logits; c.amax_val = e->amax_val; c.amax_idx = e->amax_idx;
+  return c;
+}
+
+inline bf16* slot(bf16* p, int64_t stride, int i) { return p + stride * i; }
+
+// Per-op decode step: embedding, then per layer LayerNorm + rowgroup GEMVs, RoPE (v2), KV append and split attention.
+int run_chain_per_op(const DecodeChain& c, const int32_t* ids, int B, int nsplit, cudaStream_t st) {
+  const int H = c.H, D = c.D, n = c.n_layer;
+  if (ids) launch_embed_tokens(ids, c.wte, c.wpe, c.state, c.x, B, H, c.vocab, c.n_positions, st, c.rows);
+  for (int i = 0; i < n; ++i) {
+    const DecLayer& L = c.layers[i];
+    bf16* kc = c.kcache + c.layer_stride * i;
+    bf16* vc = c.vtcache + c.layer_stride * i;
+    bf16 *x0 = slot(c.x, c.sx, 2 * i), *x1 = slot(c.x, c.sx, 2 * i + 1), *x2 = slot(c.x, c.sx, 2 * i + 2);
+    bf16 *ln1 = slot(c.ln, c.sln, 2 * i), *ln2 = slot(c.ln, c.sln, 2 * i + 1), *qkv = slot(c.qkv, c.sqkv, i);
+    bf16 *attn = slot(c.attn, c.sattn, i), *h = slot(c.h, c.sh, i);
+    launch_layernorm(x0, L.ln1_w, L.ln1_b, ln1, B, H, c.ln_eps, H, st);
+    launch_linear_rowgroup(ln1, L.attn_w, L.attn_b, nullptr, qkv, B, c.qkv_cols, H, SV_ACT_NONE, st);
+    if (c.rope)
+      launch_rope(qkv, B, 1, c.qkv_cols, c.n_head + c.n_kv, D, c.rope_cos, c.rope_sin, c.state, c.n_positions, 0, st, c.rows);
+    launch_kv_append(qkv, kc, vc, c.state, B, c.n_head * D, c.n_kv, D, c.tcap, st, c.rows);
+    launch_attention_decode(qkv, c.qkv_cols, kc, vc, attn, c.attn_partial, c.state, B, c.n_head, c.n_kv, D, c.tcap, nsplit,
+                            c.window, st, c.rows);
+    launch_linear_rowgroup(attn, L.proj_w, L.proj_b, x0, x1, B, H, H, SV_ACT_NONE, st);
+    launch_layernorm(x1, L.ln2_w, L.ln2_b, ln2, B, H, c.ln_eps, H, st);
+    launch_linear_rowgroup(ln2, L.fc_w, L.fc_b, nullptr, h, B, c.I, H, SV_ACT_GELU_TANH, st);
+    launch_linear_rowgroup(h, L.fc2_w, L.fc2_b, x1, x2, B, H, c.I, SV_ACT_NONE, st);
   }
-  launch_layernorm(e->d_x, e->lnf_w, e->lnf_b, e->d_ln, B, H, d.ln_eps, H, st);
-  launch_linear_rowgroup(e->d_ln, e->lm_head, nullptr, nullptr, e->logits, B, d.vocab, H, SV_ACT_NONE, st);
+  if (c.lm_tail) {
+    bf16* lnf = slot(c.ln, c.sln, 2 * n);
+    launch_layernorm(slot(c.x, c.sx, 2 * n), c.lnf_w, c.lnf_b, lnf, B, H, c.ln_eps, H, st);
+    launch_linear_rowgroup(lnf, c.lm_head, nullptr, nullptr, c.logits, B, c.vocab, H, SV_ACT_NONE, st);
+  }
   return SV_OK;
 }
 
 // Fused decode step: 5 kernels per layer (4 weight-ring GEMVs with fused LayerNorm / bias / GELU / residual / KV append,
 // 1 cluster attention) + lm_head, chained with programmatic dependent launch.  `ids` != nullptr embeds those tokens first
-// (teacher forcing / sampling); with nullptr, d_x was already written by select_fused.
-// Leaves bf16 logits in e->logits and per-tile argmax partials in e->amax_*.  rows != nullptr: a session step.
-// cmap != nullptr: a speculative verify step, B columns of one cache row placed by the column map (v1 only).
-int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st,
-                            const RowState* rows = nullptr, const svspec::ColMap* cmap = nullptr) {
-  const sv_model_desc& d = e->d;
-  const int H = d.hidden, D = d.head_dim;
-  if (ids) launch_embed_tokens(ids, e->wte, e->wpe, e->state, e->d_x, B, H, d.vocab, d.n_positions, st, rows);
+// (teacher forcing / sampling); with nullptr, x[0] was already written (by select_fused).
+// Leaves bf16 logits and per-tile argmax partials in amax_*.
+int run_chain_fused(const DecodeChain& c, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st) {
+  const int H = c.H, D = c.D, n = c.n_layer;
+  if (ids) launch_embed_tokens(ids, c.wte, c.wpe, c.state, c.x, B, H, c.vocab, c.n_positions, st, c.rows);
   bool first = true;
   RingGemvLaunch g{};
-  g.B = B; g.ln_eps = d.ln_eps; g.n_head = d.n_head; g.n_kv = d.n_kv_head; g.tcap = e->tcap; g.state = e->state; g.rows = rows;
-  g.cmap = cmap;
-  g.amax_val = e->amax_val; g.amax_idx = e->amax_idx;
+  g.B = B; g.ln_eps = c.ln_eps; g.n_head = c.n_head; g.n_kv = c.n_kv; g.tcap = c.tcap; g.state = c.state; g.rows = c.rows;
+  g.cmap = c.cmap;
+  g.amax_val = c.amax_val; g.amax_idx = c.amax_idx;
   auto gemv = [&](const bf16* X, const bf16* W, const uint8_t* Wt, const bf16* bias, const bf16* res, bf16* Y, int N, int K, int act,
                   const bf16* lw, const bf16* lb, int epi, bf16* kc, bf16* vc, bool p) {
-    g.X = X; g.W = W; g.Wt = e->ring_tiles ? Wt : nullptr; g.bias = bias; g.res = res; g.Y = Y; g.N = N; g.K = K; g.act = act; g.ln_w = lw; g.ln_b = lb;
+    g.X = X; g.W = W; g.Wt = Wt; g.bias = bias; g.res = res; g.Y = Y; g.N = N; g.K = K; g.act = act; g.ln_w = lw; g.ln_b = lb;
     g.epi = epi; g.kcache = kc; g.vtcache = vc; g.pdl = p;
     launch_gemv_ring(g, st);
   };
-  for (int i = 0; i < d.n_layer; ++i) {
-    const DecLayer& L = e->dec[i];
-    bf16* kc = e->kcache + e->cache_layer_stride * i;
-    bf16* vc = e->vtcache + e->cache_layer_stride * i;
-    const bool tl = e->ring_tiles;
-    gemv(e->d_x, L.attn_w, tl ? e->t_attn[i] : nullptr, L.attn_b, nullptr, e->d_qkv, e->qkv_cols, H, SV_ACT_NONE, L.ln1_w, L.ln1_b, e->v2 ? 0 : 1, kc, vc,
-         pdl && !first);
+  for (int i = 0; i < n; ++i) {
+    const DecLayer& L = c.layers[i];
+    bf16* kc = c.kcache + c.layer_stride * i;
+    bf16* vc = c.vtcache + c.layer_stride * i;
+    bf16 *x0 = slot(c.x, c.sx, 2 * i), *x1 = slot(c.x, c.sx, 2 * i + 1), *x2 = slot(c.x, c.sx, 2 * i + 2);
+    bf16 *qkv = slot(c.qkv, c.sqkv, i), *attn = slot(c.attn, c.sattn, i), *h = slot(c.h, c.sh, i);
+    gemv(x0, L.attn_w, c.t_attn ? c.t_attn[i] : nullptr, L.attn_b, nullptr, qkv, c.qkv_cols, H, SV_ACT_NONE, L.ln1_w, L.ln1_b,
+         c.rope ? 0 : 1, kc, vc, pdl && !first);
     first = false;
-    if (e->v2)   // RoPE on q,k then append (the GEMV epilogue cannot rotate: the pair element lives in another tile)
-      launch_rope_append(e->d_qkv, B, e->qkv_cols, d.n_head, d.n_kv_head, D, e->rope_cos, e->rope_sin, kc, vc, e->state,
-                         e->tcap, d.n_positions, pdl, st, rows);
-    launch_attention_decode_cluster(e->d_qkv, e->qkv_cols, kc, vc, e->d_attn, e->state, B, d.n_head, d.n_kv_head, D, e->tcap,
-                                    std::min(ncta, 8), e->window, pdl, st, rows, cmap);
-    gemv(e->d_attn, L.proj_w, tl ? e->t_proj[i] : nullptr, L.proj_b, e->d_x, e->d_x, H, H, SV_ACT_NONE, nullptr, nullptr, 0, nullptr, nullptr, pdl);
-    gemv(e->d_x, L.fc_w, tl ? e->t_fc[i] : nullptr, L.fc_b, nullptr, e->d_h, d.n_inner, H, SV_ACT_GELU_TANH, L.ln2_w, L.ln2_b, 0, nullptr, nullptr, pdl);
-    gemv(e->d_h, L.fc2_w, tl ? e->t_fc2[i] : nullptr, L.fc2_b, e->d_x, e->d_x, H, d.n_inner, SV_ACT_NONE, nullptr, nullptr, 0, nullptr, nullptr, pdl);
+    if (c.rope)   // RoPE on q,k then append (the GEMV epilogue cannot rotate: the pair element lives in another tile)
+      launch_rope_append(qkv, B, c.qkv_cols, c.n_head, c.n_kv, D, c.rope_cos, c.rope_sin, kc, vc, c.state, c.tcap,
+                         c.n_positions, pdl, st, c.rows);
+    launch_attention_decode_cluster(qkv, c.qkv_cols, kc, vc, attn, c.state, B, c.n_head, c.n_kv, D, c.tcap, std::min(ncta, 8),
+                                    c.window, pdl, st, c.rows, c.cmap);
+    gemv(attn, L.proj_w, c.t_proj ? c.t_proj[i] : nullptr, L.proj_b, x0, x1, H, H, SV_ACT_NONE, nullptr, nullptr, 0, nullptr,
+         nullptr, pdl);
+    gemv(x1, L.fc_w, c.t_fc ? c.t_fc[i] : nullptr, L.fc_b, nullptr, h, c.I, H, SV_ACT_GELU_TANH, L.ln2_w, L.ln2_b, 0, nullptr,
+         nullptr, pdl);
+    gemv(h, L.fc2_w, c.t_fc2 ? c.t_fc2[i] : nullptr, L.fc2_b, x1, x2, H, c.I, SV_ACT_NONE, nullptr, nullptr, 0, nullptr, nullptr,
+         pdl);
   }
-  gemv(e->d_x, e->lm_head, (e->ring_tiles && e->t_lm_src == e->lm_head) ? e->t_lm_head : nullptr, nullptr, nullptr, e->logits, d.vocab, H, SV_ACT_NONE, e->lnf_w, e->lnf_b, 2, nullptr, nullptr, pdl);
+  if (c.lm_tail)
+    gemv(slot(c.x, c.sx, 2 * n), c.lm_head, c.t_lm_head, nullptr, nullptr, c.logits, c.vocab, H, SV_ACT_NONE, c.lnf_w, c.lnf_b, 2,
+         nullptr, nullptr, pdl);
   return SV_OK;
+}
+
+// The engine's steps: its own buffers and caches.  rows != nullptr: a session step.  cmap != nullptr: a speculative verify
+// step, B columns of one cache row placed by the column map (v1 only).
+int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaStream_t st, const RowState* rows = nullptr) {
+  return run_chain_per_op(engine_chain(e, rows), ids, B, nsplit, st);
+}
+
+int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st,
+                            const RowState* rows = nullptr, const svspec::ColMap* cmap = nullptr) {
+  return run_chain_fused(engine_chain(e, rows, cmap), ids, B, ncta, pdl, st);
 }
 
 // (re)build the slab-tiled copies the dataflow kernel streams, after any weight changed
@@ -634,7 +700,7 @@ FlowLaunch flow_launch_desc(sv_engine* e, int B) {
   return m;
 }
 
-int nsplit_for(const sv_engine* e, int total_len) {
+int nsplit_for(int total_len) {
   int blocks = (total_len + 31) / 32;
   return std::max(1, std::min(kMaxSplit, blocks));
 }
@@ -993,7 +1059,7 @@ int sv_decode_step(sv_engine* e, const int32_t* ids, float* logits, void* stream
   } else {
     r = e->fused_decode
             ? run_decode_layers_fused(e, ids, e->cur_batch, attention_decode_cluster_ncta(e->host_cur_len + 1), e->use_pdl, st)
-            : run_decode_layers(e, ids, e->cur_batch, nsplit_for(e, e->host_cur_len + 1), st);
+            : run_decode_layers(e, ids, e->cur_batch, nsplit_for(e->host_cur_len + 1), st);
     if (r != SV_OK) return r;
     launch_advance_len(e->state, st);
   }
@@ -1119,7 +1185,7 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
                        e->d.hidden, e->d.n_positions, e->spec, false, st);
   }
 
-  const int nsplit = fused ? attention_decode_cluster_ncta(e->prefix_len + max_new) : nsplit_for(e, e->prefix_len + max_new);
+  const int nsplit = fused ? attention_decode_cluster_ncta(e->prefix_len + max_new) : nsplit_for(e->prefix_len + max_new);
   const long long key = (long long)(spec ? ncols : B) * 100000 + nsplit * 8 + (p->do_sample ? 1 : 0) + (fused ? 2 : 0) +
                         (e->use_pdl ? 4 : 0);
   GraphEntry& ge = spec ? e->spec_graphs[key] : e->graphs[key];
@@ -1478,7 +1544,7 @@ int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_
   };
   bookkeeping(/*advance=*/0);                       // step 0: candidates from the prefill logits
 
-  const int nsplit = fused ? attention_decode_cluster_ncta(e->prefix_len + max_new) : nsplit_for(e, e->prefix_len + max_new);
+  const int nsplit = fused ? attention_decode_cluster_ncta(e->prefix_len + max_new) : nsplit_for(e->prefix_len + max_new);
   const long long key = (long long)R * 100000 + nsplit * 8 + (fused ? 2 : 0) + (e->use_pdl ? 4 : 0);
   GraphEntry& ge = e->beam_graphs[key];
   if (!ge.exec && max_new > 1) {
@@ -1748,7 +1814,7 @@ int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int3
     ensure_flow_tiles(e, st);    // (no-op unless a weight was loaded since the tiles were built)
     const bool fused = e->fused_decode, fused_select = fused && !e->sess_p.do_sample;
     const int total = e->Q + e->sess_prompt_len + e->sess_p.max_new_tokens;     // the session cap fixes the split count
-    const int nsplit = fused ? attention_decode_cluster_ncta(total) : nsplit_for(e, total);
+    const int nsplit = fused ? attention_decode_cluster_ncta(total) : nsplit_for(total);
     const long long key = (1LL << 40) + (long long)S * 100000 + nsplit * 8 + (e->sess_p.do_sample ? 1 : 0) + (fused ? 2 : 0) +
                           (e->use_pdl ? 4 : 0);
     GraphEntry& ge = e->graphs[key];
@@ -2273,6 +2339,170 @@ int sv_op_rope(void* qkv, const void* cos_t, const void* sin_t, int32_t rows, in
   if (r == cudaSuccess) r = cudaStreamSynchronize(st);
   if (buf) cudaFree(buf);
   return r == cudaSuccess ? SV_OK : op_fail("rope", r);
+}
+
+// ---- the decode step as the engine chains it, over weights, caches and buffers the caller owns ----------------------
+static_assert(sizeof(sv_op_chain) == 296 && offsetof(sv_op_chain, layer_stride) == 136 && offsetof(sv_op_chain, pdl_used) == 292,
+              "sv_op_chain layout (the ctypes binding mirrors it)");
+int sv_op_decode_chain(sv_op_chain* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad decode_chain arguments: null descriptor");
+  sv_op_chain& o = *args;
+  const bool fused = o.mode == SV_CHAIN_FUSED;
+  const int D = 128, B = o.B;
+  const int64_t qkv_cols = (int64_t)o.hidden + 2 * (int64_t)o.n_kv * D;
+  const char* bad = nullptr;
+  auto al = [](const void* p) { return aligned16(p); };
+  auto stride_ok = [&](int64_t s, int64_t width) { return s == 0 || (s >= (int64_t)B * width && s % 8 == 0); };
+  if (o.mode != SV_CHAIN_FUSED && o.mode != SV_CHAIN_PER_OP) bad = "unknown mode";
+  else if (o.n_layer < 1) bad = "n_layer < 1";
+  else if (B < 1 || B > kSessionRows) bad = "B not in [1, 16]";
+  else if (o.per_row != 0 && o.per_row != 1) bad = "per_row is 0 or 1";
+  else if (o.n_head < 1 || o.n_kv < 1 || o.n_head % o.n_kv || o.n_head / o.n_kv > 16) bad = "n_head % n_kv != 0 or group > 16";
+  else if (o.hidden != o.n_head * D) bad = "hidden != n_head * 128";
+  else if (o.hidden % 64 || o.n_inner < 64 || o.n_inner % 64) bad = "hidden and n_inner must be multiples of 64";
+  else if (o.vocab < 1 || o.n_positions < 1) bad = "vocab and n_positions must be >= 1";
+  else if (o.tcap < 32 || o.tcap % 32) bad = "tcap % 32 != 0";
+  else if (o.window < 0) bad = "window < 0";
+  else if (!(o.ln_eps >= 0.f)) bad = "ln_eps < 0";
+  else if ((o.rope | o.pdl | o.graph | o.tiled | o.lm_head_tail) & ~1) bad = "rope, pdl, graph, tiled and lm_head_tail are 0 or 1";
+  else if (o.rope && (!o.rope_cos || !o.rope_sin || !al(o.rope_cos) || !al(o.rope_sin))) bad = "rope needs 16-byte aligned rope_cos and rope_sin";
+  else if (o.tiled && !fused) bad = "tiled weights are streamed by the FUSED chain only";
+  else if (fused && (!gemv_ring_supported(o.hidden, true) || !gemv_ring_supported(o.n_inner, false))) bad = "no ring GEMV for these widths";
+  else if (fused && !o.rope && gemv_ring_ln_streamed(o.hidden))
+    bad = "the FUSED v1 chain appends K/V in the c_attn epilogue, which a LayerNorm over more than two slabs does not have";
+  else if (fused && B > 8 && (o.rope || gemv_ring_ln_streamed(o.hidden) || B > gemv_ring_max_rows()))
+    bad = "the FUSED chain over more than 8 rows needs v1 with a register-resident LayerNorm";
+  else if (o.parts < 0 || o.parts > (fused ? 8 : kMaxSplit)) bad = "parts not in [0, 8] (FUSED) / [0, 128] (PER_OP)";
+  else if (!o.layers || !o.pos_host || !o.kcache || !o.vtcache || !o.x || !o.qkv || !o.attn || !o.h || (!fused && !o.ln))
+    bad = "null pointer (layers, pos_host, caches, x, qkv, attn, h; PER_OP also ln)";
+  else if (o.ids && (!o.wte || !al(o.wte) || (o.wpe && !al(o.wpe)))) bad = "ids need a 16-byte aligned wte (and wpe)";
+  else if (o.lm_head_tail && (!o.lm_head || !o.lnf_w || !o.lnf_b || !o.logits || !al(o.lm_head) || !al(o.lnf_w) || !al(o.lnf_b) ||
+                              !al(o.logits) || (fused && (!o.amax_val || !o.amax_idx))))
+    bad = "the lm_head tail needs 16-byte aligned lm_head, lnf_w, lnf_b and logits (FUSED: amax_val and amax_idx)";
+  else if (o.layer_stride < (int64_t)B * o.n_kv * o.tcap * D) bad = "layer_stride < B * n_kv * tcap * 128";
+  else if (!stride_ok(o.x_stride, o.hidden) || !stride_ok(o.ln_stride, o.hidden) || !stride_ok(o.qkv_stride, qkv_cols) ||
+           !stride_ok(o.attn_stride, o.hidden) || !stride_ok(o.h_stride, o.n_inner))
+    bad = "an activation stride is neither 0 nor a multiple of 8 of at least one slot (B rows)";
+  else if (!al(o.kcache) || !al(o.vtcache) || !al(o.x) || (o.ln && !al(o.ln)) || !al(o.qkv) || !al(o.attn) || !al(o.h))
+    bad = "the caches and activation buffers must be 16-byte aligned";
+  for (int b = 0; !bad && b < B; ++b) {
+    if (o.pos_host[b] < 0 || o.pos_host[b] >= o.tcap) bad = "a position is not in [0, tcap - 1]";
+    else if (!o.per_row && o.pos_host[b] != o.pos_host[0]) bad = "per_row = 0 needs equal positions";
+  }
+  for (int l = 0; !bad && l < o.n_layer; ++l) {
+    const void* const* p = &o.layers[l].ln1_w;
+    for (int k = 0; !bad && k < 12; ++k)
+      if (!p[k] || !al(p[k])) bad = "every layer weight must be given and 16-byte aligned";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad decode_chain arguments: %s", bad);
+
+  cudaStream_t st = (cudaStream_t)stream;
+  int total = 0;
+  for (int b = 0; b < B; ++b) total = std::max(total, o.pos_host[b] + 1);
+  const int parts = o.parts ? o.parts : fused ? attention_decode_cluster_ncta(total) : nsplit_for(total);
+  std::vector<DecLayer> layers(o.n_layer);
+  for (int l = 0; l < o.n_layer; ++l) {
+    const sv_op_chain_layer& s = o.layers[l];
+    auto w = [](const void* p) { return const_cast<bf16*>(static_cast<const bf16*>(p)); };
+    layers[l] = DecLayer{w(s.ln1_w), w(s.ln1_b), w(s.attn_w), w(s.attn_b), w(s.proj_w), w(s.proj_b), w(s.ln2_w), w(s.ln2_b),
+                         w(s.fc_w), w(s.fc_b), w(s.fc2_w), w(s.fc2_b)};
+  }
+  // scratch: the state header, the split partials (PER_OP), the slab-tiled copies (tiled)
+  auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const int ncta = fused ? gemv_ring_ncta() : 0;
+  const size_t part_bytes = fused ? 0 : up((size_t)B * o.n_kv * kMaxSplit * (32 + 16 * D) * sizeof(float));
+  size_t tile_bytes = 0;
+  if (o.tiled) {
+    tile_bytes = (size_t)o.n_layer * (up(flow_tiled_bytes((int)qkv_cols, o.hidden, ncta)) + up(flow_tiled_bytes(o.hidden, o.hidden, ncta)) +
+                                      up(flow_tiled_bytes(o.n_inner, o.hidden, ncta)) + up(flow_tiled_bytes(o.hidden, o.n_inner, ncta)));
+    if (o.lm_head_tail) tile_bytes += up(flow_tiled_bytes(o.vocab, o.hidden, ncta));
+  }
+  void* buf = nullptr;
+  cudaError_t r = cudaMalloc(&buf, kOpState + part_bytes + tile_bytes);
+  if (r != cudaSuccess) return op_fail("decode_chain alloc", r);
+  uint8_t* q = static_cast<uint8_t*>(buf) + kOpState;
+  DecodeChain c;
+  c.attn_partial = fused ? nullptr : reinterpret_cast<float*>(q);
+  q += part_bytes;
+  std::vector<uint8_t*> t_attn, t_proj, t_fc, t_fc2;
+  if (o.tiled) {
+    auto tile = [&](const bf16* W, const bf16* bias, int N, int K) {
+      uint8_t* t = q;
+      q += up(flow_tiled_bytes(N, K, ncta));
+      launch_flow_repack(W, bias, t, N, K, ncta, st);
+      return t;
+    };
+    for (const DecLayer& L : layers) {
+      t_attn.push_back(tile(L.attn_w, L.attn_b, (int)qkv_cols, o.hidden));
+      t_proj.push_back(tile(L.proj_w, L.proj_b, o.hidden, o.hidden));
+      t_fc.push_back(tile(L.fc_w, L.fc_b, o.n_inner, o.hidden));
+      t_fc2.push_back(tile(L.fc2_w, L.fc2_b, o.hidden, o.n_inner));
+    }
+    c.t_attn = t_attn.data(); c.t_proj = t_proj.data(); c.t_fc = t_fc.data(); c.t_fc2 = t_fc2.data();
+    if (o.lm_head_tail) c.t_lm_head = tile((const bf16*)o.lm_head, nullptr, o.vocab, o.hidden);
+  }
+  GenState gs{};
+  RowState rs{};
+  gs.cur_len = o.pos_host[0];
+  for (int b = 0; b < B; ++b) rs.row_len[b] = o.pos_host[b];
+  c.n_layer = o.n_layer; c.layers = layers.data();
+  c.kcache = (bf16*)o.kcache; c.vtcache = (bf16*)o.vtcache; c.layer_stride = o.layer_stride;
+  c.state = reinterpret_cast<GenState*>(buf);
+  c.rows = o.per_row ? reinterpret_cast<const RowState*>(buf) : nullptr;
+  c.H = o.hidden; c.I = o.n_inner; c.n_head = o.n_head; c.n_kv = o.n_kv; c.D = D; c.qkv_cols = (int)qkv_cols; c.vocab = o.vocab;
+  c.n_positions = o.n_positions; c.tcap = o.tcap; c.window = o.window; c.ln_eps = o.ln_eps; c.rope = o.rope != 0;
+  c.rope_cos = (const bf16*)o.rope_cos; c.rope_sin = (const bf16*)o.rope_sin; c.wte = (const bf16*)o.wte; c.wpe = (const bf16*)o.wpe;
+  c.lnf_w = (const bf16*)o.lnf_w; c.lnf_b = (const bf16*)o.lnf_b; c.lm_head = (const bf16*)o.lm_head;
+  c.x = (bf16*)o.x; c.ln = (bf16*)o.ln; c.qkv = (bf16*)o.qkv; c.attn = (bf16*)o.attn; c.h = (bf16*)o.h;
+  c.sx = o.x_stride; c.sln = o.ln_stride; c.sqkv = o.qkv_stride; c.sattn = o.attn_stride; c.sh = o.h_stride;
+  c.lm_tail = o.lm_head_tail != 0; c.logits = (bf16*)o.logits; c.amax_val = o.amax_val; c.amax_idx = o.amax_idx;
+  auto run = [&](bool pdl, cudaStream_t s) {
+    return fused ? run_chain_fused(c, o.ids, B, parts, pdl, s) : run_chain_per_op(c, o.ids, B, parts, s);
+  };
+  if (o.per_row) r = cudaMemcpyAsync(buf, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
+  else r = cudaMemcpyAsync(buf, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = gemv_ring_init();
+  if (r == cudaSuccess) r = attention_decode_cluster_init();
+  bool pdl_used = false;
+  if (r == cudaSuccess && !o.graph) {
+    run(fused && o.pdl, st);
+    pdl_used = fused && o.pdl;
+    r = cudaGetLastError();
+  } else if (r == cudaSuccess) {
+    // the capture goes to a stream of its own (the caller's may be the legacy stream, which cannot be captured); a PDL
+    // capture the driver refuses is retried in plain stream order, as generate does
+    cudaStream_t cs = nullptr;
+    r = cudaStreamSynchronize(st);
+    if (r == cudaSuccess) r = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
+    cudaGraphExec_t exec = nullptr;
+    for (int attempt = 0; r == cudaSuccess && attempt < 2 && !exec; ++attempt) {
+      const bool pdl = fused && o.pdl && attempt == 0;
+      cudaGraph_t graph = nullptr;
+      r = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
+      if (r != cudaSuccess) break;
+      run(pdl, cs);
+      cudaError_t ce = cudaStreamEndCapture(cs, &graph);
+      if (ce == cudaSuccess) ce = cudaGraphInstantiate(&exec, graph, 0);
+      if (graph) cudaGraphDestroy(graph);
+      if (ce != cudaSuccess) {
+        exec = nullptr;
+        cudaGetLastError();
+        if (!pdl) r = ce;
+        continue;
+      }
+      pdl_used = pdl;
+    }
+    if (r == cudaSuccess) r = cudaGraphLaunch(exec, cs);
+    if (r == cudaSuccess) r = cudaStreamSynchronize(cs);
+    if (exec) cudaGraphExecDestroy(exec);
+    if (cs) cudaStreamDestroy(cs);
+  }
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  if (r != cudaSuccess) return op_fail("decode_chain", r);
+  o.parts_used = parts;
+  o.pdl_used = pdl_used ? 1 : 0;
+  return SV_OK;
 }
 
 // ---- the token-selection kernels one at a time ---------------------------------------------------------------------

@@ -794,3 +794,65 @@ def op_session_admit(slots, lens, max_new, seeds, seen: torch.Tensor, out_ids: t
         state[k] = list(arrs[k])[:S]
     state["row_seed"], state["event"] = list(row_seed)[:S], int(event[0])
     return state
+
+
+def op_decode_chain(mode: int, layers: Sequence[Dict[str, torch.Tensor]], kcache: torch.Tensor, vtcache: torch.Tensor, pos,
+                    n_head: int, n_kv: int, n_positions: int, *, ids: Optional[torch.Tensor] = None,
+                    x: Optional[torch.Tensor] = None, wte: Optional[torch.Tensor] = None, wpe: Optional[torch.Tensor] = None,
+                    lnf: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, lm_head: Optional[torch.Tensor] = None,
+                    rope: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, window: int = 0, ln_eps: float = 1e-5,
+                    per_row: bool = False, keep: bool = False, pdl: bool = True, graph: bool = False, tiled: bool = False,
+                    parts: int = 0) -> Dict[str, object]:
+    """One decode step through `sv_op_decode_chain` (the engine's chain, SV_CHAIN_FUSED or SV_CHAIN_PER_OP) over the
+    layers given (dicts of the `_lib.CHAIN_LAYER_FIELDS` tensors), caches `kcache [n_layer, >= B, n_kv, tcap, 128]` /
+    `vtcache [n_layer, >= B, n_kv, 128, tcap]` (updated) and positions `pos [B]`.  The input is the embedding of `ids`
+    (int32 `[B]`) or `x [B, hidden]`; with `lm_head` (and `lnf`) the tail runs too.  `keep`: every layer's intermediates in
+    slots of their own (see sv_op_chain) instead of one buffer per activation.  Returns the activation buffers as
+    `[slots, B, width]` tensors (`x`, `ln`, `qkv`, `attn`, `h`), `logits [B, vocab]`, FUSED `amax` (val, idx), and the
+    `parts_used` / `pdl_used` the call reports."""
+    lib = _lib.load()
+    n, B = len(layers), len(pos)
+    dev = kcache.device
+    L0 = layers[0]
+    H, I = L0["proj_w"].shape[0], L0["fc_w"].shape[0]
+    qkv_cols = L0["attn_w"].shape[0]
+    bf = dict(dtype=torch.bfloat16, device=dev)
+
+    def buf(slots, width):    # NaN-filled: a slot read before it is written shows up
+        return torch.full((slots if keep else 1, B, width), float("nan"), **bf)
+
+    out = {"x": buf(2 * n + 1, H), "ln": buf(2 * n + 1, H), "qkv": buf(n, qkv_cols), "attn": buf(n, H), "h": buf(n, I)}
+    if x is not None:
+        out["x"][0].copy_(x.view(B, H))
+    larr = (_lib.OpChainLayer * n)(*[_lib.OpChainLayer(*[L[f].data_ptr() for f in _lib.CHAIN_LAYER_FIELDS]) for L in layers])
+    posv = _i32s(pos)
+    a = _lib.OpChain(mode=mode, n_layer=n, B=B, per_row=int(per_row), hidden=H, n_inner=I, n_head=n_head, n_kv=n_kv,
+                     vocab=(wte if wte is not None else lm_head).shape[0] if (wte is not None or lm_head is not None) else 1, n_positions=n_positions, tcap=kcache.shape[3],
+                     window=window, ln_eps=ln_eps, rope=int(rope is not None), layers=larr, layer_stride=kcache.stride(0),
+                     pos_host=C.cast(posv, C.POINTER(C.c_int32)), pdl=int(pdl), graph=int(graph), tiled=int(tiled),
+                     parts=parts, lm_head_tail=int(lm_head is not None))
+    a.kcache, a.vtcache = kcache.data_ptr(), vtcache.data_ptr()
+    for name in ("x", "ln", "qkv", "attn", "h"):
+        t = out[name]
+        setattr(a, name, t.data_ptr())
+        setattr(a, name + "_stride", t[0].numel() if keep else 0)
+    if ids is not None:
+        a.ids = ids.data_ptr()
+    for name, t in (("wte", wte), ("wpe", wpe), ("lm_head", lm_head)):
+        if t is not None:
+            setattr(a, name, t.data_ptr())
+    if lnf is not None:
+        a.lnf_w, a.lnf_b = lnf[0].data_ptr(), lnf[1].data_ptr()
+    if rope is not None:
+        a.rope_cos, a.rope_sin = rope[0].data_ptr(), rope[1].data_ptr()
+    if lm_head is not None:
+        out["logits"] = torch.full((B, lm_head.shape[0]), float("nan"), **bf)
+        a.logits = out["logits"].data_ptr()
+        if mode == _lib.SV_CHAIN_FUSED:
+            nt, rs = lib.sv_op_ring_ntiles(lm_head.shape[0]), lib.sv_op_ring_row_stride(B)
+            out["amax"] = (torch.full((nt, rs), float("nan"), dtype=torch.float32, device=dev),
+                           torch.full((nt, rs), -1, dtype=torch.int32, device=dev))
+            a.amax_val, a.amax_idx = out["amax"][0].data_ptr(), out["amax"][1].data_ptr()
+    _lib.check(lib, lib.sv_op_decode_chain(C.byref(a), _stream_ptr(dev)))
+    out["parts_used"], out["pdl_used"] = int(a.parts_used), bool(a.pdl_used)
+    return out

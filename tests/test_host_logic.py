@@ -713,3 +713,71 @@ def test_v2_tokenizer_preparation(tmp_path):
         assert len(tok.encode(t)) == 1
     syn = load_tokenizer(None, 500, v2=True)
     assert isinstance(syn, SyntheticTokenizer) and syn.padding_side == "left" and syn.pad_token_id == 495
+
+
+def test_decode_chain_op_symbol_and_descriptor_layout():
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    assert "sv_op_decode_chain" in _header_symbols() and "sv_op_decode_chain" in _lib.SIGNATURES and "sv_op_decode_chain" in exported
+    assert _lib.ABI_VERSION == 7
+    assert C.sizeof(_lib.OpChainLayer) == 12 * 8
+    # 12 int32, float, int32, 10 pointers, int64, 2 pointers, 5 pointers, 5 int64, int32 (+4), 3 pointers, 6 int32
+    o = _lib.OpChain
+    assert C.sizeof(o) == 296
+    assert (o.ln_eps.offset, o.layers.offset, o.layer_stride.offset, o.pos_host.offset, o.x.offset, o.x_stride.offset,
+            o.lm_head_tail.offset, o.logits.offset, o.pdl.offset, o.parts_used.offset, o.pdl_used.offset) == \
+        (48, 56, 136, 152, 160, 200, 240, 248, 272, 288, 292)
+
+
+def _bad_chain(**kw):
+    """A v1 1B-shaped descriptor (2 layers, 2 rows) with fake aligned pointers, changed by kw; returns the call's code."""
+    a = dict(mode=0, n_layer=2, B=2, per_row=0, hidden=2048, n_inner=8192, n_head=16, n_kv=1, vocab=49156, n_positions=8192,
+             tcap=8224, window=0, ln_eps=1e-5, rope=0, pos=[100, 100], graph=0, pdl=1, tiled=0, parts=0, lm_head_tail=1,
+             layer_stride=2 * 8224 * 128, x_stride=0, h_stride=0, null_layer_field=None, ptr=0x10000, ids=0x20000, amax=True,
+             ln=0x30000, rope_tables=False)
+    a.update(kw)
+    layers = (_lib.OpChainLayer * 2)()
+    for L in layers:
+        for f in _lib.CHAIN_LAYER_FIELDS:
+            setattr(L, f, a["ptr"])
+    if a["null_layer_field"]:
+        setattr(layers[1], a["null_layer_field"], 0)
+    pos = (C.c_int32 * len(a["pos"]))(*a["pos"])
+    o = _lib.OpChain(mode=a["mode"], n_layer=a["n_layer"], B=a["B"], per_row=a["per_row"], hidden=a["hidden"],
+                     n_inner=a["n_inner"], n_head=a["n_head"], n_kv=a["n_kv"], vocab=a["vocab"], n_positions=a["n_positions"],
+                     tcap=a["tcap"], window=a["window"], ln_eps=a["ln_eps"], rope=a["rope"], layers=layers,
+                     layer_stride=a["layer_stride"], pos_host=C.cast(pos, C.POINTER(C.c_int32)), graph=a["graph"],
+                     pdl=a["pdl"], tiled=a["tiled"], parts=a["parts"], lm_head_tail=a["lm_head_tail"],
+                     x_stride=a["x_stride"], h_stride=a["h_stride"])
+    for f in ("wte", "wpe", "lnf_w", "lnf_b", "lm_head", "kcache", "vtcache", "x", "qkv", "attn", "h", "logits"):
+        setattr(o, f, 0x40000)
+    o.ln, o.ids = a["ln"], a["ids"]
+    if a["amax"]:
+        o.amax_val, o.amax_idx = 0x50000, 0x60000
+    if a["rope_tables"]:
+        o.rope_cos, o.rope_sin = 0x70000, 0x80000
+    lib = _lib.load()
+    return lib.sv_op_decode_chain(C.byref(o), None), lib.sv_last_error(None)
+
+
+@pytest.mark.parametrize("kw", [
+    dict(mode=2), dict(n_layer=0), dict(B=0), dict(B=17), dict(per_row=2), dict(n_head=16, n_kv=3), dict(n_head=17),
+    dict(hidden=2050), dict(n_inner=100), dict(vocab=0), dict(tcap=8200), dict(window=-1), dict(ln_eps=-1.0), dict(pdl=2),
+    dict(graph=-1), dict(rope=1), dict(mode=1, tiled=1), dict(parts=9), dict(mode=1, parts=129), dict(parts=-1),
+    dict(pos=[100, 101]), dict(pos=[8224, 8224]), dict(pos=[-1, -1]), dict(per_row=1, pos=[5, 8224]),
+    dict(layer_stride=8224 * 128), dict(x_stride=2048), dict(x_stride=2 * 2048 + 4), dict(h_stride=-8),
+    dict(null_layer_field="fc2_b"), dict(ptr=0x10008), dict(mode=1, ln=0), dict(ln=0x30008), dict(amax=False),
+    # 8B widths on the FUSED chain: v1 (no RoPE) has no QKV epilogue behind a streamed LayerNorm; v2 holds 8 rows
+    dict(hidden=4608, n_inner=18432, n_head=36, n_kv=4, layer_stride=2 * 4 * 8224 * 128),
+    dict(hidden=4608, n_inner=18432, n_head=36, n_kv=4, layer_stride=9 * 4 * 8224 * 128, rope=1, rope_tables=True, B=9,
+         pos=[7] * 9),
+], ids=str)
+def test_decode_chain_op_rejects_on_the_host(kw):
+    """Checked before any CUDA call: SV_ERR_INVALID on a machine without a GPU too."""
+    code, msg = _bad_chain(**kw)
+    assert code == _lib.SV_ERR_INVALID and b"decode_chain" in msg, (code, msg)
+
+
+def test_decode_chain_op_null_descriptor():
+    lib = _lib.load()
+    assert lib.sv_op_decode_chain(None, None) == _lib.SV_ERR_INVALID
