@@ -412,6 +412,51 @@ typedef struct sv_op_chain {
 } sv_op_chain;
 SV_API int sv_op_decode_chain(sv_op_chain* args, void* stream);
 
+/* The dataflow decode kernel (SV_FLOW=1 engines: decode_flow_kernel, `nsteps` whole tokens per cooperative launch) over
+ * weights, caches and exchange buffers the caller owns.  The call builds the slab-tiled weight copies the kernel streams,
+ * runs ONE launch and waits for it.  Activations travel between CTAs as flagged words: a 32-bit word holds a bf16 value
+ * (low half) and a phase tag (high half), word i of a row sits at (i >> 3) * 64 + (i & 7), rows are (n >> 3) * 64 words
+ * apart; attention partials are 64-bit words (fp32 value, 32-bit tag), each lm_head argmax partial a 64-bit word
+ * [tag16 | bf16 | index] at tile * 8 + row.  The tag of phase gp = step * (n_layer + 1) + layer is
+ * ((gp & 0x7fff) + 1) << 16 (the lm_head is "layer n_layer"; tag32: (gp + 1) << 32).  After a launch the buffers hold the
+ * last step's words: qkv, att, xb, hb of the last layer, xa its output (tag of the lm_head phase), or with do_select the
+ * next step's input (tag of (step + 1) * (n_layer + 1)).
+ * Every argument is checked on the host and refused with SV_ERR_INVALID before any launch, including every combination
+ * the kernel could not complete: first_plain = 0 needs xa words carrying the first step's tag (the call reads them back).
+ * Synchronous on `stream`. */
+enum { SV_FLOW_XA = 0, SV_FLOW_XB = 1, SV_FLOW_QKV = 2, SV_FLOW_ATT = 3, SV_FLOW_HB = 4, SV_FLOW_PART = 5, SV_FLOW_AMAX = 6 };
+/* bytes of exchange buffer `which` (SV_FLOW_*) for these dims (amax: room for any number of SMs); -1 if out of range */
+SV_API int64_t sv_op_flow_buffer_bytes(int32_t which, int32_t B, int32_t hidden, int32_t n_inner, int32_t n_kv, int32_t vocab);
+typedef struct sv_op_flow {
+  int32_t n_layer, B;                  /* [1, 24] layers from layer 0; rows in [1, 8] */
+  int32_t hidden, n_inner, n_head, n_kv, vocab, n_positions, tcap;   /* hidden = n_head * 128 */
+  float ln_eps;
+  const sv_op_chain_layer* layers;     /* host array [n_layer] */
+  const void *wte, *wpe;               /* wpe may be NULL */
+  const void *lnf_w, *lnf_b, *lm_head;
+  void *kcache, *vtcache;              /* [layer][B][n_kv][tcap][128] / [layer][B][n_kv][128][tcap], layer_stride apart */
+  int64_t layer_stride;
+  int32_t nsteps;                      /* tokens in the launch */
+  int32_t step0;                       /* phase-tag epoch of its first step (steps since the buffers were cleared) */
+  int32_t cur_len0;                    /* tokens in the cache at the start; cur_len0 + nsteps <= tcap - 1 */
+  int32_t first_plain;                 /* 1: the first step's input is x_plain (bf16 [B][hidden]) */
+  int32_t do_select;                   /* 1: greedy selection + HF bookkeeping + the next token's embedding after every step */
+  int32_t l2_ahead;                    /* weight slabs the L2 prefetch warp runs ahead of the ring, [0, 64] */
+  int32_t realloc;                     /* 1: the register-reallocating variant (SV_FLOW=1), 0: the plain one (SV_FLOW=3) */
+  int32_t clear;                       /* 1: zero the seven exchange buffers first (a new sequence; needs first_plain) */
+  sv_gen_params params;                /* do_select: greedy (do_sample = 0); repetition_penalty is read in any case */
+  int32_t out_stride;                  /* do_select: columns of out_ids */
+  int32_t* counters_host;              /* do_select: [3] step, cur_len, done; read on entry, written back */
+  int32_t* unfinished_host;            /* do_select: [B], read on entry, written back */
+  void* seen;                          /* do_select: uint8 [B][vocab] */
+  int32_t *out_ids, *next_ids;         /* do_select: [B][out_stride], [B] */
+  void *x_plain, *logits;              /* bf16 [B][hidden] (refreshed by every select), bf16 [B][vocab] (the last step's) */
+  void *xa, *xb, *qkv, *att, *hb, *part, *amax;   /* exchange buffers, sv_op_flow_buffer_bytes each */
+  int32_t ncta_used;                   /* out: CTAs of the launch (one per SM) */
+  int32_t realloc_used;                /* out: 1 if the register-reallocating variant ran */
+} sv_op_flow;
+SV_API int sv_op_decode_flow(sv_op_flow* args, void* stream);
+
 /* The token-selection kernels one launch at a time: what follows the logits of a decode step.  The caller owns the device
  * tensors; the generation state travels as HOST arrays that are read on entry and written back on return.  The same
  * logits are selected from `nsteps` times in one call, the bookkeeping advancing between the launches (B x nsteps draws

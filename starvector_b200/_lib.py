@@ -87,6 +87,23 @@ class OpChain(C.Structure):   # sv_op_chain
         (n, C.c_int32) for n in ("pdl", "graph", "tiled", "parts", "parts_used", "pdl_used")]
 
 
+SV_FLOW_XA, SV_FLOW_XB, SV_FLOW_QKV, SV_FLOW_ATT, SV_FLOW_HB, SV_FLOW_PART, SV_FLOW_AMAX = range(7)
+FLOW_BUFFERS = ("xa", "xb", "qkv", "att", "hb", "part", "amax")    # in SV_FLOW_* order
+
+
+class OpFlow(C.Structure):   # sv_op_flow
+    _fields_ = [(n, C.c_int32) for n in ("n_layer", "B", "hidden", "n_inner", "n_head", "n_kv", "vocab", "n_positions",
+                                         "tcap")] + [
+        ("ln_eps", C.c_float), ("layers", C.POINTER(OpChainLayer))] + [
+        (n, C.c_void_p) for n in ("wte", "wpe", "lnf_w", "lnf_b", "lm_head", "kcache", "vtcache")] + [
+        ("layer_stride", C.c_int64)] + [
+        (n, C.c_int32) for n in ("nsteps", "step0", "cur_len0", "first_plain", "do_select", "l2_ahead", "realloc", "clear")] + [
+        ("params", GenParams), ("out_stride", C.c_int32), ("counters_host", C.POINTER(C.c_int32)),
+        ("unfinished_host", C.POINTER(C.c_int32)), ("seen", C.c_void_p), ("out_ids", C.c_void_p), ("next_ids", C.c_void_p),
+        ("x_plain", C.c_void_p), ("logits", C.c_void_p)] + [(n, C.c_void_p) for n in FLOW_BUFFERS] + [
+        ("ncta_used", C.c_int32), ("realloc_used", C.c_int32)]
+
+
 SV_SELECT_GREEDY, SV_SELECT_SAMPLE, SV_SELECT_FUSED = 0, 1, 2
 SV_ADAPTER_NORM_SLAB, SV_ADAPTER_NORM_TOKENS = 0, 1
 
@@ -211,6 +228,8 @@ SIGNATURES = {
     "sv_op_rope_table": (C.c_int, [_P, _P, _I, _I, _F, _P]),
     "sv_op_rope": (C.c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _I, C.POINTER(_I), _I, _P, _P, _I, _P]),
     "sv_op_decode_chain": (C.c_int, [C.POINTER(OpChain), _P]),
+    "sv_op_flow_buffer_bytes": (C.c_int64, [_I, _I, _I, _I, _I, _I]),
+    "sv_op_decode_flow": (C.c_int, [C.POINTER(OpFlow), _P]),
     "sv_op_select": (C.c_int, [C.POINTER(OpSelect), _P]),
     "sv_op_spec_select": (C.c_int, [C.POINTER(OpSpec), _P]),
     "sv_op_beam_candidates": (C.c_int, [_P, _I, C.POINTER(BeamParams), _I, _I, C.POINTER(C.c_float), _P, _I, _P, _P, _P, _P]),

@@ -487,9 +487,10 @@ SV_DEVINL void gemv_flow(FCtx& cx, Ring& r, LnRing& lr, const bool has_ln, const
 //      register layout the P.V MMA wants as its A operand (so there is no transpose);
 //   2. output dims split over warps: warp w computes out[:, 16w .. 16w+15] = P . V over ALL keys of the item: it owns a
 //      disjoint slice of the output, its V^T rows are 16-byte coalesced loads that are issued before the softmax finishes.
-// One item covers <= 16 key blocks (512 keys).  Up to 512 keys of context a single item holds the whole row: it
-// normalises and writes the attention output directly (no merge hop).  Longer rows are cut into items of <= 8 blocks
-// whose (m, l, acc) partials go to merge_flow as flagged fp32 words.
+// One item covers <= ATT_BLKS = 8 key blocks (256 keys).  Up to 256 keys of context (the new token included) a single
+// item holds the whole row: it normalises and writes the attention output directly (no merge hop).  Longer rows are cut
+// into MAXS items or fewer of <= 8 blocks each, whose (m, l, acc) partials go to merge_flow as flagged fp32 words: at most
+// MAXS * 256 = 16384 keys (decode_flow_max_keys).
 constexpr int ATT_R = 1;                                  // key blocks per warp and item (2: a warp's blocks run one after the other)
 constexpr int ATT_BLKS = NWC * ATT_R;                     // key blocks per item
 constexpr int ATT_P_BYTES = ATT_BLKS * 2 * 32 * 16;       // P fragments: [block][h][lane] x 16 bytes
@@ -1207,11 +1208,19 @@ bool decode_flow_realloc_supported() { return g_flow_realloc_ok; }
 int decode_flow_ncta() { return g_flow_ncta; }
 int decode_flow_max_splits() { return flow::MAXS; }
 int decode_flow_partial_floats() { return mega::PSZ; }
-bool decode_flow_supported(int H, int I, int head_dim, int max_batch, int window, bool rope) {
-  auto okk = [](int K) { return K % 32 == 0 && (K <= mega::KS_MAX ? true : K % mega::KS_MAX == 0); };
-  return mega::NWC == 8 && g_flow_ncta > 0 && head_dim == mega::D && okk(H) && okk(I) && H <= 2 * mega::KS_MAX && max_batch <= 8 &&
-         window == 0 && !rope;      // (+ n_layer <= FLOW_MAX_LAYERS, checked at launch)
+// The widths the kernel takes, without asking the device.  A vector the consumers stage in shared memory (the hidden
+// vector, and the c_fc output when I <= 2048) must be a power-of-two number of 8-value fragments, a multiple of 32 of them
+// (stage_vector): 256, 512, 1024 or 2048 values.  A wider c_fc output is streamed per slab: I % KS_MAX == 0.
+bool decode_flow_shape_ok(int H, int I, int head_dim, int max_batch, int window, bool rope) {
+  auto staged = [](int n) { return n == 256 || n == 512 || n == 1024 || n == 2048; };
+  return mega::NWC == 8 && head_dim == mega::D && staged(H) && (staged(I) || (I > 2 * mega::KS_MAX && I % mega::KS_MAX == 0)) &&
+         max_batch >= 1 && max_batch <= 8 && window == 0 && !rope;      // (+ n_layer <= FLOW_MAX_LAYERS, checked at launch)
 }
+bool decode_flow_supported(int H, int I, int head_dim, int max_batch, int window, bool rope) {
+  return g_flow_ncta > 0 && decode_flow_shape_ok(H, I, head_dim, max_batch, window, rope);
+}
+int decode_flow_max_keys() { return flow::MAXS * flow::ATT_BLKS * 32; }
+int decode_flow_max_layers() { return flow::FLOW_MAX_LAYERS; }
 
 cudaError_t launch_decode_flow(const FlowLaunch& m, cudaStream_t st) {
   flow::FlowArgs a{};

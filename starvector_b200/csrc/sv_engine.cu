@@ -686,6 +686,9 @@ void ensure_flow_tiles(sv_engine* e, cudaStream_t st) {
   e->tiles_dirty = false;
 }
 
+// Both fillers of a FlowLaunch (this one and sv_op_decode_flow's) set every field: a field added to the descriptor changes
+// its size, and this assert sends whoever adds it to both.
+static_assert(sizeof(FlowLaunch) == 256, "FlowLaunch changed: fill the new field in flow_launch_desc AND sv_op_decode_flow");
 FlowLaunch flow_launch_desc(sv_engine* e, int B) {
   FlowLaunch m{};
   m.layers_dev = e->mega_layers; m.n_layer = e->d.n_layer; m.B = B; m.H = e->d.hidden; m.I = e->d.n_inner;
@@ -883,7 +886,8 @@ int sv_engine_create(const sv_model_desc* desc, int device, sv_engine** out) {
       sv_engine_destroy(e);
       return fail(nullptr, SV_ERR_CUDA, "persistent decode kernel setup failed: %s", cudaGetErrorString(cudaGetLastError()));
     }
-    if (!decode_flow_supported(d.hidden, d.n_inner, d.head_dim, d.max_batch, e->window, e->v2) || !e->fused_decode || d.n_layer > 24 || !e->use_tiles) e->use_flow = false;
+    if (!decode_flow_supported(d.hidden, d.n_inner, d.head_dim, d.max_batch, e->window, e->v2) || !e->fused_decode || d.n_layer > decode_flow_max_layers() ||
+        d.max_len > decode_flow_max_keys() || !e->use_tiles) e->use_flow = false;
     if (e->flow_realloc && !decode_flow_realloc_supported()) e->flow_realloc = false;
   }
   if (attention_decode_cluster_init() != cudaSuccess) {
@@ -2502,6 +2506,169 @@ int sv_op_decode_chain(sv_op_chain* args, void* stream) {
   if (r != cudaSuccess) return op_fail("decode_chain", r);
   o.parts_used = parts;
   o.pdl_used = pdl_used ? 1 : 0;
+  return SV_OK;
+}
+
+// ---- the dataflow decode kernel over weights, caches and exchange buffers the caller owns ----------------------------
+int64_t sv_op_flow_buffer_bytes(int32_t which, int32_t B, int32_t hidden, int32_t n_inner, int32_t n_kv, int32_t vocab) {
+  if (B < 1 || hidden < 8 || hidden % 8 || n_inner < 8 || n_inner % 8 || n_kv < 1 || vocab < 1) return -1;
+  const int64_t row = 64 * 4;          // bytes per 8 values: one flagged fragment per 256-byte chunk
+  switch (which) {
+    case SV_FLOW_XA: case SV_FLOW_XB: case SV_FLOW_ATT: return (int64_t)B * (hidden / 8) * row;
+    case SV_FLOW_QKV: return (int64_t)B * ((hidden + 2 * (int64_t)n_kv * 128) / 8) * row;
+    case SV_FLOW_HB: return (int64_t)B * (n_inner / 8) * row;
+    case SV_FLOW_PART: return (int64_t)B * n_kv * decode_flow_max_splits() * decode_flow_partial_floats() * 8;
+    case SV_FLOW_AMAX: return (int64_t)vocab * 8 * 8;        // a tile holds >= 1 row: at most `vocab` tiles on any device
+    default: return -1;
+  }
+}
+
+static_assert(sizeof(sv_op_flow) == 360 && offsetof(sv_op_flow, params) == 144 && offsetof(sv_op_flow, out_stride) == 232 &&
+              offsetof(sv_op_flow, ncta_used) == 352, "sv_op_flow layout (the ctypes binding mirrors it)");
+int sv_op_decode_flow(sv_op_flow* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad decode_flow arguments: null descriptor");
+  sv_op_flow& o = *args;
+  const int D = 128, B = o.B;
+  const sv_gen_params& p = o.params;
+  void* xbuf[7] = {o.xa, o.xb, o.qkv, o.att, o.hb, o.part, o.amax};
+  const char* bad = nullptr;
+  auto al = [](const void* q) { return aligned16(q); };
+  if (o.n_layer < 1 || o.n_layer > decode_flow_max_layers()) bad = "n_layer not in [1, 24]";
+  else if (B < 1 || B > 8) bad = "B not in [1, 8]";
+  else if (o.n_head < 1 || o.n_kv < 1 || o.n_head % o.n_kv || o.n_head / o.n_kv > 16) bad = "n_head % n_kv != 0 or group > 16";
+  else if (o.hidden != o.n_head * D) bad = "hidden != n_head * 128";
+  else if (!decode_flow_shape_ok(o.hidden, o.n_inner, D, B, 0, false))
+    bad = "the dataflow kernel takes hidden in {256, 512, 1024, 2048} and n_inner the same or a multiple of 1024 above 2048";
+  else if (o.vocab < 1 || o.n_positions < 1) bad = "vocab and n_positions must be >= 1";
+  else if (o.tcap < 32 || o.tcap % 32) bad = "tcap % 32 != 0";
+  else if (!(o.ln_eps >= 0.f)) bad = "ln_eps < 0";
+  else if ((o.first_plain | o.do_select | o.realloc | o.clear) & ~1) bad = "first_plain, do_select, realloc and clear are 0 or 1";
+  else if (o.nsteps < 1 || o.step0 < 0 || o.cur_len0 < 0) bad = "nsteps must be >= 1, step0 and cur_len0 >= 0";
+  else if ((int64_t)o.cur_len0 + o.nsteps > o.tcap - 1) bad = "cur_len0 + nsteps > tcap - 1";
+  else if ((int64_t)o.cur_len0 + o.nsteps > decode_flow_max_keys()) bad = "cur_len0 + nsteps > 16384 (the attention's item split)";
+  else if (o.l2_ahead < 0 || o.l2_ahead > 64) bad = "l2_ahead not in [0, 64]";
+  else if (o.clear && !o.first_plain) bad = "clear zeroes the xa words: the first step's input must come from x_plain (first_plain = 1)";
+  else if (!o.layers || !o.wte || !o.lnf_w || !o.lnf_b || !o.lm_head || !o.kcache || !o.vtcache || !o.x_plain || !o.logits)
+    bad = "null pointer (layers, wte, lnf_w, lnf_b, lm_head, caches, x_plain, logits)";
+  else if (!o.xa || !o.xb || !o.qkv || !o.att || !o.hb || !o.part || !o.amax) bad = "null exchange buffer (xa xb qkv att hb part amax)";
+  else if (!al(o.wte) || !al(o.wpe) || !al(o.lnf_w) || !al(o.lnf_b) || !al(o.lm_head) || !al(o.kcache) || !al(o.vtcache) ||
+           !al(o.x_plain) || !al(o.logits))
+    bad = "wte, wpe, lnf_w, lnf_b, lm_head, the caches, x_plain and logits must be 16-byte aligned";
+  else if (!al(o.xa) || !al(o.xb) || !al(o.qkv) || !al(o.att) || !al(o.hb) || !al(o.part) || !al(o.amax))
+    bad = "the exchange buffers must be 16-byte aligned";
+  else if (o.layer_stride < (int64_t)B * o.n_kv * o.tcap * D || o.layer_stride % 8) bad = "layer_stride < B * n_kv * tcap * 128 or not a multiple of 8";
+  else if (!(p.repetition_penalty > 0.f)) bad = "repetition_penalty must be > 0";
+  else if (o.do_select) {
+    if (p.do_sample) bad = "the dataflow kernel selects greedily: do_sample must be 0";
+    else if (p.n_stop_ids < 0 || p.n_stop_ids > 8) bad = "n_stop_ids outside [0, 8]";
+    else if (!o.seen || !o.out_ids || !o.next_ids || !o.counters_host || !o.unfinished_host)
+      bad = "do_select needs seen, out_ids, next_ids, counters_host and unfinished_host";
+    else if (o.out_stride < 1) bad = "out_stride < 1";
+    else if (o.counters_host[0] < 0 || o.counters_host[1] < 0) bad = "step and cur_len must be >= 0";
+    else if (!o.counters_host[2] && (int64_t)o.counters_host[0] + o.nsteps > o.out_stride) bad = "step + nsteps > out_stride";
+  }
+  for (int l = 0; !bad && l < o.n_layer; ++l) {
+    const void* const* w = &o.layers[l].ln1_w;
+    for (int k = 0; !bad && k < 12; ++k)
+      if (!w[k] || !al(w[k])) bad = "every layer weight must be given and 16-byte aligned";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad decode_flow arguments: %s", bad);
+
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t r = decode_flow_init();
+  if (r != cudaSuccess) return op_fail("decode_flow init", r);
+  if (!decode_flow_supported(o.hidden, o.n_inner, D, B, 0, false))
+    return fail(nullptr, SV_ERR_UNSUPPORTED, "the dataflow kernel cannot run on this device: %s", decode_flow_status());
+  if (o.realloc && !decode_flow_realloc_supported())
+    return fail(nullptr, SV_ERR_UNSUPPORTED, "the register-reallocating variant cannot run on this device: %s", decode_flow_status());
+  const int ncta = decode_flow_ncta();
+  const int64_t qkv_cols = (int64_t)o.hidden + 2 * (int64_t)o.n_kv * D;
+  if (o.clear) {
+    for (int i = 0; r == cudaSuccess && i < 7; ++i)
+      r = cudaMemsetAsync(xbuf[i], 0, (size_t)sv_op_flow_buffer_bytes(i, B, o.hidden, o.n_inner, o.n_kv, o.vocab), st);
+    if (r != cudaSuccess) return op_fail("decode_flow clear", r);
+  }
+  if (!o.first_plain) {
+    // the first step polls xa for the tag of phase step0 * (n_layer + 1): words without it would never be accepted
+    std::vector<uint32_t> w((size_t)sv_op_flow_buffer_bytes(SV_FLOW_XA, B, o.hidden, o.n_inner, o.n_kv, o.vocab) / 4);
+    r = cudaMemcpyAsync(w.data(), o.xa, w.size() * 4, cudaMemcpyDeviceToHost, st);
+    if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+    if (r != cudaSuccess) return op_fail("decode_flow xa read-back", r);
+    const uint32_t gp = (uint32_t)o.step0 * (uint32_t)(o.n_layer + 1), E0 = ((gp & 0x7fffu) + 1u) << 16;
+    for (int b = 0; b < B; ++b)
+      for (int i = 0; i < o.hidden; ++i)
+        if ((w[(size_t)b * (o.hidden / 8) * 64 + (size_t)(i >> 3) * 64 + (i & 7)] & 0xffff0000u) != E0)
+          return fail(nullptr, SV_ERR_INVALID,
+                      "bad decode_flow arguments: first_plain = 0 but xa word %d of row %d does not carry the tag of step %d", i, b, o.step0);
+  }
+  // scratch: GenState, GenParamsDev, the layer table, the slab-tiled copies (built here, as the chain's tiled = 1 does)
+  auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
+  const size_t t_attn = up(flow_tiled_bytes((int)qkv_cols, o.hidden, ncta)), t_proj = up(flow_tiled_bytes(o.hidden, o.hidden, ncta));
+  const size_t t_fc = up(flow_tiled_bytes(o.n_inner, o.hidden, ncta)), t_fc2 = up(flow_tiled_bytes(o.hidden, o.n_inner, ncta));
+  const size_t t_lm = up(flow_tiled_bytes(o.vocab, o.hidden, ncta));
+  const size_t head = 2 * kOpState + up(sizeof(MegaLayer) * o.n_layer);
+  static_assert(sizeof(GenState) <= kOpState && sizeof(GenParamsDev) <= kOpState, "the state fits a scratch slot");
+  uint8_t* buf = nullptr;
+  r = cudaMalloc(reinterpret_cast<void**>(&buf), head + o.n_layer * (t_attn + t_proj + t_fc + t_fc2) + t_lm);
+  if (r != cudaSuccess) return op_fail("decode_flow alloc", r);
+  GenState* d_gs = reinterpret_cast<GenState*>(buf);
+  GenParamsDev* d_p = reinterpret_cast<GenParamsDev*>(buf + kOpState);
+  MegaLayer* d_layers = reinterpret_cast<MegaLayer*>(buf + 2 * kOpState);
+  uint8_t* q = buf + head;
+  std::vector<MegaLayer> ml(o.n_layer);
+  auto tile = [&](const void* W, const void* bias, int N, int K, size_t bytes) {
+    uint8_t* t = q;
+    q += bytes;
+    launch_flow_repack((const bf16*)W, (const bf16*)bias, t, N, K, ncta, st);
+    return reinterpret_cast<const bf16*>(t);
+  };
+  for (int l = 0; l < o.n_layer; ++l) {
+    const sv_op_chain_layer& s = o.layers[l];
+    auto w = [](const void* v) { return static_cast<const bf16*>(v); };
+    ml[l] = MegaLayer{w(s.ln1_w), w(s.ln1_b), w(s.attn_w), w(s.attn_b), w(s.proj_w), w(s.proj_b), w(s.ln2_w), w(s.ln2_b),
+                      w(s.fc_w), w(s.fc_b), w(s.fc2_w), w(s.fc2_b), (bf16*)o.kcache + o.layer_stride * l,
+                      (bf16*)o.vtcache + o.layer_stride * l, nullptr, nullptr, nullptr, nullptr};
+    ml[l].attn_t = tile(s.attn_w, s.attn_b, (int)qkv_cols, o.hidden, t_attn);
+    ml[l].proj_t = tile(s.proj_w, s.proj_b, o.hidden, o.hidden, t_proj);
+    ml[l].fc_t = tile(s.fc_w, s.fc_b, o.n_inner, o.hidden, t_fc);
+    ml[l].fc2_t = tile(s.fc2_w, s.fc2_b, o.hidden, o.n_inner, t_fc2);
+  }
+  const bf16* lm_t = tile(o.lm_head, nullptr, o.vocab, o.hidden, t_lm);
+  GenState gs{};
+  if (o.do_select) {
+    gs.step = o.counters_host[0]; gs.cur_len = o.counters_host[1]; gs.done = o.counters_host[2];
+    for (int b = 0; b < B; ++b) gs.unfinished[b] = o.unfinished_host[b];
+  }
+  const GenParamsDev hp = gen_params_dev(&p, p.stop_row0_only, o.do_select ? o.out_stride : 1);
+  r = cudaGetLastError();
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_gs, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_p, &hp, sizeof(hp), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_layers, ml.data(), sizeof(MegaLayer) * o.n_layer, cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) {
+    // every field flow_launch_desc sets for the engine, from the caller's tensors (the size assert above it keeps the two in
+    // step), then the per-launch fields; the launch itself is the engine's launch_decode_flow
+    FlowLaunch m{};
+    m.layers_dev = d_layers; m.n_layer = o.n_layer; m.B = B; m.H = o.hidden; m.I = o.n_inner; m.n_head = o.n_head; m.n_kv = o.n_kv;
+    m.qkv_cols = (int)qkv_cols; m.vocab = o.vocab; m.tcap = o.tcap; m.n_positions = o.n_positions; m.ln_eps = o.ln_eps;
+    m.wte = (const bf16*)o.wte; m.wpe = (const bf16*)o.wpe; m.lnf_w = (const bf16*)o.lnf_w; m.lnf_b = (const bf16*)o.lnf_b;
+    m.lm_head = (const bf16*)o.lm_head; m.lm_head_t = lm_t; m.x_plain = (bf16*)o.x_plain; m.logits = (bf16*)o.logits;
+    m.xa = (uint32_t*)o.xa; m.xb = (uint32_t*)o.xb; m.qkv = (uint32_t*)o.qkv; m.att = (uint32_t*)o.att; m.hb = (uint32_t*)o.hb;
+    m.part = (unsigned long long*)o.part; m.amax = (unsigned long long*)o.amax;
+    m.state = d_gs; m.params = d_p; m.seen = (uint8_t*)o.seen; m.next_ids = o.next_ids; m.out_ids = o.out_ids;
+    m.nsteps = o.nsteps; m.step0 = o.step0; m.cur_len0 = o.cur_len0; m.first_plain = o.first_plain; m.do_select = o.do_select;
+    m.l2_ahead = o.l2_ahead; m.dbg = nullptr; m.realloc = o.realloc != 0;
+    r = launch_decode_flow(m, st);
+  }
+  if (r == cudaSuccess) r = cudaMemcpyAsync(&gs, d_gs, sizeof(gs), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  if (r != cudaSuccess) return op_fail("decode_flow", r);
+  if (o.do_select) {
+    o.counters_host[0] = gs.step; o.counters_host[1] = gs.cur_len; o.counters_host[2] = gs.done;
+    for (int b = 0; b < B; ++b) o.unfinished_host[b] = gs.unfinished[b];
+  }
+  o.ncta_used = ncta;
+  o.realloc_used = o.realloc;
   return SV_OK;
 }
 

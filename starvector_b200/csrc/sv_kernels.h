@@ -241,6 +241,9 @@ int decode_flow_max_splits();
 int decode_flow_partial_floats();
 const char* decode_flow_status();
 bool decode_flow_supported(int H, int I, int head_dim, int max_batch, int window, bool rope);
+bool decode_flow_shape_ok(int H, int I, int head_dim, int max_batch, int window, bool rope);   // host only: no device query
+int decode_flow_max_keys();         // longest row (keys, the new token included) the attention's item split covers
+int decode_flow_max_layers();
 bool decode_flow_realloc_supported();
 cudaError_t launch_decode_flow(const FlowLaunch& m, cudaStream_t st);
 size_t flow_tiled_bytes(int N, int K, int ncta);      // bytes of the slab-tiled copy of a [N][K] decode weight matrix

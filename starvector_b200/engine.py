@@ -856,3 +856,63 @@ def op_decode_chain(mode: int, layers: Sequence[Dict[str, torch.Tensor]], kcache
     _lib.check(lib, lib.sv_op_decode_chain(C.byref(a), _stream_ptr(dev)))
     out["parts_used"], out["pdl_used"] = int(a.parts_used), bool(a.pdl_used)
     return out
+
+
+def flow_buffers(B: int, hidden: int, n_inner: int, n_kv: int, vocab: int, device) -> Dict[str, torch.Tensor]:
+    """The seven exchange buffers of the dataflow decode kernel (`sv_op_flow_buffer_bytes`), zeroed: `xa xb qkv att hb` as
+    int32 flagged words, `part amax` as int64."""
+    lib = _lib.load()
+    out = {}
+    for i, name in enumerate(_lib.FLOW_BUFFERS):
+        n = int(lib.sv_op_flow_buffer_bytes(i, B, hidden, n_inner, n_kv, vocab))
+        if n < 0:
+            raise ValueError(f"no {name} buffer for B={B} hidden={hidden} n_inner={n_inner} n_kv={n_kv} vocab={vocab}")
+        out[name] = torch.zeros(n // (8 if name in ("part", "amax") else 4),
+                                dtype=torch.int64 if name in ("part", "amax") else torch.int32, device=device)
+    return out
+
+
+def op_decode_flow(layers: Sequence[Dict[str, torch.Tensor]], kcache: torch.Tensor, vtcache: torch.Tensor, n_head: int,
+                   n_kv: int, n_positions: int, *, wte: torch.Tensor, lnf: Tuple[torch.Tensor, torch.Tensor],
+                   lm_head: torch.Tensor, x_plain: torch.Tensor, bufs: Dict[str, torch.Tensor], cur_len0: int,
+                   wpe: Optional[torch.Tensor] = None, nsteps: int = 1, step0: int = 0, first_plain: bool = True,
+                   do_select: bool = False, l2_ahead: int = 0, realloc: bool = True, clear: bool = False,
+                   params: Optional[GenerationParams] = None, state: Optional[Dict[str, object]] = None,
+                   seen: Optional[torch.Tensor] = None, out_ids: Optional[torch.Tensor] = None,
+                   next_ids: Optional[torch.Tensor] = None, logits: Optional[torch.Tensor] = None,
+                   ln_eps: float = 1e-5) -> Dict[str, object]:
+    """One launch of the dataflow decode kernel through `sv_op_decode_flow` over the layers given (dicts of the
+    `_lib.CHAIN_LAYER_FIELDS` tensors), caches `kcache [n_layer, >= B, n_kv, tcap, 128]` / `vtcache [n_layer, >= B, n_kv,
+    128, tcap]` (updated), the exchange buffers `bufs` (`flow_buffers`; left holding the last step's flagged words) and
+    `x_plain [B, hidden]` (the first step's input with `first_plain`; rewritten by every selection).  With `do_select`,
+    `state` (dict step / cur_len / done / unfinished, updated in place), `seen [B, vocab]` uint8, `out_ids [B, stride]` and
+    `next_ids [B]` (int32) are the generation state.  Returns `logits [B, vocab]` (the last step's), `state`, and the
+    `ncta` / `realloc` the launch ran with."""
+    lib = _lib.load()
+    n, B, H = len(layers), x_plain.shape[0], x_plain.shape[1]
+    dev = kcache.device
+    V = lm_head.shape[0]
+    p = (params or GenerationParams(max_new_tokens=1 << 30, eos_token_id=None)).to_c()
+    if logits is None:
+        logits = torch.full((B, V), float("nan"), dtype=torch.bfloat16, device=dev)
+    larr = (_lib.OpChainLayer * n)(*[_lib.OpChainLayer(*[L[f].data_ptr() for f in _lib.CHAIN_LAYER_FIELDS]) for L in layers])
+    a = _lib.OpFlow(n_layer=n, B=B, hidden=H, n_inner=layers[0]["fc_w"].shape[0], n_head=n_head, n_kv=n_kv, vocab=V,
+                    n_positions=n_positions, tcap=kcache.shape[3], ln_eps=ln_eps, layers=larr, layer_stride=kcache.stride(0),
+                    nsteps=nsteps, step0=step0, cur_len0=cur_len0, first_plain=int(first_plain), do_select=int(do_select),
+                    l2_ahead=l2_ahead, realloc=int(realloc), clear=int(clear), params=p)
+    a.wte, a.lnf_w, a.lnf_b, a.lm_head = wte.data_ptr(), lnf[0].data_ptr(), lnf[1].data_ptr(), lm_head.data_ptr()
+    if wpe is not None:
+        a.wpe = wpe.data_ptr()
+    a.kcache, a.vtcache, a.x_plain, a.logits = kcache.data_ptr(), vtcache.data_ptr(), x_plain.data_ptr(), logits.data_ptr()
+    for name in _lib.FLOW_BUFFERS:
+        setattr(a, name, bufs[name].data_ptr())
+    counters = unfinished = None
+    if do_select:
+        counters = _i32s([state["step"], state["cur_len"], state["done"]])
+        unfinished = _i32s(state["unfinished"])
+        a.counters_host, a.unfinished_host = C.cast(counters, C.POINTER(C.c_int32)), C.cast(unfinished, C.POINTER(C.c_int32))
+        a.seen, a.out_ids, a.next_ids, a.out_stride = seen.data_ptr(), out_ids.data_ptr(), next_ids.data_ptr(), out_ids.shape[1]
+    _lib.check(lib, lib.sv_op_decode_flow(C.byref(a), _stream_ptr(dev)))
+    if do_select:
+        state.update(step=counters[0], cur_len=counters[1], done=counters[2], unfinished=[unfinished[b] for b in range(B)])
+    return {"logits": logits, "state": state, "ncta": int(a.ncta_used), "realloc": bool(a.realloc_used)}

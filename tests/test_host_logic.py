@@ -781,3 +781,114 @@ def test_decode_chain_op_rejects_on_the_host(kw):
 def test_decode_chain_op_null_descriptor():
     lib = _lib.load()
     assert lib.sv_op_decode_chain(None, None) == _lib.SV_ERR_INVALID
+
+
+def test_decode_flow_op_symbols_and_descriptor_layout():
+    exported = set(re.findall(r" T (sv_\w+)", subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH],
+                                                             capture_output=True, text=True, check=True).stdout))
+    for name in ("sv_op_decode_flow", "sv_op_flow_buffer_bytes"):
+        assert name in _header_symbols() and name in _lib.SIGNATURES and name in exported, name
+    # 9 int32, float, pointer, 7 pointers, int64, 8 int32, sv_gen_params (88), int32 (+4), 14 pointers, 2 int32
+    o = _lib.OpFlow
+    assert C.sizeof(o) == 360
+    assert (o.ln_eps.offset, o.layers.offset, o.wte.offset, o.layer_stride.offset, o.nsteps.offset, o.clear.offset,
+            o.params.offset, o.out_stride.offset, o.counters_host.offset, o.x_plain.offset, o.xa.offset, o.amax.offset,
+            o.ncta_used.offset, o.realloc_used.offset) == \
+        (36, 40, 48, 104, 112, 140, 144, 232, 240, 280, 296, 344, 352, 356)
+    text = open(os.path.join(ROOT, "include", "starvector_b200.h")).read()
+    order = re.search(r"enum \{ SV_FLOW_XA = 0, SV_FLOW_XB = 1, SV_FLOW_QKV = 2, SV_FLOW_ATT = 3, SV_FLOW_HB = 4, "
+                      r"SV_FLOW_PART = 5, SV_FLOW_AMAX = 6 \};", text)
+    assert order and _lib.FLOW_BUFFERS == ("xa", "xb", "qkv", "att", "hb", "part", "amax")
+
+
+def test_decode_flow_buffer_bytes():
+    """One flagged 32-bit word per value, each 8-value fragment in its own 256-byte chunk; attention partials: 64 splits of
+    (m[16], l[16], acc[16][128]) 64-bit words per (row, kv head); argmax partials: 8 rows of 64-bit words per lm_head tile,
+    room for one tile per vocabulary row."""
+    lib = _lib.load()
+    size = lambda w, B=8, H=2048, I=8192, kv=1, V=49157: lib.sv_op_flow_buffer_bytes(w, B, H, I, kv, V)
+    assert size(_lib.SV_FLOW_XA) == size(_lib.SV_FLOW_XB) == size(_lib.SV_FLOW_ATT) == 8 * 256 * 256
+    assert size(_lib.SV_FLOW_QKV) == 8 * (2304 // 8) * 256 and size(_lib.SV_FLOW_QKV, kv=2, H=512) == 8 * (1024 // 8) * 256
+    assert size(_lib.SV_FLOW_HB) == 8 * 1024 * 256
+    assert size(_lib.SV_FLOW_PART, B=3, kv=2) == 3 * 2 * 64 * (32 + 16 * 128) * 8
+    assert size(_lib.SV_FLOW_AMAX) == 49157 * 64
+    for bad in (dict(B=0), dict(H=2044), dict(I=0), dict(kv=0), dict(V=0)):
+        assert size(_lib.SV_FLOW_XA, **bad) == -1, bad
+    assert size(7) == -1 and size(-1) == -1
+
+
+def _bad_flow(**kw):
+    """A 1B-shaped descriptor (2 layers, 8 rows, greedy selection) with fake aligned pointers, changed by kw."""
+    a = dict(n_layer=2, B=8, hidden=2048, n_inner=8192, n_head=16, n_kv=1, vocab=49156, n_positions=8192, tcap=8224,
+             ln_eps=1e-5, layer_stride=8 * 8224 * 128, nsteps=16, step0=0, cur_len0=100, first_plain=1, do_select=1,
+             l2_ahead=0, realloc=1, clear=1, rp=1.0, do_sample=0, n_stop=0, out_stride=64, counters=[0, 100, 0],
+             unfinished=True, null_layer_field=None, ptr=0x10000, wte=0x40000, xa=0x50000, amax=0x60000, x_plain=0x70000,
+             seen=0x80000)
+    a.update(kw)
+    layers = (_lib.OpChainLayer * max(1, a["n_layer"]))()
+    for L in layers:
+        for f in _lib.CHAIN_LAYER_FIELDS:
+            setattr(L, f, a["ptr"])
+    if a["null_layer_field"]:
+        setattr(layers[-1], a["null_layer_field"], 0)
+    p = GenerationParams(max_new_tokens=64, repetition_penalty=a["rp"], do_sample=bool(a["do_sample"]),
+                         stop_ids=[7] * a["n_stop"] if a["n_stop"] <= 8 else []).to_c()
+    if a["n_stop"] > 8 or a["n_stop"] < 0:
+        p.n_stop_ids = a["n_stop"]
+    o = _lib.OpFlow(n_layer=a["n_layer"], B=a["B"], hidden=a["hidden"], n_inner=a["n_inner"], n_head=a["n_head"],
+                    n_kv=a["n_kv"], vocab=a["vocab"], n_positions=a["n_positions"], tcap=a["tcap"], ln_eps=a["ln_eps"],
+                    layers=layers, layer_stride=a["layer_stride"], nsteps=a["nsteps"], step0=a["step0"],
+                    cur_len0=a["cur_len0"], first_plain=a["first_plain"], do_select=a["do_select"], l2_ahead=a["l2_ahead"],
+                    realloc=a["realloc"], clear=a["clear"], params=p, out_stride=a["out_stride"])
+    for f in ("wpe", "lnf_w", "lnf_b", "lm_head", "kcache", "vtcache", "logits", "xb", "qkv", "att", "hb", "part", "out_ids",
+              "next_ids"):
+        setattr(o, f, 0x40000)
+    o.wte, o.xa, o.amax, o.x_plain, o.seen = a["wte"], a["xa"], a["amax"], a["x_plain"], a["seen"]
+    counters = (C.c_int32 * 3)(*a["counters"]) if a["counters"] else None
+    unfinished = (C.c_int32 * 8)(*([1] * 8)) if a["unfinished"] else None
+    if counters:
+        o.counters_host = C.cast(counters, C.POINTER(C.c_int32))
+    if unfinished:
+        o.unfinished_host = C.cast(unfinished, C.POINTER(C.c_int32))
+    lib = _lib.load()
+    return lib.sv_op_decode_flow(C.byref(o), None), lib.sv_last_error(None)
+
+
+@pytest.mark.parametrize("kw", [
+    dict(B=0), dict(B=9), dict(n_layer=0), dict(n_layer=25), dict(n_head=16, n_kv=3), dict(n_head=17),
+    # widths the kernel does not take: the 8B decoder, a hidden vector that is not 2^k fragments, a staged c_fc output
+    # that is not either, a wide one that is not whole slabs, RoPE-free GQA beyond 16 heads per group
+    dict(hidden=4608, n_inner=18432, n_head=36, n_kv=4, layer_stride=8 * 4 * 8224 * 128), dict(hidden=768, n_head=6),
+    dict(n_inner=1536), dict(n_inner=2560), dict(hidden=2048, n_head=16, n_kv=1, n_inner=96),
+    dict(vocab=0), dict(n_positions=0), dict(tcap=8200), dict(tcap=0), dict(ln_eps=-1.0),
+    dict(first_plain=2), dict(do_select=-1), dict(realloc=2), dict(clear=3),
+    dict(nsteps=0), dict(step0=-1), dict(cur_len0=-1), dict(cur_len0=8208), dict(cur_len0=8208, nsteps=16),
+    dict(tcap=16416, layer_stride=8 * 16416 * 128, cur_len0=16380, nsteps=5), dict(l2_ahead=-1), dict(l2_ahead=65),
+    dict(clear=1, first_plain=0), dict(wte=0), dict(x_plain=0), dict(xa=0), dict(amax=0), dict(wte=0x40004),
+    dict(xa=0x50008), dict(amax=0x60008), dict(x_plain=0x70002), dict(layer_stride=8 * 8224 * 128 - 8),
+    dict(layer_stride=8 * 8224 * 128 + 4), dict(null_layer_field="ln2_b"), dict(ptr=0x10008), dict(rp=0.0), dict(rp=-1.0),
+    dict(do_sample=1), dict(n_stop=9), dict(n_stop=-1), dict(seen=0), dict(counters=None), dict(unfinished=False),
+    dict(out_stride=0), dict(counters=[-1, 100, 0]), dict(counters=[60, 100, 0]), dict(counters=[0, -1, 0]),
+], ids=str)
+def test_decode_flow_op_rejects_on_the_host(kw):
+    """Every combination the kernel could not complete (its polls would spin until the watchdog traps) or would compute
+    wrong is refused before any CUDA call: SV_ERR_INVALID on a machine without a GPU too."""
+    code, msg = _bad_flow(**kw)
+    assert code == _lib.SV_ERR_INVALID and b"decode_flow" in msg, (code, msg)
+
+
+def test_decode_flow_op_accepts_what_it_should_on_the_host():
+    """The base descriptor and its edge cases pass every host check: on a machine without a GPU the call then fails in the
+    first CUDA call, not as SV_ERR_INVALID.  (A finished generation may run past out_stride: nothing is written then.)"""
+    if torch.cuda.is_available():
+        pytest.skip("a GPU would run these launches over fake pointers")
+    for kw in (dict(), dict(cur_len0=8207, nsteps=16), dict(do_select=0, seen=0,
+               counters=None, unfinished=False), dict(counters=[60, 100, 1]), dict(hidden=512, n_head=4, n_kv=2, n_inner=1024,
+               layer_stride=8 * 2 * 8224 * 128), dict(n_layer=24), dict(B=1, layer_stride=8224 * 128), dict(l2_ahead=64)):
+        code, msg = _bad_flow(**kw)
+        assert code != _lib.SV_ERR_INVALID, (kw, msg)
+
+
+def test_decode_flow_op_null_descriptor():
+    lib = _lib.load()
+    assert lib.sv_op_decode_flow(None, None) == _lib.SV_ERR_INVALID
