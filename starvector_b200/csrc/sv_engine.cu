@@ -16,6 +16,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "../../include/starvector_b200.h"
@@ -44,7 +45,19 @@ struct Weight {
 struct VitLayer { bf16 *ln1_w, *ln1_b, *qkv_w, *qkv_b, *out_w, *out_b, *ln2_w, *ln2_b, *fc_w, *fc_b, *proj_w, *proj_b; };
 struct DecLayer { bf16 *ln1_w, *ln1_b, *attn_w, *attn_b, *proj_w, *proj_b, *ln2_w, *ln2_b, *fc_w, *fc_b, *fc2_w, *fc2_b; };
 
-struct GraphEntry { cudaGraphExec_t exec = nullptr; int kernels = 0; };
+// The decode-step graphs of generate, speculative generate, beam search and sessions share one cache.  Two captures that
+// enqueue different kernels or arguments must never share a key: `rows` is the batch, the verify step's columns or the
+// session's slots, `parts` the attention partition (decode_parts).
+enum class StepKind { generate, speculative, beam, session };
+struct StepKey {
+  StepKind kind;
+  int rows, parts;
+  bool sample, fused, pdl;
+  bool operator<(const StepKey& o) const {
+    return std::tie(kind, rows, parts, sample, fused, pdl) < std::tie(o.kind, o.rows, o.parts, o.sample, o.fused, o.pdl);
+  }
+};
+struct GraphEntry { cudaGraphExec_t exec = nullptr; int kernels = 0; bool pdl = false; };
 
 }  // namespace
 
@@ -106,7 +119,6 @@ struct sv_engine {
   float *beam_key = nullptr, *beam_val = nullptr;
   int32_t *beam_tok = nullptr, *beam_run_seq = nullptr, *beam_fin_seq = nullptr;
   bf16 *kstage = nullptr, *vstage = nullptr;        // staging copy of the cache for the KV suffix moves (all layers)
-  std::map<long long, GraphEntry> beam_graphs;
   bf16 *kcache, *vtcache;           // [layer][max_batch][n_kv][tcap][D] / [layer][max_batch][n_kv][D][tcap]
   int64_t cache_layer_stride = 0;
   GenState* state = nullptr;
@@ -130,7 +142,7 @@ struct sv_engine {
 
   cudaStream_t gen_stream = nullptr;
   cudaEvent_t ev_in = nullptr, ev_t0 = nullptr, ev_t1 = nullptr;
-  std::map<long long, GraphEntry> graphs;   // key = batch * 1000 + nsplit * 2 + do_sample
+  std::map<StepKey, GraphEntry> step_graphs;
   float last_decode_ms = 0.f;
   int last_decode_steps = 0;
 
@@ -140,16 +152,14 @@ struct sv_engine {
   sv_gen_params sess_p{};
   int sess_slots = 0, sess_prompt_len = 0;   // the prompt length is fixed by the first admission
   RowState* rows = nullptr;                  // device, allocated by the first session
-  RowState* rows_host = nullptr;             // pinned read-back of the polled fields
+  RowState* rows_host = nullptr;             // pinned read-back of row_step / row_active
   bf16* sess_logits = nullptr;               // [max_batch][vocab]: the prefill logits of admitted slots (token 0 is read there)
   std::vector<int> sess_live;                // host: slot holds a request whose finish was not reported yet
   std::vector<int> sess_len;                 // host: tokens of each slot at the last poll
 
-  // prompt-lookup speculative decoding (sv_generate_speculative): device state allocated by the first call, one verify-step
-  // graph per (columns, split count, sampling, PDL)
+  // prompt-lookup speculative decoding (sv_generate_speculative): device state allocated by the first call
   svspec::State* spec = nullptr;
   RowState* spec_pos = nullptr;              // sv_spec_verify_step: the columns' embedding positions (row_len)
-  std::map<long long, GraphEntry> spec_graphs;
   int32_t spec_stats[3] = {0, 0, 0};         // steps, drafted, accepted of the last call
 };
 
@@ -170,6 +180,12 @@ int fail(sv_engine* e, int code, const char* fmt, ...) {
     cudaError_t _err = (call);                                                                      \
     if (_err != cudaSuccess)                                                                        \
       return fail((e), SV_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(_err), __FILE__, __LINE__); \
+  } while (0)
+
+#define SV_TRY(call)              \
+  do {                            \
+    const int _r = (call);        \
+    if (_r != SV_OK) return _r;   \
   } while (0)
 
 struct LaunchScope {   // routes count_launch() of this thread to the engine's counter
@@ -583,7 +599,7 @@ DecodeChain engine_chain(sv_engine* e, const RowState* rows = nullptr, const svs
 inline bf16* slot(bf16* p, int64_t stride, int i) { return p + stride * i; }
 
 // Per-op decode step: embedding, then per layer LayerNorm + rowgroup GEMVs, RoPE (v2), KV append and split attention.
-int run_chain_per_op(const DecodeChain& c, const int32_t* ids, int B, int nsplit, cudaStream_t st) {
+void run_chain_per_op(const DecodeChain& c, const int32_t* ids, int B, int nsplit, cudaStream_t st) {
   const int H = c.H, D = c.D, n = c.n_layer;
   if (ids) launch_embed_tokens(ids, c.wte, c.wpe, c.state, c.x, B, H, c.vocab, c.n_positions, st, c.rows);
   for (int i = 0; i < n; ++i) {
@@ -610,14 +626,13 @@ int run_chain_per_op(const DecodeChain& c, const int32_t* ids, int B, int nsplit
     launch_layernorm(slot(c.x, c.sx, 2 * n), c.lnf_w, c.lnf_b, lnf, B, H, c.ln_eps, H, st);
     launch_linear_rowgroup(lnf, c.lm_head, nullptr, nullptr, c.logits, B, c.vocab, H, SV_ACT_NONE, st);
   }
-  return SV_OK;
 }
 
 // Fused decode step: 5 kernels per layer (4 weight-ring GEMVs with fused LayerNorm / bias / GELU / residual / KV append,
 // 1 cluster attention) + lm_head, chained with programmatic dependent launch.  `ids` != nullptr embeds those tokens first
 // (teacher forcing / sampling); with nullptr, x[0] was already written (by select_fused).
 // Leaves bf16 logits and per-tile argmax partials in amax_*.
-int run_chain_fused(const DecodeChain& c, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st) {
+void run_chain_fused(const DecodeChain& c, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st) {
   const int H = c.H, D = c.D, n = c.n_layer;
   if (ids) launch_embed_tokens(ids, c.wte, c.wpe, c.state, c.x, B, H, c.vocab, c.n_positions, st, c.rows);
   bool first = true;
@@ -655,18 +670,76 @@ int run_chain_fused(const DecodeChain& c, const int32_t* ids, int B, int ncta, b
   if (c.lm_tail)
     gemv(slot(c.x, c.sx, 2 * n), c.lm_head, c.t_lm_head, nullptr, nullptr, c.logits, c.vocab, H, SV_ACT_NONE, c.lnf_w, c.lnf_b, 2,
          nullptr, nullptr, pdl);
+}
+
+// The attention partition of a decode step whose keys reach total_len: CTAs per image of the cluster kernel (fused chain)
+// or key splits of the split / merge kernels (per-op chain).
+int decode_parts(bool fused, int total_len) {
+  if (fused) return attention_decode_cluster_ncta(total_len);
+  return std::max(1, std::min(kMaxSplit, (total_len + 31) / 32));
+}
+
+void run_chain(const DecodeChain& c, bool fused, const int32_t* ids, int B, int parts, bool pdl, cudaStream_t st) {
+  if (fused) run_chain_fused(c, ids, B, parts, pdl, st);
+  else run_chain_per_op(c, ids, B, parts, st);
+}
+
+// The engine's step over its own buffers and caches.  rows != nullptr: a session step.  cmap != nullptr: a speculative
+// verify step, B columns of one cache row placed by the column map (fused chain, v1 only).
+void run_engine_step(sv_engine* e, const int32_t* ids, int B, int parts, bool pdl, cudaStream_t st,
+                     const RowState* rows = nullptr, const svspec::ColMap* cmap = nullptr) {
+  run_chain(engine_chain(e, rows, cmap), e->fused_decode, ids, B, parts, pdl, st);
+}
+
+// Captures `enqueue(pdl)` on `st` into g: the instantiated graph, its kernel count and whether the PDL capture was kept.
+// A PDL capture the driver refuses is retried once in plain stream order.  The launch counter active before is restored.
+template <typename Enqueue>
+cudaError_t capture_step(cudaStream_t st, bool try_pdl, const Enqueue& enqueue, GraphEntry& g) {
+  int64_t* const outer = g_launch_counter;
+  cudaError_t ce = cudaSuccess;
+  for (int attempt = try_pdl ? 0 : 1; attempt < 2; ++attempt) {
+    int64_t counted = 0;
+    g_launch_counter = &counted;
+    cudaGraph_t graph = nullptr;
+    ce = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
+    if (ce != cudaSuccess) break;
+    enqueue(attempt == 0);
+    ce = cudaStreamEndCapture(st, &graph);
+    if (ce == cudaSuccess) ce = cudaGraphInstantiate(&g.exec, graph, 0);
+    if (graph) cudaGraphDestroy(graph);
+    if (ce == cudaSuccess) {
+      g.kernels = (int)counted;
+      g.pdl = attempt == 0;
+      break;
+    }
+    g.exec = nullptr;
+    cudaGetLastError();
+  }
+  g_launch_counter = outer;
+  return ce;
+}
+
+// Replays the step graph n times on the engine's stream.
+int replay(sv_engine* e, const GraphEntry& g, int n) {
+  for (int i = 0; i < n; ++i) {
+    SV_CK(e, cudaGraphLaunch(g.exec, e->gen_stream));
+    e->launches += g.kernels;
+  }
   return SV_OK;
 }
 
-// The engine's steps: its own buffers and caches.  rows != nullptr: a session step.  cmap != nullptr: a speculative verify
-// step, B columns of one cache row placed by the column map (v1 only).
-int run_decode_layers(sv_engine* e, const int32_t* ids, int B, int nsplit, cudaStream_t st, const RowState* rows = nullptr) {
-  return run_chain_per_op(engine_chain(e, rows), ids, B, nsplit, st);
+// Reads n device words into host_flag once the engine's stream has reached this point.
+int read_flags(sv_engine* e, const int32_t* dev, int n) {
+  SV_CK(e, cudaMemcpyAsync(e->host_flag, dev, n * sizeof(int32_t), cudaMemcpyDeviceToHost, e->gen_stream));
+  SV_CK(e, cudaStreamSynchronize(e->gen_stream));
+  return SV_OK;
 }
 
-int run_decode_layers_fused(sv_engine* e, const int32_t* ids, int B, int ncta, bool pdl, cudaStream_t st,
-                            const RowState* rows = nullptr, const svspec::ColMap* cmap = nullptr) {
-  return run_chain_fused(engine_chain(e, rows, cmap), ids, B, ncta, pdl, st);
+// Orders the engine's stream after the work queued so far on the caller's.
+int join_caller(sv_engine* e, void* stream) {
+  SV_CK(e, cudaEventRecord(e->ev_in, (cudaStream_t)stream));
+  SV_CK(e, cudaStreamWaitEvent(e->gen_stream, e->ev_in, 0));
+  return SV_OK;
 }
 
 // (re)build the slab-tiled copies the dataflow kernel streams, after any weight changed
@@ -703,17 +776,22 @@ FlowLaunch flow_launch_desc(sv_engine* e, int B) {
   return m;
 }
 
-int nsplit_for(int total_len) {
-  int blocks = (total_len + 31) / 32;
-  return std::max(1, std::min(kMaxSplit, blocks));
-}
-
-void launch_select(sv_engine* e, int B, int do_sample, cudaStream_t st) {
-  if (do_sample)
-    launch_select_sample(e->logits, e->d.vocab, B, e->state, e->params, e->seen, e->next_ids, e->out_ids,
-                         e->logits_f32, st);
+// Token selection from `logits` [B][vocab]: sampling, or greedy through the fused kernel (which also embeds the next step's
+// input; `partials`: the lm_head left its argmax partials) on the fused decode path, or the plain greedy kernel.
+// rows != nullptr: the session variants, rows in `mask` only, row_len advanced by advance_len.  Without rows, the
+// sampling and plain greedy kernels leave the step bookkeeping to launch_gen_finalize.
+void launch_token_select(sv_engine* e, const bf16* logits, int B, bool sample, bool partials, int advance_len, bool pdl,
+                         cudaStream_t st, RowState* rows = nullptr, uint32_t mask = 0) {
+  const sv_model_desc& d = e->d;
+  if (sample)
+    launch_select_sample(logits, d.vocab, B, e->state, e->params, e->seen, e->next_ids, e->out_ids, e->logits_f32, st, rows,
+                         mask, advance_len);
+  else if (e->fused_decode)
+    launch_select_fused(logits, d.vocab, B, partials ? e->amax_val : nullptr, e->amax_idx, gemv_ring_ntiles(d.vocab),
+                        8 * ring_row_groups(B), e->state, e->params, e->seen, e->next_ids, e->out_ids, advance_len, e->wte,
+                        e->wpe, e->d_x, d.hidden, d.n_positions, pdl, st, rows, mask);
   else
-    launch_select_greedy(e->logits, e->d.vocab, B, e->state, e->params, e->seen, e->next_ids, e->out_ids, st);
+    launch_select_greedy(logits, d.vocab, B, e->state, e->params, e->seen, e->next_ids, e->out_ids, st, rows, mask, advance_len);
 }
 
 // Entry points that use the cache as one rectangle of rows refuse to run while a session holds per-row state in it.
@@ -908,9 +986,7 @@ void sv_engine_destroy(sv_engine* e) {
   if (!e) return;
   cudaSetDevice(e->device);
   cudaDeviceSynchronize();
-  for (auto& g : e->graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
-  for (auto& g : e->beam_graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
-  for (auto& g : e->spec_graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
+  for (auto& g : e->step_graphs) if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
   for (void* p : e->allocs) cudaFree(p);
   if (e->host_flag) cudaFreeHost(e->host_flag);
   if (e->host_stream) cudaFreeHost(e->host_stream);
@@ -1048,7 +1124,6 @@ int sv_decode_step(sv_engine* e, const int32_t* ids, float* logits, void* stream
   SV_CK(e, cudaSetDevice(e->device));
   LaunchScope scope(e);
   cudaStream_t st = (cudaStream_t)stream;
-  int r = SV_OK;
   if (e->use_flow) {
     // one token through the dataflow kernel: embed (plain) -> all layers -> logits, no selection
     const sv_model_desc& d = e->d;
@@ -1061,10 +1136,7 @@ int sv_decode_step(sv_engine* e, const int32_t* ids, float* logits, void* stream
     e->flow_epoch += 1;
     launch_advance_len(e->state, st);
   } else {
-    r = e->fused_decode
-            ? run_decode_layers_fused(e, ids, e->cur_batch, attention_decode_cluster_ncta(e->host_cur_len + 1), e->use_pdl, st)
-            : run_decode_layers(e, ids, e->cur_batch, nsplit_for(e->host_cur_len + 1), st);
-    if (r != SV_OK) return r;
+    run_engine_step(e, ids, e->cur_batch, decode_parts(e->fused_decode, e->host_cur_len + 1), e->use_pdl, st);
     launch_advance_len(e->state, st);
   }
   if (logits) launch_logits_to_float(e->logits, logits, (int64_t)e->cur_batch * e->d.vocab, st);
@@ -1109,6 +1181,14 @@ int sv_score_tokens(sv_engine* e, const int32_t* ids, int32_t batch, int32_t n_t
   return finish_prefill_impl(e, B, pos0 + n, nullptr, st);
 }
 
+// What every entry point checks in sv_gen_params: nullptr, or what is wrong.
+static const char* gen_params_error(const sv_gen_params& p) {
+  if (p.n_stop_ids < 0 || p.n_stop_ids > 8) return "n_stop_ids outside [0, 8]";
+  if (p.do_sample && !(p.temperature > 0.f)) return "temperature must be > 0";
+  if (!(p.repetition_penalty > 0.f)) return "repetition_penalty must be > 0";
+  return nullptr;
+}
+
 // The device-side generation parameters (n_stop_ids already checked to lie in [0, 8]).
 static GenParamsDev gen_params_dev(const sv_gen_params* p, int stop_row0_only, int out_stride) {
   GenParamsDev hp;
@@ -1136,9 +1216,7 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
   if (max_new < 1) return fail(e, SV_ERR_INVALID, "max_new_tokens must be >= 1");
   if (e->prefix_len + max_new > e->d.max_len)
     return fail(e, SV_ERR_INVALID, "prefix %d + max_new_tokens %d exceeds max_len %d", e->prefix_len, max_new, e->d.max_len);
-  if (p->n_stop_ids < 0 || p->n_stop_ids > 8) return fail(e, SV_ERR_INVALID, "n_stop_ids outside [0,8]");
-  if (p->do_sample && !(p->temperature > 0.f)) return fail(e, SV_ERR_INVALID, "temperature must be > 0");
-  if (!(p->repetition_penalty > 0.f)) return fail(e, SV_ERR_INVALID, "repetition_penalty must be > 0");
+  if (const char* bad = gen_params_error(*p)) return fail(e, SV_ERR_INVALID, "%s", bad);
   const int ncols = spec ? spec->num_tokens + 1 : 0;
   if (spec) {
     if (e->v2) return fail(e, SV_ERR_UNSUPPORTED, "sv_generate_speculative: v2 engines decode through the per-op kernels; only v1 is built");
@@ -1154,9 +1232,8 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
   LaunchScope scope(e);
   if (spec && !e->spec && dev_alloc(e, &e->spec, 1) != cudaSuccess)
     return fail(e, SV_ERR_CUDA, "allocation of the speculative decoding state failed: %s", cudaGetErrorString(cudaGetLastError()));
-  cudaStream_t caller = (cudaStream_t)stream, st = e->gen_stream;
-  SV_CK(e, cudaEventRecord(e->ev_in, caller));
-  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  cudaStream_t st = e->gen_stream;
+  SV_TRY(join_caller(e, stream));
 
   const GenParamsDev hp = gen_params_dev(p, p->stop_row0_only, e->d.max_len);
   SV_CK(e, cudaMemcpyAsync(e->params, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));
@@ -1167,17 +1244,9 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
   // HF stop rules and embeds the token for the first decode step.
   const bool fused = e->fused_decode;
   const bool fused_select = fused && !p->do_sample;
-  const int ntiles = gemv_ring_ntiles(e->d.vocab);
   auto select_step = [&](int advance_len, bool have_partials, bool pdl) {
-    if (fused_select) {
-      launch_select_fused(e->logits, e->d.vocab, B, have_partials ? e->amax_val : nullptr, e->amax_idx, ntiles,
-                          8 * ring_row_groups(B), e->state,
-                          e->params, e->seen, e->next_ids, e->out_ids, advance_len, e->wte, e->wpe, e->d_x, e->d.hidden,
-                          e->d.n_positions, pdl, st);
-    } else {
-      launch_select(e, B, p->do_sample, st);
-      launch_gen_finalize(e->state, e->params, B, advance_len, st);
-    }
+    launch_token_select(e, e->logits, B, p->do_sample, have_partials, advance_len, pdl, st);
+    if (!fused_select) launch_gen_finalize(e->state, e->params, B, advance_len, st);
   };
   select_step(/*advance_len=*/0, /*have_partials=*/false, /*pdl=*/false);
   if (spec) {   // nothing to accept yet (n_live = 0): the first drafts, the column map and the columns' embeddings
@@ -1189,49 +1258,30 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
                        e->d.hidden, e->d.n_positions, e->spec, false, st);
   }
 
-  const int nsplit = fused ? attention_decode_cluster_ncta(e->prefix_len + max_new) : nsplit_for(e->prefix_len + max_new);
-  const long long key = (long long)(spec ? ncols : B) * 100000 + nsplit * 8 + (p->do_sample ? 1 : 0) + (fused ? 2 : 0) +
-                        (e->use_pdl ? 4 : 0);
-  GraphEntry& ge = spec ? e->spec_graphs[key] : e->graphs[key];
+  const int parts = decode_parts(fused, e->prefix_len + max_new);
+  GraphEntry& ge = e->step_graphs[{spec ? StepKind::speculative : StepKind::generate, spec ? ncols : B, parts, p->do_sample != 0,
+                                   fused, e->use_pdl}];
   const bool flow = e->use_flow && fused_select && !spec;
-  if (!ge.exec && max_new > 1 && !flow) {
-    for (int attempt = 0; attempt < 2 && !ge.exec; ++attempt) {
-      const bool pdl = e->use_pdl && fused && attempt == 0;
-      int64_t counted = 0;
-      g_launch_counter = &counted;
-      cudaGraph_t graph = nullptr;
-      SV_CK(e, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      int r;
-      if (spec) {           // verify step: the columns' inputs were embedded by the previous accept
-        r = run_decode_layers_fused(e, nullptr, ncols, nsplit, pdl, st, nullptr, &e->spec->map);
-        if (fused_select) {
-          launch_select_fused_spec(e->logits, e->d.vocab, e->amax_val, e->amax_idx, ntiles, 8 * ring_row_groups(ncols),
-                                   e->state, e->params, e->seen, e->next_ids, e->out_ids, e->wte, e->wpe, e->d_x,
-                                   e->d.hidden, e->d.n_positions, e->spec, pdl, st);
-        } else {
-          launch_select_sample_spec(e->logits, e->d.vocab, ncols, e->state, e->params, e->seen, e->logits_f32, e->spec, st);
-          launch_spec_accept(e->state, e->params, e->seen, e->next_ids, e->out_ids, e->d.vocab, e->wte, e->wpe, e->d_x,
-                             e->d.hidden, e->d.n_positions, e->spec, false, st);
-        }
+  auto step = [&](bool pdl) {
+    if (spec) {           // verify step: the columns' inputs were embedded by the previous accept
+      run_engine_step(e, nullptr, ncols, parts, pdl, st, nullptr, &e->spec->map);
+      if (fused_select) {
+        launch_select_fused_spec(e->logits, e->d.vocab, e->amax_val, e->amax_idx, gemv_ring_ntiles(e->d.vocab),
+                                 8 * ring_row_groups(ncols), e->state, e->params, e->seen, e->next_ids, e->out_ids, e->wte,
+                                 e->wpe, e->d_x, e->d.hidden, e->d.n_positions, e->spec, pdl, st);
       } else {
-        if (fused) r = run_decode_layers_fused(e, fused_select ? nullptr : e->next_ids, B, nsplit, pdl, st);
-        else r = run_decode_layers(e, e->next_ids, B, nsplit, st);
-        select_step(/*advance_len=*/1, /*have_partials=*/fused, pdl);
+        launch_select_sample_spec(e->logits, e->d.vocab, ncols, e->state, e->params, e->seen, e->logits_f32, e->spec, st);
+        launch_spec_accept(e->state, e->params, e->seen, e->next_ids, e->out_ids, e->d.vocab, e->wte, e->wpe, e->d_x,
+                           e->d.hidden, e->d.n_positions, e->spec, false, st);
       }
-      cudaError_t ce = cudaStreamEndCapture(st, &graph);
-      g_launch_counter = &e->launches;
-      if (r != SV_OK) { if (graph) cudaGraphDestroy(graph); return r; }
-      if (ce == cudaSuccess) ce = cudaGraphInstantiate(&ge.exec, graph, 0);
-      if (graph) cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) {
-        ge.exec = nullptr;
-        cudaGetLastError();
-        if (!pdl) SV_CK(e, ce);          // plain capture failed: a real error
-        e->use_pdl = false;              // programmatic edges refused by this driver: plain stream order
-        continue;
-      }
-      ge.kernels = (int)counted;
+    } else {
+      run_engine_step(e, fused_select ? nullptr : e->next_ids, B, parts, pdl, st);
+      select_step(/*advance_len=*/1, /*have_partials=*/fused, pdl);
     }
+  };
+  if (!ge.exec && max_new > 1 && !flow) {
+    SV_CK(e, capture_step(st, e->use_pdl && fused, step, ge));
+    if (fused && !ge.pdl) e->use_pdl = false;     // programmatic edges refused by this driver: plain stream order
   }
 
   const int poll = p->poll_interval > 0 ? p->poll_interval : 16;
@@ -1251,13 +1301,12 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
     }
     return SV_OK;
   };
-  auto poll_device = [&](bool& done_flag) -> int {  // done flag (+ step count when streaming), then the new tokens
-    SV_CK(e, cudaMemcpyAsync(e->host_flag, &e->state->step, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));   // {step, done}
-    SV_CK(e, cudaStreamSynchronize(st));
+  auto poll_device = [&](bool& done_flag) -> int {  // {step, done} into host_flag, then the new tokens when streaming
+    SV_TRY(read_flags(e, &e->state->step, 2));
     done_flag = e->host_flag[1] != 0;
-    const int r = emit_upto(std::min(e->host_flag[0], max_new));
+    SV_TRY(emit_upto(std::min(e->host_flag[0], max_new)));
     if (cancelled) done_flag = true;
-    return r;
+    return SV_OK;
   };
   SV_CK(e, cudaEventRecord(e->ev_t0, st));
   int steps = 0;
@@ -1281,14 +1330,7 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
       e->flow_epoch += m.nsteps;
       left -= m.nsteps;
       steps += m.nsteps;
-      if (cb && left > 0) {
-        const int r = poll_device(done);
-        if (r != SV_OK) return r;
-      } else if (can_stop && left > 0) {
-        SV_CK(e, cudaMemcpyAsync(e->host_flag, &e->state->done, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        SV_CK(e, cudaStreamSynchronize(st));
-        done = e->host_flag[0] != 0;
-      }
+      if ((cb || can_stop) && left > 0) SV_TRY(poll_device(done));
     }
   }
   if (spec) {
@@ -1298,44 +1340,23 @@ static int generate_impl(sv_engine* e, const sv_gen_params* p, int32_t* out_ids,
     int known = 1;
     while (!done && known < max_new) {
       const int n_rep = std::max(1, std::min(poll, (max_new - known + ncols - 1) / ncols));
-      for (int i = 0; i < n_rep; ++i) {
-        SV_CK(e, cudaGraphLaunch(ge.exec, st));
-        e->launches += ge.kernels;
-        ++steps;
-      }
-      if (cb) {
-        const int r = poll_device(done);
-        if (r != SV_OK) return r;
-      } else {
-        SV_CK(e, cudaMemcpyAsync(e->host_flag, &e->state->step, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        SV_CK(e, cudaStreamSynchronize(st));
-        done = e->host_flag[1] != 0;
-      }
+      SV_TRY(replay(e, ge, n_rep));
+      steps += n_rep;
+      SV_TRY(poll_device(done));
       known = e->host_flag[0];
     }
   }
+  // with neither a callback, an EOS nor a stop sequence armed, no host read and no sync until the end
   for (int s = 1; s < max_new && !done && !flow && !spec; ++s) {
-    SV_CK(e, cudaGraphLaunch(ge.exec, st));
-    e->launches += ge.kernels;
+    SV_TRY(replay(e, ge, 1));
     ++steps;
-    if (cb && (s % poll == 0)) {
-      const int r = poll_device(done);
-      if (r != SV_OK) return r;
-    } else if (can_stop && (s % poll == 0)) {
-      SV_CK(e, cudaMemcpyAsync(e->host_flag, &e->state->done, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-      SV_CK(e, cudaStreamSynchronize(st));
-      done = e->host_flag[0] != 0;
-    }
+    if ((cb || can_stop) && s % poll == 0) SV_TRY(poll_device(done));
   }
   SV_CK(e, cudaEventRecord(e->ev_t1, st));
   // rectangular result: [B, n_generated] new tokens, padded (HF returns the same rectangle)
-  SV_CK(e, cudaMemcpyAsync(e->host_flag, &e->state->step, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  SV_CK(e, cudaStreamSynchronize(st));
+  SV_TRY(read_flags(e, &e->state->step, 1));
   const int n_gen = std::min(e->host_flag[0], max_new);
-  if (cb) {
-    const int r = emit_upto(n_gen);
-    if (r != SV_OK) return r;
-  }
+  SV_TRY(emit_upto(n_gen));
   SV_CK(e, cudaMemcpy2DAsync(out_ids, (size_t)max_new * 4, e->out_ids, (size_t)e->d.max_len * 4, (size_t)max_new * 4, B,
                              cudaMemcpyDeviceToDevice, st));
   if (out_len) launch_fill_i32(out_len, n_gen, B, st);
@@ -1401,9 +1422,7 @@ int sv_spec_verify_step(sv_engine* e, const int32_t* ids_host, int32_t ncols, fl
   SV_CK(e, cudaMemcpyAsync(e->spec_pos, &rs, sizeof(rs), cudaMemcpyHostToDevice, st));
   SV_CK(e, cudaMemcpyAsync(e->ids_tmp, ids_host, (size_t)ncols * 4, cudaMemcpyHostToDevice, st));
   launch_embed_tokens(e->ids_tmp, e->wte, e->wpe, e->state, e->d_x, ncols, d.hidden, d.vocab, d.n_positions, st, e->spec_pos);
-  const int r = run_decode_layers_fused(e, nullptr, ncols, attention_decode_cluster_ncta(e->host_cur_len + ncols), false, st,
-                                        nullptr, &e->spec->map);
-  if (r != SV_OK) return r;
+  run_engine_step(e, nullptr, ncols, decode_parts(true, e->host_cur_len + ncols), false, st, nullptr, &e->spec->map);
   launch_logits_to_float(e->logits, logits, (int64_t)ncols * d.vocab, st);
   SV_CK(e, cudaStreamSynchronize(st));
   SV_CK(e, cudaGetLastError());
@@ -1523,9 +1542,8 @@ int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_
 #undef BAL
     if (!ok) { e->beam_state = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the beam-search state failed: %s", cudaGetErrorString(cudaGetLastError())); }
   }
-  cudaStream_t caller = (cudaStream_t)stream, st = e->gen_stream;
-  SV_CK(e, cudaEventRecord(e->ev_in, caller));
-  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  cudaStream_t st = e->gen_stream;
+  SV_TRY(join_caller(e, stream));
 
   const svbeam::Params hp = beam_params_dev(bp, batch, d.vocab, stride);
   svbeam::State hs;
@@ -1548,46 +1566,26 @@ int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_
   };
   bookkeeping(/*advance=*/0);                       // step 0: candidates from the prefill logits
 
-  const int nsplit = fused ? attention_decode_cluster_ncta(e->prefix_len + max_new) : nsplit_for(e->prefix_len + max_new);
-  const long long key = (long long)R * 100000 + nsplit * 8 + (fused ? 2 : 0) + (e->use_pdl ? 4 : 0);
-  GraphEntry& ge = e->beam_graphs[key];
+  const int parts = decode_parts(fused, e->prefix_len + max_new);
+  // beam sampling is read from the device parameters: the same graph serves both
+  GraphEntry& ge = e->step_graphs[{StepKind::beam, R, parts, false, fused, e->use_pdl}];
+  auto step = [&](bool pdl) {
+    run_engine_step(e, fused ? nullptr : e->next_ids, R, parts, pdl, st);
+    bookkeeping(/*advance=*/1);
+  };
   if (!ge.exec && max_new > 1) {
-    for (int attempt = 0; attempt < 2 && !ge.exec; ++attempt) {
-      const bool pdl = e->use_pdl && fused && attempt == 0;
-      int64_t counted = 0;
-      g_launch_counter = &counted;
-      cudaGraph_t graph = nullptr;
-      SV_CK(e, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      int r;
-      if (fused) r = run_decode_layers_fused(e, nullptr, R, nsplit, pdl, st);
-      else r = run_decode_layers(e, e->next_ids, R, nsplit, st);
-      bookkeeping(/*advance=*/1);
-      cudaError_t ce = cudaStreamEndCapture(st, &graph);
-      g_launch_counter = &e->launches;
-      if (r != SV_OK) { if (graph) cudaGraphDestroy(graph); return r; }
-      if (ce == cudaSuccess) ce = cudaGraphInstantiate(&ge.exec, graph, 0);
-      if (graph) cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) {
-        ge.exec = nullptr;
-        cudaGetLastError();
-        if (!pdl) SV_CK(e, ce);
-        e->use_pdl = false;
-        continue;
-      }
-      ge.kernels = (int)counted;
-    }
+    SV_CK(e, capture_step(st, e->use_pdl && fused, step, ge));
+    if (fused && !ge.pdl) e->use_pdl = false;
   }
   const int poll = bp->poll_interval > 0 ? bp->poll_interval : 16;
   SV_CK(e, cudaEventRecord(e->ev_t0, st));
   int steps = 0;
   bool done = false;
   for (int s = 1; s < max_new && !done; ++s) {
-    SV_CK(e, cudaGraphLaunch(ge.exec, st));
-    e->launches += ge.kernels;
+    SV_TRY(replay(e, ge, 1));
     ++steps;
     if (s % poll == 0) {
-      SV_CK(e, cudaMemcpyAsync(e->host_flag, &e->beam_state->done, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-      SV_CK(e, cudaStreamSynchronize(st));
+      SV_TRY(read_flags(e, &e->beam_state->done, 1));
       done = e->host_flag[0] != 0;
     }
   }
@@ -1668,9 +1666,7 @@ int sv_session_begin(sv_engine* e, const sv_gen_params* p, int32_t slots) {
   if (slots < 1 || slots > e->d.max_batch) return fail(e, SV_ERR_INVALID, "slots %d outside [1,%d]", slots, e->d.max_batch);
   if (p->max_new_tokens < 1 || p->max_new_tokens > e->d.max_len)
     return fail(e, SV_ERR_INVALID, "max_new_tokens %d outside [1,%d]", p->max_new_tokens, e->d.max_len);
-  if (p->n_stop_ids < 0 || p->n_stop_ids > 8) return fail(e, SV_ERR_INVALID, "n_stop_ids outside [0,8]");
-  if (p->do_sample && !(p->temperature > 0.f)) return fail(e, SV_ERR_INVALID, "temperature must be > 0");
-  if (!(p->repetition_penalty > 0.f)) return fail(e, SV_ERR_INVALID, "repetition_penalty must be > 0");
+  if (const char* bad = gen_params_error(*p)) return fail(e, SV_ERR_INVALID, "%s", bad);
   int r = check_ready(e);
   if (r != SV_OK) return r;
   SV_CK(e, cudaSetDevice(e->device));
@@ -1728,9 +1724,8 @@ int sv_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t*
   }
   SV_CK(e, cudaSetDevice(e->device));
   LaunchScope scope(e);
-  cudaStream_t caller = (cudaStream_t)stream, st = e->gen_stream;
-  SV_CK(e, cudaEventRecord(e->ev_in, caller));
-  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  cudaStream_t st = e->gen_stream;
+  SV_TRY(join_caller(e, stream));
   const int64_t img = (int64_t)3 * d.image_size * d.image_size, row_stride = (int64_t)d.n_kv_head * e->tcap * d.head_dim;
   const size_t lrow = (size_t)d.vocab * sizeof(bf16);
   uint32_t mask = 0;
@@ -1774,15 +1769,8 @@ int sv_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t*
   }
   launch_session_admit(e->rows, adm, e->seen, d.vocab, e->out_ids, d.max_len, e->sess_p.pad_token_id, st);
   // token 0 of the admitted slots from their prefill logits (generate_impl's first select, no position advance)
-  if (e->sess_p.do_sample)
-    launch_select_sample(e->sess_logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, e->logits_f32, st,
-                         e->rows, mask, 0);
-  else if (e->fused_decode)
-    launch_select_fused(e->sess_logits, d.vocab, S, nullptr, e->amax_idx, gemv_ring_ntiles(d.vocab), 8 * ring_row_groups(S),
-                        e->state, e->params, e->seen, e->next_ids, e->out_ids, 0, e->wte, e->wpe, e->d_x, d.hidden,
-                        d.n_positions, false, st, e->rows, mask);
-  else
-    launch_select_greedy(e->sess_logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, st, e->rows, mask, 0);
+  launch_token_select(e, e->sess_logits, S, e->sess_p.do_sample, /*partials=*/false, /*advance_len=*/0, /*pdl=*/false, st,
+                      e->rows, mask);
   SV_CK(e, cudaGetLastError());
   SV_CK(e, cudaStreamSynchronize(st));     // the caller may release pixels / prompt_ids on return
   for (int j = 0; j < k; ++j) e->sess_live[slots_host[j]] = 1;
@@ -1796,75 +1784,37 @@ int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int3
   if (max_steps < 0) return fail(e, SV_ERR_INVALID, "max_steps must be >= 0");
   SV_CK(e, cudaSetDevice(e->device));
   LaunchScope scope(e);
-  const sv_model_desc& d = e->d;
   const int S = e->sess_slots;
-  cudaStream_t caller = (cudaStream_t)stream, st = e->gen_stream;
-  SV_CK(e, cudaEventRecord(e->ev_in, caller));
-  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  cudaStream_t st = e->gen_stream;
+  SV_TRY(join_caller(e, stream));
   // the select kernels raise RowState::event when a row finishes (at admission too: a first token may end a row), so a
   // poll reads that one word; the per-row fields are read once, at the end, and the event is cleared with them
-  auto poll_event = [&](bool& fin) -> int {
-    SV_CK(e, cudaMemcpyAsync(&e->rows_host->event, &e->rows->event, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    SV_CK(e, cudaStreamSynchronize(st));
-    fin = e->rows_host->event != 0;
-    return SV_OK;
-  };
-  bool any_live = false, any_fin = false;
+  bool any_live = false;
   for (int s = 0; s < S; ++s) any_live = any_live || e->sess_live[s];
-  int r = poll_event(any_fin);
-  if (r != SV_OK) return r;
+  SV_TRY(read_flags(e, &e->rows->event, 1));
+  bool any_fin = e->host_flag[0] != 0;
   int steps = 0;
   if (!any_fin && any_live && max_steps > 0) {
     ensure_flow_tiles(e, st);    // (no-op unless a weight was loaded since the tiles were built)
-    const bool fused = e->fused_decode, fused_select = fused && !e->sess_p.do_sample;
+    const bool fused = e->fused_decode, sample = e->sess_p.do_sample != 0;
     const int total = e->Q + e->sess_prompt_len + e->sess_p.max_new_tokens;     // the session cap fixes the split count
-    const int nsplit = fused ? attention_decode_cluster_ncta(total) : nsplit_for(total);
-    const long long key = (1LL << 40) + (long long)S * 100000 + nsplit * 8 + (e->sess_p.do_sample ? 1 : 0) + (fused ? 2 : 0) +
-                          (e->use_pdl ? 4 : 0);
-    GraphEntry& ge = e->graphs[key];
-    for (int attempt = 0; attempt < 2 && !ge.exec; ++attempt) {
-      const bool pdl = e->use_pdl && fused && attempt == 0;
-      int64_t counted = 0;
-      g_launch_counter = &counted;
-      cudaGraph_t graph = nullptr;
-      SV_CK(e, cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      int rr;
-      if (fused) rr = run_decode_layers_fused(e, fused_select ? nullptr : e->next_ids, S, nsplit, pdl, st, e->rows);
-      else rr = run_decode_layers(e, e->next_ids, S, nsplit, st, e->rows);
-      const uint32_t all = (1u << S) - 1u;
-      if (fused_select)
-        launch_select_fused(e->logits, d.vocab, S, e->amax_val, e->amax_idx, gemv_ring_ntiles(d.vocab), 8 * ring_row_groups(S),
-                            e->state, e->params, e->seen, e->next_ids, e->out_ids, 1, e->wte, e->wpe, e->d_x, d.hidden,
-                            d.n_positions, pdl, st, e->rows, all);
-      else if (e->sess_p.do_sample)
-        launch_select_sample(e->logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, e->logits_f32, st,
-                             e->rows, all, 1);
-      else
-        launch_select_greedy(e->logits, d.vocab, S, e->state, e->params, e->seen, e->next_ids, e->out_ids, st, e->rows, all, 1);
-      cudaError_t ce = cudaStreamEndCapture(st, &graph);
-      g_launch_counter = &e->launches;
-      if (rr != SV_OK) { if (graph) cudaGraphDestroy(graph); return rr; }
-      if (ce == cudaSuccess) ce = cudaGraphInstantiate(&ge.exec, graph, 0);
-      if (graph) cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) {
-        ge.exec = nullptr;
-        cudaGetLastError();
-        if (!pdl) SV_CK(e, ce);
-        e->use_pdl = false;
-        continue;
-      }
-      ge.kernels = (int)counted;
+    const int parts = decode_parts(fused, total);
+    GraphEntry& ge = e->step_graphs[{StepKind::session, S, parts, sample, fused, e->use_pdl}];
+    auto step = [&](bool pdl) {
+      run_engine_step(e, fused && !sample ? nullptr : e->next_ids, S, parts, pdl, st, e->rows);
+      launch_token_select(e, e->logits, S, sample, /*partials=*/true, /*advance_len=*/1, pdl, st, e->rows, (1u << S) - 1u);
+    };
+    if (!ge.exec) {
+      SV_CK(e, capture_step(st, e->use_pdl && fused, step, ge));
+      if (fused && !ge.pdl) e->use_pdl = false;
     }
     const int every = e->sess_p.poll_interval > 0 ? e->sess_p.poll_interval : 16;
     while (steps < max_steps && !any_fin && any_live) {
       const int n = std::min(every, max_steps - steps);
-      for (int i = 0; i < n; ++i) {
-        SV_CK(e, cudaGraphLaunch(ge.exec, st));
-        e->launches += ge.kernels;
-      }
+      SV_TRY(replay(e, ge, n));
       steps += n;
-      r = poll_event(any_fin);
-      if (r != SV_OK) return r;
+      SV_TRY(read_flags(e, &e->rows->event, 1));
+      any_fin = e->host_flag[0] != 0;
     }
   }
   {
@@ -1891,8 +1841,7 @@ int sv_session_read(sv_engine* e, int32_t slot, int32_t* ids, void* stream) {
   if (slot < 0 || slot >= e->sess_slots) return fail(e, SV_ERR_INVALID, "slot %d outside [0,%d)", slot, e->sess_slots);
   SV_CK(e, cudaSetDevice(e->device));
   cudaStream_t st = e->gen_stream;
-  SV_CK(e, cudaEventRecord(e->ev_in, (cudaStream_t)stream));
-  SV_CK(e, cudaStreamWaitEvent(st, e->ev_in, 0));
+  SV_TRY(join_caller(e, stream));
   const int n = e->sess_len[slot];
   if (n > 0) SV_CK(e, cudaMemcpyAsync(ids, e->out_ids + (int64_t)slot * e->d.max_len, (size_t)n * 4, cudaMemcpyDefault, st));
   SV_CK(e, cudaStreamSynchronize(st));
@@ -2403,7 +2352,7 @@ int sv_op_decode_chain(sv_op_chain* args, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   int total = 0;
   for (int b = 0; b < B; ++b) total = std::max(total, o.pos_host[b] + 1);
-  const int parts = o.parts ? o.parts : fused ? attention_decode_cluster_ncta(total) : nsplit_for(total);
+  const int parts = o.parts ? o.parts : decode_parts(fused, total);
   std::vector<DecLayer> layers(o.n_layer);
   for (int l = 0; l < o.n_layer; ++l) {
     const sv_op_chain_layer& s = o.layers[l];
@@ -2460,45 +2409,26 @@ int sv_op_decode_chain(sv_op_chain* args, void* stream) {
   c.x = (bf16*)o.x; c.ln = (bf16*)o.ln; c.qkv = (bf16*)o.qkv; c.attn = (bf16*)o.attn; c.h = (bf16*)o.h;
   c.sx = o.x_stride; c.sln = o.ln_stride; c.sqkv = o.qkv_stride; c.sattn = o.attn_stride; c.sh = o.h_stride;
   c.lm_tail = o.lm_head_tail != 0; c.logits = (bf16*)o.logits; c.amax_val = o.amax_val; c.amax_idx = o.amax_idx;
-  auto run = [&](bool pdl, cudaStream_t s) {
-    return fused ? run_chain_fused(c, o.ids, B, parts, pdl, s) : run_chain_per_op(c, o.ids, B, parts, s);
-  };
   if (o.per_row) r = cudaMemcpyAsync(buf, &rs, sizeof(rs), cudaMemcpyHostToDevice, st);
   else r = cudaMemcpyAsync(buf, &gs, sizeof(gs), cudaMemcpyHostToDevice, st);
   if (r == cudaSuccess) r = gemv_ring_init();
   if (r == cudaSuccess) r = attention_decode_cluster_init();
   bool pdl_used = false;
   if (r == cudaSuccess && !o.graph) {
-    run(fused && o.pdl, st);
+    run_chain(c, fused, o.ids, B, parts, fused && o.pdl, st);
     pdl_used = fused && o.pdl;
     r = cudaGetLastError();
   } else if (r == cudaSuccess) {
-    // the capture goes to a stream of its own (the caller's may be the legacy stream, which cannot be captured); a PDL
-    // capture the driver refuses is retried in plain stream order, as generate does
+    // the capture goes to a stream of its own (the caller's may be the legacy stream, which cannot be captured)
     cudaStream_t cs = nullptr;
+    GraphEntry g;
     r = cudaStreamSynchronize(st);
     if (r == cudaSuccess) r = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
-    cudaGraphExec_t exec = nullptr;
-    for (int attempt = 0; r == cudaSuccess && attempt < 2 && !exec; ++attempt) {
-      const bool pdl = fused && o.pdl && attempt == 0;
-      cudaGraph_t graph = nullptr;
-      r = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-      if (r != cudaSuccess) break;
-      run(pdl, cs);
-      cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-      if (ce == cudaSuccess) ce = cudaGraphInstantiate(&exec, graph, 0);
-      if (graph) cudaGraphDestroy(graph);
-      if (ce != cudaSuccess) {
-        exec = nullptr;
-        cudaGetLastError();
-        if (!pdl) r = ce;
-        continue;
-      }
-      pdl_used = pdl;
-    }
-    if (r == cudaSuccess) r = cudaGraphLaunch(exec, cs);
+    if (r == cudaSuccess) r = capture_step(cs, fused && o.pdl, [&](bool pdl) { run_chain(c, fused, o.ids, B, parts, pdl, cs); }, g);
+    if (r == cudaSuccess) r = cudaGraphLaunch(g.exec, cs);
     if (r == cudaSuccess) r = cudaStreamSynchronize(cs);
-    if (exec) cudaGraphExecDestroy(exec);
+    pdl_used = g.pdl;
+    if (g.exec) cudaGraphExecDestroy(g.exec);
     if (cs) cudaStreamDestroy(cs);
   }
   if (r == cudaSuccess) r = cudaStreamSynchronize(st);
@@ -2557,10 +2487,9 @@ int sv_op_decode_flow(sv_op_flow* args, void* stream) {
   else if (!al(o.xa) || !al(o.xb) || !al(o.qkv) || !al(o.att) || !al(o.hb) || !al(o.part) || !al(o.amax))
     bad = "the exchange buffers must be 16-byte aligned";
   else if (o.layer_stride < (int64_t)B * o.n_kv * o.tcap * D || o.layer_stride % 8) bad = "layer_stride < B * n_kv * tcap * 128 or not a multiple of 8";
-  else if (!(p.repetition_penalty > 0.f)) bad = "repetition_penalty must be > 0";
+  else if ((bad = gen_params_error(p))) {}
   else if (o.do_select) {
     if (p.do_sample) bad = "the dataflow kernel selects greedily: do_sample must be 0";
-    else if (p.n_stop_ids < 0 || p.n_stop_ids > 8) bad = "n_stop_ids outside [0, 8]";
     else if (!o.seen || !o.out_ids || !o.next_ids || !o.counters_host || !o.unfinished_host)
       bad = "do_select needs seen, out_ids, next_ids, counters_host and unfinished_host";
     else if (o.out_stride < 1) bad = "out_stride < 1";
@@ -2688,8 +2617,7 @@ int sv_op_select(const sv_op_select_args* args, void* stream) {
   else if (o.advance_len != 0 && o.advance_len != 1) bad = "advance_len is 0 or 1";
   else if (sampling && !(p.temperature > 0.f)) bad = "temperature must be > 0";
   else if (sampling && !(p.top_p > 0.f && p.top_p <= 1.f)) bad = "top_p not in (0, 1]";
-  else if (!(p.repetition_penalty > 0.f)) bad = "repetition_penalty must be > 0";
-  else if (p.n_stop_ids < 0 || p.n_stop_ids > 8) bad = "n_stop_ids outside [0, 8]";
+  else if ((bad = gen_params_error(p))) {}
   else if (!o.per_row) {
     if (!o.counters_host || !o.unfinished_host) bad = "per_row = 0 needs counters_host and unfinished_host";
     else if (o.counters_host[0] < 0 || o.counters_host[1] < 0) bad = "step and cur_len must be >= 0";
@@ -2788,8 +2716,7 @@ int sv_op_spec_select(const sv_op_spec_args* args, void* stream) {
   else if (o.vocab < 1) bad = "vocab < 1";
   else if (o.impl == SV_SPEC_SAMPLE && !(p.temperature > 0.f)) bad = "temperature must be > 0";
   else if (o.impl == SV_SPEC_SAMPLE && !(p.top_p > 0.f && p.top_p <= 1.f)) bad = "top_p not in (0, 1]";
-  else if (!(p.repetition_penalty > 0.f)) bad = "repetition_penalty must be > 0";
-  else if (p.n_stop_ids < 0 || p.n_stop_ids > 8) bad = "n_stop_ids outside [0, 8]";
+  else if ((bad = gen_params_error(p))) {}
   else if (p.max_new_tokens < 1 || p.max_new_tokens > o.out_stride) bad = "max_new_tokens not in [1, out_stride]";
   else if (o.gen_host[0] < 1 || o.gen_host[0] >= o.out_stride) bad = "step (the history's length) not in [1, out_stride)";
   else if (o.gen_host[1] < 0 || o.gen_host[1] >= o.n_positions) bad = "cur_len not in [0, n_positions - 1]";
