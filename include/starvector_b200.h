@@ -263,8 +263,8 @@ SV_API int sv_spec_accept_host(const sv_gen_params* p, int32_t* state, int32_t* 
  * shape) then continues.  Every request gets the tokens a one-image sv_generate with the same parameters gives
  * (greedy and sampling, bit for bit), up to and including its stop.  While a session is open, sv_encode_images,
  * sv_prefill*, sv_decode_step, sv_score_tokens, sv_generate*, sv_beam_search, sv_reorder_cache, sv_expand_batch and
- * sv_engine_load_weight return SV_ERR_STATE.  The session runs the CUDA-graph decode path (never the SV_FLOW dataflow kernel); beam search has
- * no session form.
+ * sv_engine_load_weight return SV_ERR_STATE.  The session runs the CUDA-graph decode path (never the SV_FLOW dataflow kernel).
+ * Beam search has its own session form (sv_beam_session_begin / sv_beam_session_admit below).
  *
  * sv_session_begin: p = the session's generation parameters: max_new_tokens is the session cap (it fixes the decode
  * attention's split count together with the prompt length, as prefix + max_new_tokens does in sv_generate), eos, stop ids
@@ -288,6 +288,26 @@ SV_API int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_hos
 SV_API int sv_session_read(sv_engine* e, int32_t slot, int32_t* ids, void* stream);
 /* Close the session: the rectangle-batch entry points work again (after a new prefill). */
 SV_API int sv_session_end(sv_engine* e);
+/* Beam sessions: continuous batching of sv_beam_search.  The `slots` cache rows form slots / num_beams groups; group g owns
+ * rows [g * num_beams, (g + 1) * num_beams) and runs one image's beam search (beam-sample with do_sample) with its own
+ * token cap and seed, while the other groups keep decoding.  A request whose cap equals the session cap gets the token ids
+ * and length the one-image sv_beam_search (after a prefill of the image repeated num_beams times) returns with the same
+ * parameters, bit for bit; a smaller cap gets the same as the one-image search at that cap when the decode attention's
+ * partition of prefix + cap equals that of prefix + session cap.  sv_session_run, sv_session_read and sv_session_end serve
+ * beam sessions: the run reports a finished group at its first slot, sv_session_read(first slot) returns its best
+ * hypothesis.  sv_session_admit is refused in a beam session, sv_beam_session_admit in a plain one.
+ *
+ * sv_beam_session_begin: p->max_new_tokens is the session cap; num_beams >= 2, slots a multiple of num_beams, <= max_batch.
+ * p->seed is the default seed of admitted groups.  SV_ERR_UNSUPPORTED when a logits row does not fit the candidate kernel. */
+SV_API int sv_beam_session_begin(sv_engine* e, const sv_beam_params* p, int32_t slots);
+/* Encode and prefill k images into free groups: pixels bf16 [k,3,S,S] and prompt_ids int32 [k,prompt_len] (device);
+ * groups_host int32 [k] the groups to fill; max_new_host int32 [k] (NULL = the session cap, else in [1, cap]); seeds_host
+ * uint64 [k] (NULL = the session seed).  Each image is encoded and prefilled repeated num_beams times, as a one-image
+ * beam search does, and the search's first step runs here.  The prompt length is fixed by the first admission; prefix +
+ * cap <= max_len.  Synchronises `stream`. */
+SV_API int sv_beam_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t* prompt_ids, int32_t prompt_len,
+                                 const int32_t* groups_host, const int32_t* max_new_host, const uint64_t* seeds_host,
+                                 void* stream);
 
 /* ---- introspection for bench/profiles ------------------------------------------------- */
 /* Kernel launches issued by this engine since creation (graph replays count their nodes). */

@@ -211,6 +211,8 @@ SIGNATURES = {
     "sv_session_run": (C.c_int, [_P, _I, _P, _P, _P]),
     "sv_session_read": (C.c_int, [_P, _I, _P, _P]),
     "sv_session_end": (C.c_int, [_P]),
+    "sv_beam_session_begin": (C.c_int, [_P, C.POINTER(BeamParams), _I]),
+    "sv_beam_session_admit": (C.c_int, [_P, _P, _I, _P, _I, _P, _P, _P, _P]),
     "sv_launch_count": (C.c_int64, [_P]),
     "sv_engine_describe": (C.c_char_p, [_P]),
     "sv_debug_read_timeline": (C.c_int, [_P, C.POINTER(C.c_longlong), _I]),

@@ -6,8 +6,9 @@ it.  Running a large workload as groups of `max_batch` rows makes every group as
 and prefilled into that slot while the other slots keep their caches, and the replayed decode graph continues.
 
 `ContinuousScheduler` is the host side: a FIFO queue of requests and a free-slot list.  It only talks to the engine
-through `session_begin / session_admit / session_run / session_read / session_end`, so it can be driven by a stand-in
-engine on a machine without a GPU.
+through `session_begin / session_admit / session_run / session_read / session_end` (beam sessions: `beam_session_begin /
+beam_session_admit` and the same run / read / end), so it can be driven by a stand-in engine on a machine without a GPU.
+With `num_beams > 1` the unit of admission is a group of `num_beams` contiguous slots that runs one image's beam search.
 """
 from __future__ import annotations
 
@@ -27,11 +28,14 @@ class ContinuousScheduler:
     every completion, the number of decode steps the session had run when it was admitted (while two rows decode side
     by side, their context lengths differ by the difference of their admit steps)."""
 
-    def __init__(self, engine, slots: Optional[int] = None):
+    def __init__(self, engine, slots: Optional[int] = None, num_beams: int = 1):
         self.engine = engine
         self.slots = int(slots if slots is not None else engine.dims.max_batch)
+        self.num_beams = int(num_beams)
         if not 1 <= self.slots <= engine.dims.max_batch:
             raise ValueError(f"slots {self.slots} outside [1, {engine.dims.max_batch}]")
+        if self.num_beams < 1 or self.slots % self.num_beams:
+            raise ValueError(f"slots {self.slots} must be a multiple of num_beams {self.num_beams}")
         self.stats = {}
 
     def run(self, pixels: torch.Tensor, prompt_ids: torch.Tensor, params, *, max_new_tokens: Optional[Sequence[int]] = None,
@@ -40,10 +44,15 @@ class ContinuousScheduler:
         """pixels `[N, 3, S, S]`; prompt_ids `[P]` (shared) or `[N, P]`; params: the session's `GenerationParams` (its
         `max_new_tokens` is the session cap).  `max_new_tokens`: one cap per image, each in [1, params.max_new_tokens].
         `seeds`: one per completion (default `params.seed + k` for completion k = i * n + j).  Returns one int32 tensor per
-        completion, in request order (index i * n + j); `on_finish(index, ids)` is called as each one completes."""
+        completion, in request order (index i * n + j); `on_finish(index, ids)` is called as each one completes.
+        With `num_beams > 1`, params is a `BeamSearchParams` of that width and every image is one request (n = 1) whose
+        result is its best hypothesis."""
         N = int(pixels.shape[0])
         n = int(n)
         cap = int(params.max_new_tokens)
+        nb = self.num_beams
+        if nb > 1 and (n != 1 or int(params.num_beams) != nb):
+            raise ValueError(f"a beam session of width {nb} takes one request per image and params with num_beams = {nb}")
         if n < 1 or n > self.slots:
             raise ValueError(f"n = {n} completions per image must be in [1, {self.slots}] (the session's slots)")
         if prompt_ids.dim() == 1:
@@ -62,16 +71,19 @@ class ContinuousScheduler:
 
         eng = self.engine
         queue = collections.deque(range(N))
-        free = list(range(self.slots))
-        owner = {}                                   # slot -> completion index
+        free = list(range(0, self.slots, nb))       # free units: slots, or the first slots of free beam groups
+        owner = {}                                   # (first) slot -> completion index
         results: List[Optional[torch.Tensor]] = [None] * (N * n)
         admit_step = [0] * (N * n)
         steps = admissions = 0
         t_admit = t_decode = 0.0
-        eng.session_begin(params, self.slots)
+        if nb > 1:
+            eng.beam_session_begin(params, self.slots)
+        else:
+            eng.session_begin(params, self.slots)
         try:
             while queue or owner:
-                # FIFO admission: as many queued images as there are free slots for all their completions
+                # FIFO admission: as many queued images as there are free units for all their completions
                 batch = []
                 while queue and len(free) >= n:
                     i = queue.popleft()
@@ -85,7 +97,11 @@ class ContinuousScheduler:
                             owner[s] = i * n + j
                             admit_step[i * n + j] = steps
                     t0 = time.perf_counter()
-                    eng.session_admit(pixels[imgs], prompt_ids[imgs], slots, max_new_tokens=mx, seeds=sd, src=src)
+                    if nb > 1:
+                        eng.beam_session_admit(pixels[imgs], prompt_ids[imgs], [s // nb for s in slots], max_new_tokens=mx,
+                                               seeds=sd)
+                    else:
+                        eng.session_admit(pixels[imgs], prompt_ids[imgs], slots, max_new_tokens=mx, seeds=sd, src=src)
                     t_admit += time.perf_counter() - t0
                     admissions += 1
                 t0 = time.perf_counter()

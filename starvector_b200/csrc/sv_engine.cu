@@ -48,7 +48,7 @@ struct DecLayer { bf16 *ln1_w, *ln1_b, *attn_w, *attn_b, *proj_w, *proj_b, *ln2_
 // The decode-step graphs of generate, speculative generate, beam search and sessions share one cache.  Two captures that
 // enqueue different kernels or arguments must never share a key: `rows` is the batch, the verify step's columns or the
 // session's slots, `parts` the attention partition (decode_parts).
-enum class StepKind { generate, speculative, beam, session };
+enum class StepKind { generate, speculative, beam, session, beam_session };
 struct StepKey {
   StepKind kind;
   int rows, parts;
@@ -112,7 +112,8 @@ struct sv_engine {
   bool tiles_dirty = true;
   int flow_epoch = 0;               // phase-tag epoch: steps run through the flow kernel since the buffers were cleared
   bf16 *kscratch = nullptr, *vscratch = nullptr;   // one layer of cache, for beam-search reorders
-  // device-resident beam search (sv_beam.cu), allocated by the first sv_beam_search call
+  // device-resident beam search (sv_beam.cu), allocated by the first sv_beam_search or beam session (beam_alloc).  Params,
+  // State and Plan hold one entry per group of a beam session (kMaxRows / 2); sv_beam_search uses the first
   svbeam::Params* beam_params = nullptr;
   svbeam::State* beam_state = nullptr;
   svbeam::Plan* beam_plan = nullptr;
@@ -156,6 +157,12 @@ struct sv_engine {
   bf16* sess_logits = nullptr;               // [max_batch][vocab]: the prefill logits of admitted slots (token 0 is read there)
   std::vector<int> sess_live;                // host: slot holds a request whose finish was not reported yet
   std::vector<int> sess_len;                 // host: tokens of each slot at the last poll
+  // beam session (sv_beam_session_*): the slots form groups of num_beams, each one image's beam search with its own
+  // beam_params / beam_state / beam_plan entry; sess_live / sess_len are kept at each group's first slot
+  bool sess_beam = false;
+  sv_beam_params sess_bp{};
+  bf16* bsess_px = nullptr;                  // staging: one admitted image repeated num_beams times
+  int32_t* bsess_ids = nullptr;              //   and its prompt
 
   // prompt-lookup speculative decoding (sv_generate_speculative): device state allocated by the first call
   svspec::State* spec = nullptr;
@@ -1509,6 +1516,23 @@ static svbeam::Params beam_params_dev(const sv_beam_params* bp, int batch, int v
   return hp;
 }
 
+// The device state of sv_beam_search and beam sessions, allocated once per engine.
+static int beam_alloc(sv_engine* e) {
+  if (e->beam_state) return SV_OK;
+  const sv_model_desc& d = e->d;
+  const int stride = d.max_len;
+  bool ok = true;
+  const int MR = svbeam::kMaxRows, MK = svbeam::kMaxK, MG = svbeam::kMaxRows / 2;
+#define BAL(ptr, n) ok = ok && (dev_alloc(e, &e->ptr, (n)) == cudaSuccess)
+  BAL(beam_params, MG); BAL(beam_state, MG); BAL(beam_plan, MG);
+  BAL(beam_key, MR * MK); BAL(beam_val, MR * MK); BAL(beam_tok, MR * MK);
+  BAL(beam_run_seq, (int64_t)2 * MR * stride); BAL(beam_fin_seq, (int64_t)2 * MR * stride);
+  BAL(kstage, e->cache_layer_stride * d.n_layer); BAL(vstage, e->cache_layer_stride * d.n_layer);
+#undef BAL
+  if (!ok) { e->beam_state = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the beam-search state failed: %s", cudaGetErrorString(cudaGetLastError())); }
+  return SV_OK;
+}
+
 // Beam search with the whole loop on the device.  Graph body = one decode step over the batch * num_beams cache rows, then
 // candidates -> bookkeeping (+ next-token embeddings) -> KV suffix copies; the host replays it and polls `done`.
 int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_t* out_ids, int32_t* out_len, void* stream) {
@@ -1531,17 +1555,7 @@ int sv_beam_search(sv_engine* e, const sv_beam_params* bp, int32_t batch, int32_
   }
   LaunchScope scope(e);
   const int stride = d.max_len;
-  if (!e->beam_state) {
-    bool ok = true;
-    const int MR = svbeam::kMaxRows, MK = svbeam::kMaxK;
-#define BAL(ptr, n) ok = ok && (dev_alloc(e, &e->ptr, (n)) == cudaSuccess)
-    BAL(beam_params, 1); BAL(beam_state, 1); BAL(beam_plan, 1);
-    BAL(beam_key, MR * MK); BAL(beam_val, MR * MK); BAL(beam_tok, MR * MK);
-    BAL(beam_run_seq, (int64_t)2 * MR * stride); BAL(beam_fin_seq, (int64_t)2 * MR * stride);
-    BAL(kstage, e->cache_layer_stride * d.n_layer); BAL(vstage, e->cache_layer_stride * d.n_layer);
-#undef BAL
-    if (!ok) { e->beam_state = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the beam-search state failed: %s", cudaGetErrorString(cudaGetLastError())); }
-  }
+  SV_TRY(beam_alloc(e));
   cudaStream_t st = e->gen_stream;
   SV_TRY(join_caller(e, stream));
 
@@ -1660,6 +1674,16 @@ int sv_expand_batch(sv_engine* e, const int32_t* src_rows_host, int32_t new_batc
 }
 
 // ---- continuous batching --------------------------------------------------------------------------------------------
+// The per-row state of a session, allocated by the first one.
+static int session_alloc(sv_engine* e) {
+  if (e->rows) return SV_OK;
+  const sv_model_desc& d = e->d;
+  bool ok = dev_alloc(e, &e->rows, 1) == cudaSuccess && dev_alloc(e, &e->sess_logits, (int64_t)d.max_batch * d.vocab) == cudaSuccess;
+  if (ok && !e->rows_host) ok = cudaMallocHost(reinterpret_cast<void**>(&e->rows_host), sizeof(RowState)) == cudaSuccess;
+  if (!ok) { e->rows = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the session state failed: %s", cudaGetErrorString(cudaGetLastError())); }
+  return SV_OK;
+}
+
 int sv_session_begin(sv_engine* e, const sv_gen_params* p, int32_t slots) {
   if (!e || !p) return fail(e, SV_ERR_INVALID, "null argument");
   if (e->session) return fail(e, SV_ERR_STATE, "a decode session is already open");
@@ -1672,11 +1696,7 @@ int sv_session_begin(sv_engine* e, const sv_gen_params* p, int32_t slots) {
   SV_CK(e, cudaSetDevice(e->device));
   LaunchScope scope(e);
   const sv_model_desc& d = e->d;
-  if (!e->rows) {
-    bool ok = dev_alloc(e, &e->rows, 1) == cudaSuccess && dev_alloc(e, &e->sess_logits, (int64_t)d.max_batch * d.vocab) == cudaSuccess;
-    if (ok && !e->rows_host) ok = cudaMallocHost(reinterpret_cast<void**>(&e->rows_host), sizeof(RowState)) == cudaSuccess;
-    if (!ok) { e->rows = nullptr; return fail(e, SV_ERR_CUDA, "allocation of the session state failed: %s", cudaGetErrorString(cudaGetLastError())); }
-  }
+  SV_TRY(session_alloc(e));
   cudaStream_t st = e->gen_stream;
   const GenParamsDev hp = gen_params_dev(p, /*stop_row0_only=*/0, d.max_len);
   SV_CK(e, cudaMemcpyAsync(e->params, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));   // pageable: staged synchronously
@@ -1699,6 +1719,7 @@ int sv_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t*
                      const int32_t* src_host, void* stream) {
   if (!e || !pixels || !prompt_ids || !slots_host) return fail(e, SV_ERR_INVALID, "null argument");
   if (!e->session) return fail(e, SV_ERR_STATE, "sv_session_admit needs sv_session_begin first");
+  if (e->sess_beam) return fail(e, SV_ERR_STATE, "sv_session_admit: a beam session is open (admit with sv_beam_session_admit)");
   const sv_model_desc& d = e->d;
   const int S = e->sess_slots, cap = e->sess_p.max_new_tokens;
   if (k < 1 || k > S) return fail(e, SV_ERR_INVALID, "k %d outside [1,%d]", k, S);
@@ -1796,11 +1817,26 @@ int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int3
   int steps = 0;
   if (!any_fin && any_live && max_steps > 0) {
     ensure_flow_tiles(e, st);    // (no-op unless a weight was loaded since the tiles were built)
-    const bool fused = e->fused_decode, sample = e->sess_p.do_sample != 0;
-    const int total = e->Q + e->sess_prompt_len + e->sess_p.max_new_tokens;     // the session cap fixes the split count
+    const bool beam = e->sess_beam;
+    const bool fused = e->fused_decode, sample = !beam && e->sess_p.do_sample != 0;
+    const int cap = beam ? e->sess_bp.max_new_tokens : e->sess_p.max_new_tokens;
+    const int total = e->Q + e->sess_prompt_len + cap;     // the session cap fixes the split count
     const int parts = decode_parts(fused, total);
-    GraphEntry& ge = e->step_graphs[{StepKind::session, S, parts, sample, fused, e->use_pdl}];
+    // (beam sessions: beam-sample and the beam width are read from the device parameters, as in sv_beam_search)
+    GraphEntry& ge = e->step_graphs[{beam ? StepKind::beam_session : StepKind::session, S, parts, sample, fused, e->use_pdl}];
+    const sv_model_desc& d = e->d;
     auto step = [&](bool pdl) {
+      if (beam) {              // the decode step, then every live group's bookkeeping, as sv_beam_search runs it
+        run_engine_step(e, fused ? nullptr : e->next_ids, S, parts, pdl, st, e->rows);
+        launch_beam_session_candidates(e->logits, d.vocab, S, e->beam_params, e->beam_state, e->beam_run_seq, e->beam_key,
+                                       e->beam_val, e->beam_tok, e->rows, ~0u, st);
+        launch_beam_session_step(e->beam_params, e->beam_state, e->beam_plan, e->beam_key, e->beam_val, e->beam_tok,
+                                 e->beam_run_seq, e->beam_fin_seq, e->rows, ~0u, S, /*advance=*/1, e->wte, e->wpe, e->d_x,
+                                 d.hidden, d.n_positions, e->next_ids, st);
+        launch_beam_session_kv_copy(e->kcache, e->vtcache, e->kstage, e->vstage, e->cache_layer_stride, d.n_layer, S,
+                                    d.n_kv_head, e->tcap, d.head_dim, e->beam_params, e->beam_plan, e->rows, ~0u, st);
+        return;
+      }
       run_engine_step(e, fused && !sample ? nullptr : e->next_ids, S, parts, pdl, st, e->rows);
       launch_token_select(e, e->logits, S, sample, /*partials=*/true, /*advance_len=*/1, pdl, st, e->rows, (1u << S) - 1u);
     };
@@ -1808,7 +1844,8 @@ int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int3
       SV_CK(e, capture_step(st, e->use_pdl && fused, step, ge));
       if (fused && !ge.pdl) e->use_pdl = false;
     }
-    const int every = e->sess_p.poll_interval > 0 ? e->sess_p.poll_interval : 16;
+    const int poll = beam ? e->sess_bp.poll_interval : e->sess_p.poll_interval;
+    const int every = poll > 0 ? poll : 16;
     while (steps < max_steps && !any_fin && any_live) {
       const int n = std::min(every, max_steps - steps);
       SV_TRY(replay(e, ge, n));
@@ -1843,7 +1880,14 @@ int sv_session_read(sv_engine* e, int32_t slot, int32_t* ids, void* stream) {
   cudaStream_t st = e->gen_stream;
   SV_TRY(join_caller(e, stream));
   const int n = e->sess_len[slot];
-  if (n > 0) SV_CK(e, cudaMemcpyAsync(ids, e->out_ids + (int64_t)slot * e->d.max_len, (size_t)n * 4, cudaMemcpyDefault, st));
+  const int32_t* src = e->out_ids + (int64_t)slot * e->d.max_len;
+  if (e->sess_beam) {          // the best hypothesis = finished slot 0 of the group's live half of fin_seq
+    const int nb = e->sess_bp.num_beams;
+    if (slot % nb) return fail(e, SV_ERR_INVALID, "slot %d is not the first slot of a group of %d", slot, nb);
+    SV_TRY(read_flags(e, &e->beam_state[slot / nb].parity, 1));
+    src = e->beam_fin_seq + ((int64_t)e->host_flag[0] * svbeam::kMaxRows + slot) * e->d.max_len;
+  }
+  if (n > 0) SV_CK(e, cudaMemcpyAsync(ids, src, (size_t)n * 4, cudaMemcpyDefault, st));
   SV_CK(e, cudaStreamSynchronize(st));
   return n;
 }
@@ -1854,9 +1898,142 @@ int sv_session_end(sv_engine* e) {
   SV_CK(e, cudaSetDevice(e->device));
   SV_CK(e, cudaStreamSynchronize(e->gen_stream));
   e->session = false;
+  e->sess_beam = false;
   e->sess_slots = 0;
   e->sess_live.clear();
   e->sess_len.clear();
+  return SV_OK;
+}
+
+// ---- beam sessions (DESIGN.md §7h) ----------------------------------------------------------------------------------
+int sv_beam_session_begin(sv_engine* e, const sv_beam_params* bp, int32_t slots) {
+  if (!e || !bp) return fail(e, SV_ERR_INVALID, "null argument");
+  if (e->session) return fail(e, SV_ERR_STATE, "a decode session is already open");
+  const sv_model_desc& d = e->d;
+  const int nb = bp->num_beams;
+  if (nb < 2 || slots < nb || slots > d.max_batch || slots % nb)
+    return fail(e, SV_ERR_INVALID, "slots %d must be a multiple of num_beams %d (>= 2) in [num_beams, %d]", slots, nb, d.max_batch);
+  if (sv_beam_params_check_rows(bp, slots / nb, d.max_batch) != SV_OK)
+    return fail(e, SV_ERR_INVALID, "bad beam parameters (need max_new_tokens >= 1, n_stop_ids in [0,8], early_stopping in {0,1,2}, "
+                                   "temperature > 0, repetition_penalty > 0, 2 * num_beams <= 16)");
+  if (bp->max_new_tokens > d.max_len) return fail(e, SV_ERR_INVALID, "max_new_tokens %d exceeds max_len %d", bp->max_new_tokens, d.max_len);
+  int r = check_ready(e);
+  if (r != SV_OK) return r;
+  SV_CK(e, cudaSetDevice(e->device));
+  if (beam_init(d.vocab) != cudaSuccess || beam_session_init(d.vocab) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(e, SV_ERR_UNSUPPORTED, "a logits row of %d entries does not fit the SM's shared memory: beam sessions need the "
+                                       "device candidate kernel", d.vocab);
+  }
+  LaunchScope scope(e);
+  SV_TRY(session_alloc(e));
+  SV_TRY(beam_alloc(e));
+  if (!e->bsess_px) {
+    const int64_t img = (int64_t)3 * d.image_size * d.image_size;
+    if (dev_alloc(e, &e->bsess_px, d.max_batch * img) != cudaSuccess || dev_alloc(e, &e->bsess_ids, d.max_batch * kMaxPrompt) != cudaSuccess) {
+      e->bsess_px = nullptr;
+      return fail(e, SV_ERR_CUDA, "allocation of the beam-session staging failed: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+  }
+  cudaStream_t st = e->gen_stream;
+  SV_CK(e, cudaMemsetAsync(e->rows, 0, sizeof(RowState), st));          // no slot live
+  const svbeam::Params hp = beam_params_dev(bp, 1, d.vocab, d.max_len);
+  for (int g = 0; g < slots / nb; ++g)     // every group's entry holds the beam width the kernels read (admission fills the rest)
+    SV_CK(e, cudaMemcpyAsync(e->beam_params + g, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));   // pageable: staged synchronously
+  SV_CK(e, cudaMemsetAsync(e->beam_plan, 0, sizeof(svbeam::Plan) * (svbeam::kMaxRows / 2), st));
+  ensure_flow_tiles(e, st);
+  SV_CK(e, cudaStreamSynchronize(st));
+  e->sess_bp = *bp;
+  e->sess_beam = true;
+  e->sess_slots = slots;
+  e->sess_prompt_len = 0;
+  e->sess_live.assign(slots, 0);
+  e->sess_len.assign(slots, 0);
+  e->session = true;
+  e->encoded = false;
+  e->prefilled = false;
+  return SV_OK;
+}
+
+int sv_beam_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t* prompt_ids, int32_t prompt_len,
+                          const int32_t* groups_host, const int32_t* max_new_host, const uint64_t* seeds_host, void* stream) {
+  if (!e || !pixels || !prompt_ids || !groups_host) return fail(e, SV_ERR_INVALID, "null argument");
+  if (!e->session || !e->sess_beam) return fail(e, SV_ERR_STATE, "sv_beam_session_admit needs sv_beam_session_begin first");
+  const sv_model_desc& d = e->d;
+  const int nb = e->sess_bp.num_beams, S = e->sess_slots, G = S / nb, cap = e->sess_bp.max_new_tokens;
+  if (k < 1 || k > G) return fail(e, SV_ERR_INVALID, "k %d outside [1,%d]", k, G);
+  if (prompt_len < 1 || prompt_len > kMaxPrompt) return fail(e, SV_ERR_INVALID, "prompt_len %d outside [1,%d]", prompt_len, kMaxPrompt);
+  if (e->sess_prompt_len != 0 && prompt_len != e->sess_prompt_len)
+    return fail(e, SV_ERR_INVALID, "prompt_len %d differs from the session's %d (the split count of the decode graph is fixed by "
+                                   "prefix + max_new_tokens)", prompt_len, e->sess_prompt_len);
+  const int prefix = e->Q + prompt_len;
+  if (prefix + cap > d.max_len)
+    return fail(e, SV_ERR_INVALID, "prefix %d + max_new_tokens %d exceeds max_len %d", prefix, cap, d.max_len);
+  std::vector<int> used(G, 0);
+  for (int j = 0; j < k; ++j) {
+    const int g = groups_host[j];
+    if (g < 0 || g >= G) return fail(e, SV_ERR_INVALID, "group %d outside [0,%d)", g, G);
+    if (used[g] || e->sess_live[g * nb]) return fail(e, SV_ERR_INVALID, "group %d is busy or listed twice", g);
+    used[g] = 1;
+    if (max_new_host && (max_new_host[j] < 1 || max_new_host[j] > cap))
+      return fail(e, SV_ERR_INVALID, "max_new[%d] = %d outside [1,%d] (the session cap)", j, max_new_host[j], cap);
+  }
+  SV_CK(e, cudaSetDevice(e->device));
+  LaunchScope scope(e);
+  cudaStream_t st = e->gen_stream;
+  SV_TRY(join_caller(e, stream));
+  const int64_t img = (int64_t)3 * d.image_size * d.image_size;
+  const int stride = d.max_len, fill = e->sess_bp.pad_token_id;
+  SessionAdmit adm;
+  memset(&adm, 0, sizeof(adm));
+  uint32_t mask = 0;
+  // Each image runs what a one-image beam search runs: the image and prompt repeated num_beams times are encoded and
+  // prefilled at batch num_beams (GEMM tiles depend on M), into the group's rows.  On an error below, the groups touched so
+  // far are not marked live, so the caller may admit into them again (or end the session).
+  for (int j = 0; j < k; ++j) {
+    const int g = groups_host[j], row0 = g * nb;
+    for (int b = 0; b < nb; ++b) {
+      SV_CK(e, cudaMemcpyAsync(e->bsess_px + b * img, (const bf16*)pixels + j * img, img * sizeof(bf16), cudaMemcpyDeviceToDevice, st));
+      SV_CK(e, cudaMemcpyAsync(e->bsess_ids + b * prompt_len, prompt_ids + (int64_t)j * prompt_len, prompt_len * sizeof(int32_t),
+                               cudaMemcpyDeviceToDevice, st));
+    }
+    int r = run_encode(e, e->bsess_px, nb, st);
+    if (r == SV_OK) r = run_prefill(e, e->visual, e->Q, e->bsess_ids, nb, prompt_len, st, row0, e->sess_logits + (int64_t)row0 * d.vocab);
+    if (r != SV_OK) return r;
+    sv_beam_params bp = e->sess_bp;
+    bp.max_new_tokens = max_new_host ? max_new_host[j] : cap;
+    if (seeds_host) bp.seed = seeds_host[j];
+    const svbeam::Params hp = beam_params_dev(&bp, 1, d.vocab, stride);
+    svbeam::State hs;
+    memset(&hs, 0, sizeof(hs));
+    svbeam::init_state(hp, hs, prefix);
+    SV_CK(e, cudaMemcpyAsync(e->beam_params + g, &hp, sizeof(hp), cudaMemcpyHostToDevice, st));   // pageable: staged synchronously
+    SV_CK(e, cudaMemcpyAsync(e->beam_state + g, &hs, sizeof(hs), cudaMemcpyHostToDevice, st));
+    SV_CK(e, cudaMemsetAsync(e->beam_plan + g, 0, sizeof(svbeam::Plan), st));
+    for (int half = 0; half < 2; ++half) {
+      const int64_t off = ((int64_t)half * svbeam::kMaxRows + row0) * stride;
+      launch_fill_i32(e->beam_run_seq + off, fill, nb * stride, st);
+      launch_fill_i32(e->beam_fin_seq + off, fill, nb * stride, st);
+    }
+    for (int b = 0; b < nb; ++b) {
+      adm.slot[adm.n] = row0 + b; adm.len[adm.n] = prefix; adm.max_new[adm.n] = bp.max_new_tokens; adm.seed[adm.n] = bp.seed;
+      ++adm.n;
+    }
+    mask |= 1u << g;
+  }
+  launch_session_admit(e->rows, adm, e->seen, d.vocab, e->out_ids, d.max_len, fill, st);     // row_len, row_active, ...
+  // step 0 of the admitted groups from their prefill logits (sv_beam_search's first bookkeeping, no position advance)
+  launch_beam_session_candidates(e->sess_logits, d.vocab, S, e->beam_params, e->beam_state, e->beam_run_seq, e->beam_key,
+                                 e->beam_val, e->beam_tok, e->rows, mask, st);
+  launch_beam_session_step(e->beam_params, e->beam_state, e->beam_plan, e->beam_key, e->beam_val, e->beam_tok, e->beam_run_seq,
+                           e->beam_fin_seq, e->rows, mask, S, /*advance=*/0, e->wte, e->wpe, e->d_x, d.hidden, d.n_positions,
+                           e->next_ids, st);
+  launch_beam_session_kv_copy(e->kcache, e->vtcache, e->kstage, e->vstage, e->cache_layer_stride, d.n_layer, S, d.n_kv_head,
+                              e->tcap, d.head_dim, e->beam_params, e->beam_plan, e->rows, mask, st);
+  SV_CK(e, cudaGetLastError());
+  SV_CK(e, cudaStreamSynchronize(st));     // the caller may release pixels / prompt_ids on return
+  for (int j = 0; j < k; ++j) e->sess_live[groups_host[j] * nb] = 1;
+  e->sess_prompt_len = prompt_len;
   return SV_OK;
 }
 
@@ -1875,7 +2052,7 @@ const char* sv_engine_describe(sv_engine* e) {
            !e->fused_decode ? "legacy-kernels" : e->use_flow ? (e->flow_realloc ? "dataflow-kernel-setmaxnreg" : "dataflow-kernel") : "ring-gemv-graph",
            e->ring_tiles ? "slab-tiled" : "row-major", (int)e->use_pdl, e->linear_impl, e->d.max_batch, decode_flow_status(),
            e->flow_requested && !e->use_flow && e->d.max_batch > 8 ? " SV_FLOW ignored: the dataflow kernel holds 8 rows, max_batch > 8 runs the graph path" : "",
-           e->use_flow ? " sessions and speculative decoding: graph path (the dataflow kernel has no per-row positions)" : "");
+           e->use_flow ? " sessions, beam sessions and speculative decoding: graph path (the dataflow kernel has no per-row positions)" : "");
   e->describe = buf;
   return e->describe.c_str();
 }

@@ -260,5 +260,22 @@ void launch_beam_step(const svbeam::Params* p, svbeam::State* st, svbeam::Plan* 
                       int32_t* next_ids, cudaStream_t st_);
 void launch_beam_kv_copy(bf16* kc, bf16* vc, bf16* kc2, bf16* vc2, int64_t layer_stride, int n_layer, int rows, int n_kv,
                          int tcap, int D, const svbeam::Plan* plan, cudaStream_t st_);
+// Beam-session variants (sv_beam_session_*): group g of num_beams = p[0].nb slots owns rows [g * nb, (g + 1) * nb) and its
+// own p[g] (B = 1), st[g], plan[g] in group-local rows; run_seq / fin_seq are [2][kMaxRows][seq_stride] by global row, each
+// group flipping its own parity half.  Groups outside group_mask, not live (rows->row_active of their first slot) or done
+// are left as they are.  Positions come from rows->row_len; the step kernel advances row_len / row_step of a continuing
+// group's slots and, at its finish, clears their row_active, writes the best hypothesis' length to row_step of its first
+// slot and raises rows->event.  (sv_beam_session.cu)
+cudaError_t beam_session_init(int vocab);  // cudaErrorInvalidValue: as beam_init
+void launch_beam_session_candidates(const bf16* logits, int vocab, int slots, const svbeam::Params* p,
+                                    const svbeam::State* st, const int32_t* run_seq, float* cand_key, float* cand_val,
+                                    int32_t* cand_tok, const RowState* rows, uint32_t group_mask, cudaStream_t st_);
+void launch_beam_session_step(const svbeam::Params* p, svbeam::State* st, svbeam::Plan* plan, const float* cand_key,
+                              const float* cand_val, const int32_t* cand_tok, int32_t* run_seq, int32_t* fin_seq,
+                              RowState* rows, uint32_t group_mask, int slots, int advance, const bf16* wte, const bf16* wpe,
+                              bf16* x, int h, int n_positions, int32_t* next_ids, cudaStream_t st_);
+void launch_beam_session_kv_copy(bf16* kc, bf16* vc, bf16* kc2, bf16* vc2, int64_t layer_stride, int n_layer, int slots,
+                                 int n_kv, int tcap, int D, const svbeam::Params* p, const svbeam::Plan* plan,
+                                 const RowState* rows, uint32_t group_mask, cudaStream_t st_);
 
 }  // namespace sv

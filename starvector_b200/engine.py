@@ -58,6 +58,43 @@ class GenerationParams:
         return p
 
 
+@dataclasses.dataclass
+class BeamSearchParams:
+    """HF `generate(num_beams > 1)` kwargs as `sv_beam_search` and beam sessions take them.  `pad_token_id` is the fill of
+    the sequence rows (HF: pad if given, else eos; -1 without EOS), as `beam_search` passes it."""
+
+    num_beams: int
+    max_new_tokens: int
+    do_sample: bool = False
+    temperature: float = 1.0
+    top_p: float = 1.0
+    repetition_penalty: float = 1.0
+    length_penalty: float = 1.0
+    early_stopping: object = True            # True, False or "never"
+    eos_token_id: Optional[int] = 0
+    pad_token_id: int = 0
+    stop_ids: Sequence[int] = ()
+    seed: int = 0
+    poll_interval: int = 16
+
+    def to_c(self) -> _lib.BeamParams:
+        if len(self.stop_ids) > 8:
+            raise ValueError("stop sequence longer than 8 tokens")
+        bp = _lib.BeamParams()
+        bp.num_beams, bp.max_new_tokens, bp.do_sample = int(self.num_beams), int(self.max_new_tokens), int(bool(self.do_sample))
+        bp.early_stopping = 2 if self.early_stopping == "never" else int(self.early_stopping is True)
+        bp.temperature, bp.top_p = float(self.temperature), float(self.top_p)
+        bp.repetition_penalty, bp.length_penalty = float(self.repetition_penalty), float(self.length_penalty)
+        bp.eos_token_id = -1 if self.eos_token_id is None else int(self.eos_token_id)
+        bp.pad_token_id = int(self.pad_token_id)
+        bp.n_stop_ids = len(self.stop_ids)
+        for i, t in enumerate(self.stop_ids):
+            bp.stop_ids[i] = int(t)
+        bp.poll_interval = int(self.poll_interval)
+        bp.seed = int(self.seed) & (2 ** 64 - 1)
+        return bp
+
+
 def _stream_ptr(device: torch.device) -> C.c_void_p:
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -232,20 +269,8 @@ class Engine:
         """`sv_beam_search`: the whole beam search / beam-sample on the device, after a prefill of batch * num_beams rows
         (every image repeated num_beams times, adjacent).  Returns int32 `[batch, n_generated]`, the best hypothesis per image.
         Raises NotImplementedError when the vocabulary does not fit the candidate kernel (use the host-stepped loop)."""
-        if len(stop_ids) > 8:
-            raise ValueError("stop sequence longer than 8 tokens")
-        bp = _lib.BeamParams()
-        bp.num_beams, bp.max_new_tokens, bp.do_sample = int(num_beams), int(max_new_tokens), int(bool(do_sample))
-        bp.early_stopping = 2 if early_stopping == "never" else int(early_stopping is True)
-        bp.temperature, bp.top_p = float(temperature), float(top_p)
-        bp.repetition_penalty, bp.length_penalty = float(repetition_penalty), float(length_penalty)
-        bp.eos_token_id = -1 if eos_token_id is None else int(eos_token_id)
-        bp.pad_token_id = int(pad_token_id)
-        bp.n_stop_ids = len(stop_ids)
-        for i, t in enumerate(stop_ids):
-            bp.stop_ids[i] = int(t)
-        bp.poll_interval = int(poll_interval)
-        bp.seed = int(seed) & (2 ** 64 - 1)
+        bp = BeamSearchParams(num_beams, max_new_tokens, do_sample, temperature, top_p, repetition_penalty, length_penalty,
+                              early_stopping, eos_token_id, pad_token_id, stop_ids, seed, poll_interval).to_c()
         out = torch.empty(batch, max(int(max_new_tokens), 1), dtype=torch.int32, device=self.device)
         olen = torch.empty(batch, dtype=torch.int32, device=self.device)
         with self._lock:
@@ -402,6 +427,55 @@ class Engine:
             if r < 0:
                 self._ck(r)
         return out[:r].clone()
+
+    def beam_requests(self, pixels: torch.Tensor, prompt_ids: torch.Tensor, *, num_beams: int, max_new_tokens: int,
+                      caps: Optional[Sequence[int]] = None, seeds: Optional[Sequence[int]] = None, do_sample: bool = False,
+                      temperature: float = 1.0, top_p: float = 1.0, repetition_penalty: float = 1.0,
+                      length_penalty: float = 1.0, early_stopping=True, eos_token_id: Optional[int] = 0, pad_token_id: int = 0,
+                      stop_ids: Sequence[int] = (), seed: int = 0, poll_interval: int = 16, on_finish=None,
+                      slots: Optional[int] = None) -> List[torch.Tensor]:
+        """Continuous batching of beam search over any number of images: a beam session of `slots` cache rows (default
+        `max_batch` rounded down to a multiple of `num_beams`) in groups of `num_beams`, each group refilled with the next
+        queued image as soon as its search ends.  Image k gets the int32 ids (CPU) that
+        `beam_search(engine, pixels[k:k+1], prompt, num_beams=..., impl="device", seed=seeds[k], max_new_tokens=caps[k], ...)`
+        returns, bit for bit, when its cap is the session cap `max_new_tokens` (a smaller cap: when the decode attention's
+        partition of prefix + cap is that of prefix + max_new_tokens).  `seeds` default to `seed + k`; `on_finish(k, ids)`
+        streams results as they complete."""
+        from .continuous import ContinuousScheduler
+
+        fill = (pad_token_id if pad_token_id is not None else eos_token_id) if eos_token_id is not None else -1
+        params = BeamSearchParams(num_beams, max_new_tokens, do_sample, temperature, top_p, repetition_penalty, length_penalty,
+                                  early_stopping, eos_token_id, fill, stop_ids, seed, poll_interval)
+        if slots is None:
+            slots = self.dims.max_batch // int(num_beams) * int(num_beams)
+        return ContinuousScheduler(self, slots, num_beams=num_beams).run(pixels, prompt_ids, params, max_new_tokens=caps,
+                                                                         seeds=seeds, on_finish=on_finish)
+
+    def beam_session_begin(self, params: BeamSearchParams, slots: int) -> None:
+        bp = params.to_c()
+        with self._lock:
+            self._ck(self._lib.sv_beam_session_begin(self._h, C.byref(bp), int(slots)))
+            self._session_slots = int(slots)
+            self._batch = 0
+
+    def beam_session_admit(self, pixels: torch.Tensor, prompt_ids: torch.Tensor, groups: Sequence[int], *,
+                           max_new_tokens: Optional[Sequence[int]] = None, seeds: Optional[Sequence[int]] = None) -> None:
+        """Encode and prefill images `[k, 3, S, S]` (prompts `[k, P]`) into the free beam groups `groups` (group g = slots
+        g * num_beams ...); image j runs its own search with cap `max_new_tokens[j]` and seed `seeds[j]`."""
+        d = self.dims
+        if pixels.dim() != 4 or tuple(pixels.shape[1:]) != (3, d.image_size, d.image_size):
+            raise ValueError(f"image batch must be [B,3,{d.image_size},{d.image_size}], got {tuple(pixels.shape)}")
+        px = self._dev(pixels, torch.bfloat16)
+        ids = self._dev(prompt_ids, torch.int32)
+        k = len(groups)
+        if px.shape[0] != k or ids.dim() != 2 or ids.shape[0] != k:
+            raise ValueError(f"{k} groups need {k} images and [{k}, P] prompt ids")
+        gr = (C.c_int32 * k)(*[int(g) for g in groups])
+        mx = None if max_new_tokens is None else (C.c_int32 * k)(*[int(m) for m in max_new_tokens])
+        sd = None if seeds is None else (C.c_uint64 * k)(*[int(x) & (2 ** 64 - 1) for x in seeds])
+        with self._lock:
+            self._ck(self._lib.sv_beam_session_admit(self._h, C.c_void_p(px.data_ptr()), k, C.c_void_p(ids.data_ptr()),
+                                                     ids.shape[1], gr, mx, sd, _stream_ptr(self.device)))
 
     def session_end(self) -> None:
         with self._lock:

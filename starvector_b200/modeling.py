@@ -342,6 +342,33 @@ class StarVectorStarCoder:
         p0 = prompt_ids[0].cpu().long()
         return tok.batch_decode([torch.cat([p0, o.long()]) for o in outs], skip_special_tokens=True)
 
+    @torch.no_grad()
+    def generate_im2svg_continuous_beams(self, batch: Dict[str, torch.Tensor], **kwargs) -> List[str]:
+        """`generate_im2svg` with beam search (the reference default, `num_beams=2`) over any number of images, with
+        continuous batching (`Engine.beam_requests`): the engine's cache rows form groups of `num_beams`, and a group is
+        refilled with the next image as soon as its search ends.  Takes the kwargs and defaults of `generate_im2svg`
+        (beam-sample when `use_nucleus_sampling` is on, `length_penalty`, ...).  Image k's string is exactly
+        `generate_im2svg({"image": image[k:k+1]}, seed=seed + k, **kwargs)[0]`."""
+        num_beams = int(kwargs.get("num_beams", 2))
+        if num_beams < 2:
+            raise ValueError("generate_im2svg_continuous_beams needs num_beams >= 2; use generate_im2svg_continuous for one "
+                             "beam per request")
+        if int(kwargs.get("num_return_sequences", 1)) > 1:
+            raise ValueError("num_return_sequences > 1 decodes one beam per completion (the reference forces num_beams=1): "
+                             "use generate_im2svg_continuous")
+        image = batch["image"]
+        prompt_ids = self._tokenize_prompt(kwargs.get("prompt"), 1)
+        params = self._gen_params(kwargs, prefix_len=self.query_length + prompt_ids.shape[1])
+        outs = self.engine.beam_requests(
+            image, prompt_ids[0], num_beams=num_beams, max_new_tokens=params.max_new_tokens,
+            seeds=[params.seed + k for k in range(image.shape[0])], do_sample=params.do_sample,
+            temperature=params.temperature, top_p=params.top_p, repetition_penalty=params.repetition_penalty,
+            length_penalty=float(kwargs.get("length_penalty", 1.0)), early_stopping=not self.v2,     # as _beam_generate
+            eos_token_id=params.eos_token_id, pad_token_id=params.pad_token_id, stop_ids=params.stop_ids)
+        tok = self.svg_transformer.tokenizer
+        p0 = prompt_ids[0].cpu().long()
+        return tok.batch_decode([torch.cat([p0, o.long()]) for o in outs], skip_special_tokens=True)
+
     def generate_im2svg_grpo(self, batch, **kwargs):                                               # :261-286
         """`num_return_sequences` completions per image (sampled independently, `num_beams` forced to 1, :277-280):
         HF's `_expand_inputs_for_generation` = every image row repeated G times, adjacent — here the image is encoded and
@@ -535,6 +562,9 @@ class StarVectorForCausalLM:
 
     def generate_im2svg_continuous(self, batch, **kwargs) -> List[str]:
         return self.model.generate_im2svg_continuous(batch, **kwargs)
+
+    def generate_im2svg_continuous_beams(self, batch, **kwargs) -> List[str]:
+        return self.model.generate_im2svg_continuous_beams(batch, **kwargs)
 
     def generate_im2text(self, batch, **kwargs):                              # :189-190 (dangling in the reference too)
         raise AttributeError("generate_im2text has no implementation in the reference model core either")
