@@ -284,6 +284,17 @@ SV_API int sv_session_admit(sv_engine* e, const void* pixels, int32_t k, const i
  * slots whose finish this call reports (each finish is reported once; the slot is free again), len_host int32 [slots]
  * (optional): tokens each slot holds.  Synchronises `stream`. */
 SV_API int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int32_t* len_host, void* stream);
+/* Speculative session (DESIGN.md §7i): sv_session_begin with prompt-lookup drafts in the columns the live rows leave
+ * free.  Every verify step streams the weights once for `slots` columns: each live row gets one column for its last token,
+ * and the spare columns carry drafts from n-gram matches in the rows' own tokens (up to sp->num_tokens per row, handed
+ * out round-robin in slot order).  Every request gets the tokens it gets in a plain session, bit for bit; the drafts change
+ * the speed only.  Admit, run (max_steps counts verify steps), read and end as for a plain session.  v1 engines on the fused
+ * graph decode path (SV_FLOW engines run it on the graph path).  SV_ERR_UNSUPPORTED for v2 and SV_DECODE=legacy;
+ * SV_ERR_INVALID for num_tokens outside [1, slots - 1] or an n-gram size < 1. */
+SV_API int sv_session_begin_speculative(sv_engine* e, const sv_gen_params* p, const sv_spec_params* sp, int32_t slots);
+/* Counters of the open speculative session: verify steps, drafts proposed, drafts accepted (any pointer may be NULL).
+ * SV_ERR_STATE unless a speculative session is open.  Synchronises the engine's stream. */
+SV_API int sv_session_spec_stats(sv_engine* e, int32_t* steps, int32_t* drafted, int32_t* accepted);
 /* Copy the tokens of `slot` (as of the last sv_session_run) to ids (int32, host or device); returns their count. */
 SV_API int sv_session_read(sv_engine* e, int32_t slot, int32_t* ids, void* stream);
 /* Close the session: the rectangle-batch entry points work again (after a new prefill). */
@@ -544,6 +555,57 @@ typedef struct sv_op_spec_args {
   int32_t h, n_positions;       /* h % 8 == 0 */
 } sv_op_spec_args;
 SV_API int sv_op_spec_select(const sv_op_spec_args* args, void* stream);
+
+/* ---- speculative sessions: host replays and one-launch hooks (tests) ---- */
+/* The per-row state of a session (RowState), field for field. */
+typedef struct sv_session_rows {
+  int32_t row_len[16], row_step[16], row_active[16], event, pad_, row_max_new[16];
+  uint64_t row_seed[16];
+} sv_session_rows;
+/* The device state of a speculative session (svspec::SessionState), field for field. */
+typedef struct sv_spec_session_state {
+  int32_t n_live, row[16], pos[16];  /* the column map: column c < n_live decodes (row[c], pos[c]); the others are inert */
+  int32_t tok[16], sel[16], off[16]; /* column inputs, selected tokens, each column's offset within its row */
+  int32_t ncols, k, max_ngram;       /* columns (the session's slots), drafts per row at most, the largest n-gram matched */
+  int32_t steps, drafted, accepted;  /* counters */
+} sv_spec_session_state;
+/* The column allocation of a verify step: S slots, active[r] != 0 for the live rows, want[r] the drafts row r asks for,
+ * at most `budget` (and S) columns in all.  Every live row gets one column; the spare columns go round-robin in slot order,
+ * one draft per pass to each row below its want.  Writes g[r] (drafts granted) and first[r] (the row's first column, -1
+ * for idle rows); returns n_live (the columns used), or SV_ERR_INVALID. */
+SV_API int sv_spec_session_plan_host(int32_t S, const int32_t* active, const int32_t* want, int32_t budget, int32_t* g,
+                                     int32_t* first);
+/* What the session's tail kernel does, on the host: with `accept`, every live row's accept walk on ss->sel with the plain
+ * session's per-token bookkeeping (rows, out_ids [S][out_stride]); then the next drafts, the allocation (column budget:
+ * tcap, the KV cache's row capacity, see DESIGN.md §7i) and the column map into ss.  Returns the next n_live, or
+ * SV_ERR_INVALID. */
+SV_API int sv_spec_session_tail_host(const sv_gen_params* p, sv_session_rows* rows, int32_t* out_ids, int32_t out_stride,
+                                     sv_spec_session_state* ss, int32_t accept, int32_t tcap);
+enum {
+  SV_SPEC_SESSION_GREEDY = 0,  /* spec_session_select_fused_kernel: per-column greedy selection, then the tail */
+  SV_SPEC_SESSION_SAMPLE = 1,  /* spec_session_select_sample_kernel (writes sel), then spec_session_tail_kernel with accept */
+  SV_SPEC_SESSION_TAIL = 2     /* spec_session_tail_kernel alone on the given sel, accept as given */
+};
+typedef struct sv_op_spec_session_args {
+  int32_t impl;                 /* SV_SPEC_SESSION_* */
+  int32_t accept;               /* TAIL: 1 accepts ss->sel first, 0 only re-plans (as after an admission) */
+  const void* logits;           /* bf16 [ncols][vocab] (GREEDY, SAMPLE) */
+  int32_t vocab;                /* >= 1 */
+  sv_gen_params params;         /* eos, stop ids, penalty, sampling; do_sample, seed and poll_interval are ignored */
+  void* seen;                   /* uint8 [ncols][vocab]: each slot's generated ids (repetition penalty), updated */
+  int32_t* out_ids;             /* [ncols][out_stride]: each slot's generated ids (the draft history), updated */
+  int32_t* next_ids;            /* [ncols] */
+  int32_t out_stride;
+  int32_t tcap;                 /* >= every live row's row_max_new + its prefix: the KV row capacity the budget uses */
+  sv_session_rows* rows_host;
+  sv_spec_session_state* ss_host;
+  const float* amax_val;        /* GREEDY only: lm_head argmax partials [sv_op_ring_ntiles(vocab)][sv_op_ring_row_stride(ncols)], */
+  const int32_t* amax_idx;      /*   or NULL: the logits rows are scanned (always so when repetition_penalty != 1) */
+  const void *wte, *wpe;        /* bf16 [vocab][h], [n_positions][h]; wpe may be NULL */
+  void* x;                      /* bf16 [ncols][h]: the next step's column inputs */
+  int32_t h, n_positions;       /* h % 8 == 0 */
+} sv_op_spec_session_args;
+SV_API int sv_op_spec_session_select(const sv_op_spec_session_args* args, void* stream);
 /* One beam_candidates_kernel launch over R = batch * num_beams rows: logits bf16 [R][vocab]; cur_len = tokens every
  * running beam holds (0: no repetition penalty yet), running_scores_host float [R], run_seq int32 [R][seq_stride] (device,
  * the beams' generated ids) -> cand_key / cand_val float and cand_tok int32 [R][2 * num_beams] (device).  p is checked as

@@ -168,6 +168,27 @@ class SpecParams(C.Structure):   # sv_spec_params
     _fields_ = [("num_tokens", C.c_int32), ("max_matching_ngram_size", C.c_int32)]
 
 
+class SessionRows(C.Structure):   # sv_session_rows (RowState)
+    _fields_ = [("row_len", C.c_int32 * 16), ("row_step", C.c_int32 * 16), ("row_active", C.c_int32 * 16),
+                ("event", C.c_int32), ("pad_", C.c_int32), ("row_max_new", C.c_int32 * 16), ("row_seed", C.c_uint64 * 16)]
+
+
+class SpecSessionState(C.Structure):   # sv_spec_session_state (svspec::SessionState)
+    _fields_ = [("n_live", C.c_int32)] + [(n, C.c_int32 * 16) for n in ("row", "pos", "tok", "sel", "off")] + [
+        (n, C.c_int32) for n in ("ncols", "k", "max_ngram", "steps", "drafted", "accepted")]
+
+
+SV_SPEC_SESSION_GREEDY, SV_SPEC_SESSION_SAMPLE, SV_SPEC_SESSION_TAIL = 0, 1, 2
+
+
+class OpSpecSession(C.Structure):   # sv_op_spec_session_args
+    _fields_ = [("impl", C.c_int32), ("accept", C.c_int32), ("logits", C.c_void_p), ("vocab", C.c_int32),
+                ("params", GenParams), ("seen", C.c_void_p), ("out_ids", C.c_void_p), ("next_ids", C.c_void_p),
+                ("out_stride", C.c_int32), ("tcap", C.c_int32), ("rows_host", C.POINTER(SessionRows)),
+                ("ss_host", C.POINTER(SpecSessionState)), ("amax_val", C.c_void_p), ("amax_idx", C.c_void_p),
+                ("wte", C.c_void_p), ("wpe", C.c_void_p), ("x", C.c_void_p), ("h", C.c_int32), ("n_positions", C.c_int32)]
+
+
 TOKEN_CALLBACK =C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32)   # sv_token_callback
 
 # name -> (restype, argtypes); must list every SV_API symbol of the header (tests check this)
@@ -211,6 +232,11 @@ SIGNATURES = {
     "sv_session_run": (C.c_int, [_P, _I, _P, _P, _P]),
     "sv_session_read": (C.c_int, [_P, _I, _P, _P]),
     "sv_session_end": (C.c_int, [_P]),
+    "sv_session_begin_speculative": (C.c_int, [_P, C.POINTER(GenParams), C.POINTER(SpecParams), _I]),
+    "sv_session_spec_stats": (C.c_int, [_P, C.POINTER(_I), C.POINTER(_I), C.POINTER(_I)]),
+    "sv_spec_session_plan_host": (C.c_int, [_I, C.POINTER(_I), C.POINTER(_I), _I, C.POINTER(_I), C.POINTER(_I)]),
+    "sv_spec_session_tail_host": (C.c_int, [C.POINTER(GenParams), C.POINTER(SessionRows), C.POINTER(_I), _I,
+                                            C.POINTER(SpecSessionState), _I, _I]),
     "sv_beam_session_begin": (C.c_int, [_P, C.POINTER(BeamParams), _I]),
     "sv_beam_session_admit": (C.c_int, [_P, _P, _I, _P, _I, _P, _P, _P, _P]),
     "sv_launch_count": (C.c_int64, [_P]),
@@ -234,6 +260,7 @@ SIGNATURES = {
     "sv_op_decode_flow": (C.c_int, [C.POINTER(OpFlow), _P]),
     "sv_op_select": (C.c_int, [C.POINTER(OpSelect), _P]),
     "sv_op_spec_select": (C.c_int, [C.POINTER(OpSpec), _P]),
+    "sv_op_spec_session_select": (C.c_int, [C.POINTER(OpSpecSession), _P]),
     "sv_op_beam_candidates": (C.c_int, [_P, _I, C.POINTER(BeamParams), _I, _I, C.POINTER(C.c_float), _P, _I, _P, _P, _P, _P]),
     "sv_op_beam_step": (C.c_int, [C.POINTER(OpBeamStep), _P]),
     "sv_op_beam_kv_copy": (C.c_int, [_P, _P, C.c_int64, _I, _I, _I, _I, C.POINTER(BeamPlan), _P]),

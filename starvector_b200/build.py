@@ -19,8 +19,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libstarvector_b200.so")
-SOURCES = ["sv_kernels_basic.cu", "sv_gemm_rowgroup.cu", "sv_gemm_wgmma.cu", "sv_attention.cu", "sv_decode_fused.cu", "sv_decode_mega.cu", "sv_decode_flow.cu", "sv_beam.cu", "sv_beam_session.cu", "sv_preprocess.cu", "sv_score.cu", "sv_engine.cu"]
-HEADERS = ["sv_common.cuh", "sv_kernels.h", "sv_ring.cuh", "sv_select.cuh", "sv_beam_core.h", "sv_beam_body.cuh", "sv_preprocess_core.h", "sv_spec_core.h", os.path.join("..", "..", "include", "starvector_b200.h")]
+SOURCES = ["sv_kernels_basic.cu", "sv_gemm_rowgroup.cu", "sv_gemm_wgmma.cu", "sv_attention.cu", "sv_decode_fused.cu", "sv_decode_mega.cu", "sv_decode_flow.cu", "sv_beam.cu", "sv_beam_session.cu", "sv_spec_session.cu", "sv_preprocess.cu", "sv_score.cu", "sv_engine.cu"]
+HEADERS = ["sv_common.cuh", "sv_kernels.h", "sv_ring.cuh", "sv_select.cuh", "sv_sample.cuh", "sv_beam_core.h", "sv_beam_body.cuh", "sv_preprocess_core.h", "sv_spec_core.h", os.path.join("..", "..", "include", "starvector_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr", "-Xcompiler", "-ffp-contract=off",

@@ -19,6 +19,16 @@ from typing import Callable, List, Optional, Sequence
 import torch
 
 
+def spec_session_k(params, slots: int, engine) -> int:
+    """Drafts per row a session with these parameters speculates with: `params.prompt_lookup_num_tokens` clamped to
+    `slots - 1` on v1 engines on the fused decode path, 0 (a plain session) without the hint, with one slot, on v2
+    (StarVector-8B) engines or with `SV_DECODE=legacy`.  Inside a session the hint changes the speed only."""
+    k = int(getattr(params, "prompt_lookup_num_tokens", 0) or 0)
+    if k <= 0 or slots < 2 or engine.dims.variant != 0 or not engine.fused_decode:
+        return 0
+    return min(k, slots - 1)
+
+
 class ContinuousScheduler:
     """Runs requests (one image each, `n` completions per image) through a decode session of `slots` cache rows.
 
@@ -26,7 +36,9 @@ class ContinuousScheduler:
     including its EOS / stop sequence, or `max_new_tokens[i]` tokens.  After `run`, `stats` holds the decode steps, the
     number of admissions, the host wall time spent in admission (encode + prefill) and in decoding, and `admit_step`: for
     every completion, the number of decode steps the session had run when it was admitted (while two rows decode side
-    by side, their context lengths differ by the difference of their admit steps)."""
+    by side, their context lengths differ by the difference of their admit steps).  A speculative session
+    (`spec_session_k`) adds `spec`: its verify steps, drafts proposed and drafts accepted; `steps` then counts verify
+    steps."""
 
     def __init__(self, engine, slots: Optional[int] = None, num_beams: int = 1):
         self.engine = engine
@@ -77,6 +89,8 @@ class ContinuousScheduler:
         admit_step = [0] * (N * n)
         steps = admissions = 0
         t_admit = t_decode = 0.0
+        spec = nb == 1 and spec_session_k(params, self.slots, eng) > 0
+        spec_stats = None
         if nb > 1:
             eng.beam_session_begin(params, self.slots)
         else:
@@ -119,8 +133,12 @@ class ContinuousScheduler:
                     if on_finish is not None:
                         on_finish(k, ids)
                 free.sort()
+            if spec:
+                spec_stats = eng.session_spec_stats()
         finally:
             eng.session_end()
         self.stats = {"steps": steps, "admissions": admissions, "admit_s": t_admit, "decode_s": t_decode,
                       "admit_step": admit_step}
+        if spec_stats is not None:
+            self.stats["spec"] = spec_stats
         return results

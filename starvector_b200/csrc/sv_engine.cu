@@ -48,7 +48,7 @@ struct DecLayer { bf16 *ln1_w, *ln1_b, *attn_w, *attn_b, *proj_w, *proj_b, *ln2_
 // The decode-step graphs of generate, speculative generate, beam search and sessions share one cache.  Two captures that
 // enqueue different kernels or arguments must never share a key: `rows` is the batch, the verify step's columns or the
 // session's slots, `parts` the attention partition (decode_parts).
-enum class StepKind { generate, speculative, beam, session, beam_session };
+enum class StepKind { generate, speculative, beam, session, beam_session, spec_session };
 struct StepKey {
   StepKind kind;
   int rows, parts;
@@ -163,6 +163,9 @@ struct sv_engine {
   sv_beam_params sess_bp{};
   bf16* bsess_px = nullptr;                  // staging: one admitted image repeated num_beams times
   int32_t* bsess_ids = nullptr;              //   and its prompt
+  // speculative session (sv_session_begin_speculative, DESIGN.md §7i): the verify step's columns belong to the live rows
+  bool sess_spec = false;
+  svspec::SessionState* spec_sess = nullptr; // device, allocated by the first speculative session
 
   // prompt-lookup speculative decoding (sv_generate_speculative): device state allocated by the first call
   svspec::State* spec = nullptr;
@@ -1390,7 +1393,8 @@ int sv_generate_stream(sv_engine* e, const sv_gen_params* p, int32_t* out_ids, i
 int sv_generate_speculative(sv_engine* e, const sv_gen_params* p, const sv_spec_params* sp, int32_t* out_ids,
                             int32_t* out_len, sv_token_callback on_tokens, void* user, void* stream) {
   if (!e || !sp) return fail(e, SV_ERR_INVALID, "null argument");
-  if (e->session) return fail(e, SV_ERR_UNSUPPORTED, "sv_generate_speculative: a decode session is open (speculation inside sessions is not built)");
+  if (e->session) return fail(e, SV_ERR_UNSUPPORTED, "sv_generate_speculative: a decode session is open (a session speculates when "
+                                                     "opened with sv_session_begin_speculative)");
   return generate_impl(e, p, out_ids, out_len, stream, on_tokens, user, sp);
 }
 
@@ -1792,6 +1796,11 @@ int sv_session_admit(sv_engine* e, const void* pixels, int32_t k, const int32_t*
   // token 0 of the admitted slots from their prefill logits (generate_impl's first select, no position advance)
   launch_token_select(e, e->sess_logits, S, e->sess_p.do_sample, /*partials=*/false, /*advance_len=*/0, /*pdl=*/false, st,
                       e->rows, mask);
+  // speculative session: nothing to accept; the next drafts, allocation and map over every live row, and every column's
+  // embedding (the select above embedded the admitted rows at their slot index, which is not the column layout)
+  if (e->sess_spec)
+    launch_spec_session_tail(false, e->rows, e->params, e->seen, e->next_ids, e->out_ids, d.vocab, e->wte, e->wpe, e->d_x,
+                             d.hidden, d.n_positions, e->tcap, e->spec_sess, false, st);
   SV_CK(e, cudaGetLastError());
   SV_CK(e, cudaStreamSynchronize(st));     // the caller may release pixels / prompt_ids on return
   for (int j = 0; j < k; ++j) e->sess_live[slots_host[j]] = 1;
@@ -1823,9 +1832,24 @@ int sv_session_run(sv_engine* e, int32_t max_steps, int32_t* finished_host, int3
     const int total = e->Q + e->sess_prompt_len + cap;     // the session cap fixes the split count
     const int parts = decode_parts(fused, total);
     // (beam sessions: beam-sample and the beam width are read from the device parameters, as in sv_beam_search)
-    GraphEntry& ge = e->step_graphs[{beam ? StepKind::beam_session : StepKind::session, S, parts, sample, fused, e->use_pdl}];
+    const bool spec = e->sess_spec;
+    const StepKind kind = beam ? StepKind::beam_session : spec ? StepKind::spec_session : StepKind::session;
+    GraphEntry& ge = e->step_graphs[{kind, S, parts, sample, fused, e->use_pdl}];
     const sv_model_desc& d = e->d;
     auto step = [&](bool pdl) {
+      if (spec) {              // verify step over the S columns of the map; the previous tail embedded their inputs
+        run_engine_step(e, nullptr, S, parts, pdl, st, nullptr, &e->spec_sess->map);
+        if (sample) {
+          launch_spec_session_select_sample(e->logits, d.vocab, S, e->rows, e->params, e->seen, e->logits_f32, e->spec_sess, st);
+          launch_spec_session_tail(true, e->rows, e->params, e->seen, e->next_ids, e->out_ids, d.vocab, e->wte, e->wpe, e->d_x,
+                                   d.hidden, d.n_positions, e->tcap, e->spec_sess, false, st);
+        } else {
+          launch_spec_session_select_fused(e->logits, d.vocab, e->amax_val, e->amax_idx, gemv_ring_ntiles(d.vocab),
+                                           8 * ring_row_groups(S), e->rows, e->params, e->seen, e->next_ids, e->out_ids,
+                                           e->wte, e->wpe, e->d_x, d.hidden, d.n_positions, e->tcap, e->spec_sess, pdl, st);
+        }
+        return;
+      }
       if (beam) {              // the decode step, then every live group's bookkeeping, as sv_beam_search runs it
         run_engine_step(e, fused ? nullptr : e->next_ids, S, parts, pdl, st, e->rows);
         launch_beam_session_candidates(e->logits, d.vocab, S, e->beam_params, e->beam_state, e->beam_run_seq, e->beam_key,
@@ -1899,10 +1923,92 @@ int sv_session_end(sv_engine* e) {
   SV_CK(e, cudaStreamSynchronize(e->gen_stream));
   e->session = false;
   e->sess_beam = false;
+  e->sess_spec = false;
   e->sess_slots = 0;
   e->sess_live.clear();
   e->sess_len.clear();
   return SV_OK;
+}
+
+// ---- speculative sessions (DESIGN.md §7i) ---------------------------------------------------------------------------
+int sv_session_begin_speculative(sv_engine* e, const sv_gen_params* p, const sv_spec_params* sp, int32_t slots) {
+  if (!e || !p || !sp) return fail(e, SV_ERR_INVALID, "null argument");
+  if (e->session) return fail(e, SV_ERR_STATE, "a decode session is already open");
+  if (e->v2) return fail(e, SV_ERR_UNSUPPORTED, "sv_session_begin_speculative: v2 engines decode through the per-op kernels; only v1 is built");
+  if (!e->fused_decode) return fail(e, SV_ERR_UNSUPPORTED, "sv_session_begin_speculative needs the fused graph decode path (SV_DECODE=legacy is set)");
+  if (slots < 2 || slots > std::min(e->d.max_batch, svspec::kMaxCols))
+    return fail(e, SV_ERR_INVALID, "slots %d outside [2,%d] (a speculative session drafts into the columns of idle slots)", slots,
+                std::min(e->d.max_batch, svspec::kMaxCols));
+  if (sp->num_tokens < 1 || sp->num_tokens > slots - 1)
+    return fail(e, SV_ERR_INVALID, "prompt_lookup_num_tokens %d outside [1, %d] (slots - 1)", sp->num_tokens, slots - 1);
+  if (sp->max_matching_ngram_size < 1)
+    return fail(e, SV_ERR_INVALID, "max_matching_ngram_size must be >= 1, got %d", sp->max_matching_ngram_size);
+  SV_CK(e, cudaSetDevice(e->device));
+  if (!e->spec_sess && dev_alloc(e, &e->spec_sess, 1) != cudaSuccess)
+    return fail(e, SV_ERR_CUDA, "allocation of the speculative session state failed: %s", cudaGetErrorString(cudaGetLastError()));
+  SV_TRY(sv_session_begin(e, p, slots));
+  svspec::SessionState hs;
+  memset(&hs, 0, sizeof(hs));          // n_live = 0: no column is live before the first admission
+  hs.ncols = slots; hs.k = sp->num_tokens; hs.max_ngram = sp->max_matching_ngram_size;
+  const cudaError_t r = cudaMemcpy(e->spec_sess, &hs, sizeof(hs), cudaMemcpyHostToDevice);
+  if (r != cudaSuccess) {
+    sv_session_end(e);
+    return fail(e, SV_ERR_CUDA, "upload of the speculative session state failed: %s", cudaGetErrorString(r));
+  }
+  e->sess_spec = true;
+  return SV_OK;
+}
+
+int sv_session_spec_stats(sv_engine* e, int32_t* steps, int32_t* drafted, int32_t* accepted) {
+  if (!e) return SV_ERR_INVALID;
+  if (!e->session || !e->sess_spec) return fail(e, SV_ERR_STATE, "sv_session_spec_stats needs an open speculative session");
+  SV_CK(e, cudaSetDevice(e->device));
+  SV_CK(e, cudaStreamSynchronize(e->gen_stream));
+  int32_t v[3];
+  SV_CK(e, cudaMemcpy(v, &e->spec_sess->steps, sizeof(v), cudaMemcpyDeviceToHost));
+  if (steps) *steps = v[0];
+  if (drafted) *drafted = v[1];
+  if (accepted) *accepted = v[2];
+  return SV_OK;
+}
+
+int sv_spec_session_plan_host(int32_t S, const int32_t* active, const int32_t* want, int32_t budget, int32_t* g,
+                              int32_t* first) {
+  if (S < 1 || S > svspec::kMaxCols || !active || !want || !g || !first) return SV_ERR_INVALID;
+  return svspec::plan_session(S, active, want, budget, g, first);
+}
+
+// sv_spec_session_state mirrors svspec::SessionState and sv_session_rows RowState, field for field.
+static_assert(sizeof(sv_spec_session_state) == sizeof(svspec::SessionState) &&
+              offsetof(sv_spec_session_state, off) == offsetof(svspec::SessionState, off) &&
+              offsetof(sv_spec_session_state, accepted) == offsetof(svspec::SessionState, accepted),
+              "sv_spec_session_state mirrors svspec::SessionState");
+static_assert(sizeof(sv_session_rows) == sizeof(RowState) && offsetof(sv_session_rows, event) == offsetof(RowState, event) &&
+              offsetof(sv_session_rows, row_seed) == offsetof(RowState, row_seed), "sv_session_rows mirrors RowState");
+
+int sv_spec_session_tail_host(const sv_gen_params* p, sv_session_rows* rows, int32_t* out_ids, int32_t out_stride,
+                              sv_spec_session_state* ss, int32_t accept, int32_t tcap) {
+  if (!p || !rows || !out_ids || !ss) return SV_ERR_INVALID;
+  const int S = ss->ncols;
+  if (S < 1 || S > svspec::kMaxCols || ss->n_live < 0 || ss->n_live > S || ss->k < 0 || ss->max_ngram < 1) return SV_ERR_INVALID;
+  if (p->n_stop_ids < 0 || p->n_stop_ids > 8 || out_stride < 1) return SV_ERR_INVALID;
+  for (int r = 0; r < S; ++r)
+    if (rows->row_active[r] && (rows->row_step[r] < 1 || rows->row_step[r] >= rows->row_max_new[r] || rows->row_max_new[r] > out_stride))
+      return SV_ERR_INVALID;
+  svspec::SessionState* s = reinterpret_cast<svspec::SessionState*>(ss);
+  RowState* rs = reinterpret_cast<RowState*>(rows);
+  const GenParamsDev hp = gen_params_dev(p, 0, out_stride);
+  int32_t next[svspec::kMaxCols];
+  if (accept) spec_session_accept(s, s->sel, rs, &hp, nullptr, /*vocab=*/0, next, out_ids);
+  int32_t w[svspec::kMaxCols] = {0}, dr[svspec::kMaxCols][svspec::kMaxCols];
+  int live = 0;
+  for (int r = 0; r < S; ++r) live += rs->row_active[r] != 0;
+  if (spec_session_budget(rs, S, tcap) > live)
+    for (int r = 0; r < S; ++r)
+      if (rs->row_active[r])
+        w[r] = svspec::draft_host(out_ids + (int64_t)r * out_stride, rs->row_step[r], s->k, s->max_ngram, hp.eos_id,
+                                  rs->row_max_new[r] - rs->row_step[r] - 1, dr[r]);
+  return spec_session_plan(s, rs, out_ids, out_stride, w, dr, tcap);
 }
 
 // ---- beam sessions (DESIGN.md §7h) ----------------------------------------------------------------------------------
@@ -2953,6 +3059,79 @@ int sv_op_spec_select(const sv_op_spec_args* args, void* stream) {
   if (r != cudaSuccess) return op_fail("spec_select", r);
   o.gen_host[0] = gs.step; o.gen_host[1] = gs.cur_len; o.gen_host[2] = gs.done; o.gen_host[3] = gs.unfinished[0];
   memcpy(o.spec_host, &sp, sizeof(sp));
+  return SV_OK;
+}
+
+// The kernels of a speculative session's verify step, launched as sv_session_run / sv_session_admit launch them.
+int sv_op_spec_session_select(const sv_op_spec_session_args* args, void* stream) {
+  if (!args) return fail(nullptr, SV_ERR_INVALID, "bad spec_session_select arguments: null descriptor");
+  const sv_op_spec_session_args& o = *args;
+  const sv_gen_params& p = o.params;
+  const char* bad = nullptr;
+  if (o.impl != SV_SPEC_SESSION_GREEDY && o.impl != SV_SPEC_SESSION_SAMPLE && o.impl != SV_SPEC_SESSION_TAIL) bad = "unknown impl";
+  else if (!o.seen || !o.out_ids || !o.next_ids || !o.rows_host || !o.ss_host) bad = "seen, out_ids, next_ids, rows_host and ss_host are required";
+  else if (o.impl != SV_SPEC_SESSION_TAIL && !o.logits) bad = "GREEDY and SAMPLE need logits";
+  else if (o.vocab < 1) bad = "vocab < 1";
+  else if (o.impl == SV_SPEC_SESSION_SAMPLE && !(p.temperature > 0.f)) bad = "temperature must be > 0";
+  else if (o.impl == SV_SPEC_SESSION_SAMPLE && !(p.top_p > 0.f && p.top_p <= 1.f)) bad = "top_p not in (0, 1]";
+  else if ((bad = gen_params_error(p))) {}
+  else if (!o.wte || !o.x) bad = "wte and x are required";
+  else if (o.h < 8 || o.h % 8) bad = "h % 8 != 0";
+  else if (o.n_positions < 1) bad = "n_positions < 1";
+  else if (!aligned16(o.wte) || !aligned16(o.wpe) || !aligned16(o.x)) bad = "wte, wpe and x must be 16-byte aligned";
+  else if ((o.amax_val != nullptr) != (o.amax_idx != nullptr)) bad = "amax_val and amax_idx go together";
+  else if (o.amax_val && o.impl != SV_SPEC_SESSION_GREEDY) bad = "the argmax partials are GREEDY's";
+  if (!bad) {
+    const sv_spec_session_state& q = *o.ss_host;
+    const sv_session_rows& rw = *o.rows_host;
+    const int S = q.ncols;
+    if (S < 2 || S > svspec::kMaxCols) bad = "ncols not in [2, 16]";
+    else if (q.n_live < 0 || q.n_live > S) bad = "n_live not in [0, ncols]";
+    else if (q.k < 1 || q.k > S - 1 || q.max_ngram < 1) bad = "k not in [1, ncols - 1] or max_ngram < 1";
+    for (int c = 0; !bad && c < S; ++c)
+      if (q.row[c] < 0 || q.row[c] >= S || q.pos[c] < 0 || q.pos[c] >= std::min(o.n_positions, o.tcap) || q.off[c] < 0 || q.off[c] > c)
+        bad = "a column's row, position or offset is out of range";
+    for (int r = 0; !bad && r < S; ++r)
+      if (rw.row_active[r] && (rw.row_step[r] < 1 || rw.row_step[r] >= rw.row_max_new[r] || rw.row_max_new[r] > o.out_stride ||
+                               rw.row_len[r] < 0 || rw.row_len[r] + rw.row_max_new[r] > o.tcap || rw.row_len[r] + rw.row_max_new[r] > o.n_positions))
+        bad = "a live row's step, cap or position is out of range (1 <= row_step < row_max_new <= out_stride, row_len + row_max_new <= min(tcap, n_positions))";
+  }
+  if (bad) return fail(nullptr, SV_ERR_INVALID, "bad spec_session_select arguments: %s", bad);
+  cudaStream_t st = (cudaStream_t)stream;
+  const GenParamsDev hp = gen_params_dev(&p, 0, o.out_stride);
+  const int S = o.ss_host->ncols;
+  const size_t probs_bytes = o.impl == SV_SPEC_SESSION_SAMPLE ? (size_t)S * o.vocab * sizeof(float) : 0;
+  char* buf = nullptr;
+  cudaError_t r = cudaMalloc(reinterpret_cast<void**>(&buf), 3 * kOpState + probs_bytes);
+  if (r != cudaSuccess) return op_fail("spec_session_select alloc", r);
+  static_assert(sizeof(svspec::SessionState) <= kOpState && sizeof(RowState) <= kOpState, "the session states fit scratch slots");
+  RowState* d_rows = reinterpret_cast<RowState*>(buf);
+  svspec::SessionState* d_ss = reinterpret_cast<svspec::SessionState*>(buf + kOpState);
+  GenParamsDev* d_p = reinterpret_cast<GenParamsDev*>(buf + 2 * kOpState);
+  float* probs = reinterpret_cast<float*>(buf + 3 * kOpState);
+  r = cudaMemcpyAsync(d_rows, o.rows_host, sizeof(RowState), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_ss, o.ss_host, sizeof(svspec::SessionState), cudaMemcpyHostToDevice, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(d_p, &hp, sizeof(hp), cudaMemcpyHostToDevice, st);
+  const bf16* lg = (const bf16*)o.logits;
+  uint8_t* seen = (uint8_t*)o.seen;
+  if (r == cudaSuccess) {
+    if (o.impl == SV_SPEC_SESSION_GREEDY) {
+      launch_spec_session_select_fused(lg, o.vocab, o.amax_val, o.amax_idx, gemv_ring_ntiles(o.vocab), 8 * ring_row_groups(S), d_rows,
+                                       d_p, seen, o.next_ids, o.out_ids, (const bf16*)o.wte, (const bf16*)o.wpe, (bf16*)o.x, o.h,
+                                       o.n_positions, o.tcap, d_ss, false, st);
+    } else {
+      if (o.impl == SV_SPEC_SESSION_SAMPLE) launch_spec_session_select_sample(lg, o.vocab, S, d_rows, d_p, seen, probs, d_ss, st);
+      launch_spec_session_tail(o.impl == SV_SPEC_SESSION_SAMPLE || o.accept != 0, d_rows, d_p, seen, o.next_ids, o.out_ids,
+                               o.vocab, (const bf16*)o.wte, (const bf16*)o.wpe, (bf16*)o.x, o.h, o.n_positions, o.tcap, d_ss,
+                               false, st);
+    }
+    r = cudaGetLastError();
+  }
+  if (r == cudaSuccess) r = cudaMemcpyAsync(o.rows_host, d_rows, sizeof(RowState), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaMemcpyAsync(o.ss_host, d_ss, sizeof(svspec::SessionState), cudaMemcpyDeviceToHost, st);
+  if (r == cudaSuccess) r = cudaStreamSynchronize(st);
+  cudaFree(buf);
+  if (r != cudaSuccess) return op_fail("spec_session_select", r);
   return SV_OK;
 }
 

@@ -180,6 +180,20 @@ void launch_spec_accept(GenState* state, const GenParamsDev* params, uint8_t* se
 void launch_select_sample_spec(const bf16* logits, int vocab, int ncols, GenState* state, const GenParamsDev* params,
                                uint8_t* seen, float* probs, svspec::State* sp, cudaStream_t st);
 
+// ---- sv_spec_session.cu : the verify step of a speculative session (S = ss->ncols columns; sv_spec_core.h, sv_select.cuh).
+// Greedy: per-column selection as launch_select_fused_spec, then every live row's accept walk, the next drafts, the column
+// allocation and map, and the columns' embeddings.  Sampled: launch_spec_session_select_sample (tokens to ss->sel), then
+// launch_spec_session_tail with accept; the tail without accept re-plans after an admission.
+void launch_spec_session_select_fused(const bf16* logits, int vocab, const float* amax_val, const int* amax_idx, int ntiles,
+                                      int amax_stride, RowState* rows, const GenParamsDev* params, uint8_t* seen,
+                                      int32_t* next_ids, int32_t* out_ids, const bf16* wte, const bf16* wpe, bf16* x, int h,
+                                      int n_positions, int tcap, svspec::SessionState* ss, bool pdl, cudaStream_t st);
+void launch_spec_session_select_sample(const bf16* logits, int vocab, int ncols, RowState* rows, const GenParamsDev* params,
+                                       uint8_t* seen, float* probs, svspec::SessionState* ss, cudaStream_t st);
+void launch_spec_session_tail(bool accept, RowState* rows, const GenParamsDev* params, uint8_t* seen, int32_t* next_ids,
+                              int32_t* out_ids, int vocab, const bf16* wte, const bf16* wpe, bf16* x, int h, int n_positions,
+                              int tcap, svspec::SessionState* ss, bool pdl, cudaStream_t st);
+
 // ---- sv_decode_mega.cu : per-phase weight-ring decode GEMV; layer descriptor shared with sv_decode_flow.cu
 struct MegaLayer {
   const bf16 *ln1_w, *ln1_b, *attn_w, *attn_b, *proj_w, *proj_b, *ln2_w, *ln2_b, *fc_w, *fc_b, *fc2_w, *fc2_b;

@@ -1,6 +1,7 @@
-// Prompt-lookup speculative decoding (sv_generate_speculative): the column map of a verify step, the draft rule and the
-// accept walk, shared by the device kernels (spec_tail in sv_decode_fused.cu) and their host replays (sv_spec_draft_host, sv_spec_accept_host,
-// tests/test_speculative_logic.py).
+// Prompt-lookup speculative decoding (sv_generate_speculative, and inside sessions sv_session_begin_speculative): the column
+// map of a verify step, the draft rule, the accept walk and the session's column allocation, shared by the device kernels
+// (spec_tail in sv_decode_fused.cu, sv_spec_session.cu) and their host replays (sv_spec_draft_host, sv_spec_accept_host,
+// sv_spec_session_plan_host, tests/test_speculative_logic.py, tests/test_spec_session_logic.py).
 //
 // A verify step feeds the last emitted token and up to k drafted tokens as k + 1 columns of ONE cache row, column c at
 // position cur_len + c.  Every column of the weight-ring GEMVs is an independent dot product and every per-row reduction
@@ -91,6 +92,41 @@ SVS_HD int accept(const int32_t* sel, const int32_t* tok, int n_live, Emit&& emi
     if (emit(sel[c]) || c + 1 >= n_live || sel[c] != tok[c + 1]) break;
   }
   return m;
+}
+
+// ---- speculation inside a continuous-batching session (sv_session_begin_speculative, DESIGN.md §7i) ----------------
+// A verify step of a session of S slots has S columns.  Live row r gets 1 + g_r contiguous columns, the rows in slot order:
+// its first column feeds its last emitted token at row_len[r], column j of the row its draft j at row_len[r] + j.  Each
+// column selects with the plain session's rule for that token (sv_spec_session.cu), so the drafts change the speed only.
+struct SessionState {
+  ColMap map;                      // first, so that &ss->map is the step's column map
+  int32_t tok[kMaxCols];           // column inputs
+  int32_t sel[kMaxCols];           // token selected at each live column (sampled path: written by the select kernel)
+  int32_t off[kMaxCols];           // column's offset within its row: 0 at the row's first column, j at its draft j
+  int32_t ncols;                   // columns of the captured step (the session's slots)
+  int32_t k, max_ngram;            // prompt_lookup_num_tokens, max_matching_ngram_size
+  int32_t steps, drafted, accepted;   // verify steps run, drafts proposed, drafts accepted
+};
+
+// The column allocation: every live row (active[r] != 0) gets its own first column; the spare columns (at most `budget`
+// columns in all, and at most S) are handed out round-robin in slot order, one draft per pass to each live row still below
+// its want w[r], until none are left or no row wants more.  Writes g[r] (drafts granted, 0 for idle rows) and first[r] (the
+// row's first column, -1 for idle rows); returns n_live, the sum of 1 + g[r] over the live rows.
+SVS_HD int plan_session(int S, const int32_t* active, const int32_t* w, int budget, int32_t* g, int32_t* first) {
+  int live = 0;
+  for (int r = 0; r < S; ++r) { g[r] = 0; live += active[r] != 0; }
+  int spare = (budget < S ? budget : S) - live;
+  for (bool more = true; spare > 0 && more;) {
+    more = false;
+    for (int r = 0; r < S && spare > 0; ++r)
+      if (active[r] && g[r] < w[r]) { ++g[r]; --spare; more = true; }
+  }
+  int c = 0;
+  for (int r = 0; r < S; ++r) {
+    first[r] = active[r] ? c : -1;
+    if (active[r]) c += 1 + g[r];
+  }
+  return c;
 }
 
 // The column map after an accept: live columns at cur_len + c; inert ones at the last live position (after the finish,

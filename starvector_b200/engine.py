@@ -376,18 +376,46 @@ class Engine:
         refilled with the next queued image whenever a row finishes (`ContinuousScheduler`).  Completion j of image i
         (index i * n + j of the returned list, int32 on the CPU) holds exactly the tokens a one-image `generate` of image i
         with `params` (seed `seeds[i * n + j]`, default `params.seed + i * n + j`, and `max_new_tokens[i]` new tokens at most)
-        returns.  `params.max_new_tokens` is the session cap; `on_finish(index, ids)` streams results as they complete."""
+        returns.  `params.max_new_tokens` is the session cap; `on_finish(index, ids)` streams results as they complete.
+        `params.prompt_lookup_num_tokens > 0` asks for a speculative session (see `session_begin`): same tokens."""
         from .continuous import ContinuousScheduler
 
         return ContinuousScheduler(self, slots).run(pixels, prompt_ids, params, max_new_tokens=max_new_tokens, seeds=seeds,
                                                     n=n, on_finish=on_finish)
 
+    @property
+    def fused_decode(self) -> bool:
+        """The engine decodes through the fused graph path (not `SV_DECODE=legacy`)."""
+        return "decode=legacy-kernels" not in self.describe()
+
     def session_begin(self, params: GenerationParams, slots: int) -> None:
+        """Open a decode session of `slots` cache rows.  `params.prompt_lookup_num_tokens` / `max_matching_ngram_size` are a
+        speed hint: on v1 engines on the fused decode path with `slots >= 2`, the session drafts up to that many tokens
+        (clamped to `slots - 1`) per row into the columns idle slots leave (`sv_session_begin_speculative`); otherwise it
+        runs plain.  Either way every request gets the same tokens."""
+        from .continuous import spec_session_k
+
         cp = params.to_c()
+        k = spec_session_k(params, slots, self)
         with self._lock:
-            self._ck(self._lib.sv_session_begin(self._h, C.byref(cp), int(slots)))
+            if k > 0:
+                sp = _lib.SpecParams(k, int(params.max_matching_ngram_size))
+                self._ck(self._lib.sv_session_begin_speculative(self._h, C.byref(cp), C.byref(sp), int(slots)))
+            else:
+                self._ck(self._lib.sv_session_begin(self._h, C.byref(cp), int(slots)))
             self._session_slots = int(slots)
+            self._session_spec = k > 0
             self._batch = 0
+
+    def session_spec_stats(self) -> Optional[Dict[str, int]]:
+        """Counters of the open speculative session (`sv_session_spec_stats`): verify steps, drafts proposed, drafts
+        accepted; None when the open session is a plain one."""
+        if not getattr(self, "_session_spec", False):
+            return None
+        v = [C.c_int32() for _ in range(3)]
+        with self._lock:
+            self._ck(self._lib.sv_session_spec_stats(self._h, *(C.byref(x) for x in v)))
+        return {"steps": v[0].value, "drafted": v[1].value, "accepted": v[2].value}
 
     def session_admit(self, pixels: torch.Tensor, prompt_ids: torch.Tensor, slots: Sequence[int], *,
                       max_new_tokens: Optional[Sequence[int]] = None, seeds: Optional[Sequence[int]] = None,
@@ -456,6 +484,7 @@ class Engine:
         with self._lock:
             self._ck(self._lib.sv_beam_session_begin(self._h, C.byref(bp), int(slots)))
             self._session_slots = int(slots)
+            self._session_spec = False
             self._batch = 0
 
     def beam_session_admit(self, pixels: torch.Tensor, prompt_ids: torch.Tensor, groups: Sequence[int], *,
@@ -480,6 +509,7 @@ class Engine:
     def session_end(self) -> None:
         with self._lock:
             self._ck(self._lib.sv_session_end(self._h))
+            self._session_spec = False
 
     # -- introspection -------------------------------------------------------------------
     def launch_count(self) -> int:
@@ -790,6 +820,28 @@ def op_spec_select(impl: int, params: GenerationParams, seen: torch.Tensor, out_
     _lib.check(lib, lib.sv_op_spec_select(C.byref(a), _stream_ptr(seen.device)))
     state["step"], state["cur_len"], state["done"], state["unfinished"] = (int(v) for v in gen)
     return state
+
+
+def op_spec_session_select(impl: int, params: GenerationParams, seen: torch.Tensor, out_ids: torch.Tensor,
+                           next_ids: torch.Tensor, rows: "_lib.SessionRows", ss: "_lib.SpecSessionState", wte: torch.Tensor,
+                           wpe: Optional[torch.Tensor], x: torch.Tensor, n_positions: int, tcap: int,
+                           logits: Optional[torch.Tensor] = None, amax: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                           accept: bool = True) -> None:
+    """One speculative-session kernel launch (see sv_op_spec_session_select) over S = ss.ncols slots: bf16 `logits [S,
+    vocab]` (GREEDY, SAMPLE); `seen` uint8 `[S, vocab]`, `out_ids` int32 `[S, out_stride]`, `next_ids` int32 `[S]` and
+    `x [S, h]` are updated in place, as are `rows` (a `_lib.SessionRows`) and `ss` (a `_lib.SpecSessionState`)."""
+    lib = _lib.load()
+    a = _lib.OpSpecSession(impl=impl, accept=int(bool(accept)), vocab=wte.shape[0], params=params.to_c(), seen=seen.data_ptr(),
+                           out_ids=out_ids.data_ptr(), next_ids=next_ids.data_ptr(), out_stride=out_ids.shape[-1], tcap=tcap,
+                           rows_host=C.pointer(rows), ss_host=C.pointer(ss), wte=wte.data_ptr(), x=x.data_ptr(),
+                           h=wte.shape[1], n_positions=n_positions)
+    if logits is not None:
+        a.logits = logits.data_ptr()
+    if wpe is not None:
+        a.wpe = wpe.data_ptr()
+    if amax is not None:
+        a.amax_val, a.amax_idx = amax[0].data_ptr(), amax[1].data_ptr()
+    _lib.check(lib, lib.sv_op_spec_session_select(C.byref(a), _stream_ptr(seen.device)))
 
 
 def op_beam_candidates(logits: torch.Tensor, bp: "_lib.BeamParams", batch: int, cur_len: int, running_scores,

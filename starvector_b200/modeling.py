@@ -322,7 +322,9 @@ class StarVectorStarCoder:
         """`generate_im2svg` over any number of images with continuous batching (`Engine.generate_requests`): the engine's
         `max_batch` cache rows are refilled with the next image as soon as a row finishes, instead of running groups of
         `max_batch` that each last as long as their longest member.  Takes the kwargs of `generate_im2svg` (max_length,
-        use_nucleus_sampling, temperature, top_p, repetition_penalty, prompt, seed, num_return_sequences).  Every image's
+        use_nucleus_sampling, temperature, top_p, repetition_penalty, prompt, seed, num_return_sequences) and HF's
+        prompt_lookup_num_tokens / max_matching_ngram_size (a speculative session where the engine runs one, see
+        `Engine.session_begin`; the strings do not change).  Every image's
         completion is what `generate_im2svg({"image": image[k:k+1]}, num_beams=1, seed=seed + k, ...)` returns (the
         `</svg>` stop and EOS end each row on its own); completion j of image i (num_return_sequences = G) is request
         k = i * G + j.  Returns prompt + completion strings in that order."""
@@ -337,6 +339,9 @@ class StarVectorStarCoder:
             raise ValueError("num_return_sequences must be >= 1")
         prompt_ids = self._tokenize_prompt(kwargs.get("prompt"), 1)
         params = self._gen_params(kwargs, prefix_len=self.query_length + prompt_ids.shape[1])
+        # prompt-lookup drafts: a speed hint for the session (Engine.session_begin), the strings are the same
+        params.prompt_lookup_num_tokens = int(kwargs.get("prompt_lookup_num_tokens") or 0)
+        params.max_matching_ngram_size = int(kwargs.get("max_matching_ngram_size") or 2)
         outs = self.engine.generate_requests(image, prompt_ids[0], params, n=G)
         tok = self.svg_transformer.tokenizer
         p0 = prompt_ids[0].cpu().long()
